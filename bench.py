@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - LiDAR frames/sec of the SST hot path (BASELINE.json metric) on N B200s of one node.
+"""bench.py - LiDAR frames/sec of the SST hot path (BASELINE.json metric) on N H100s of one node.
 
 A "step" = one forward of BASELINE config 2 per GPU: 1 synthetic Waymo-shaped sweep (150k pts, 0.32 m pillars,
 ~30k non-empty) through dynamic voxelisation -> DynamicVFE -> SSTInputLayerV2 -> SSTv2 (6 blocks = 12 SRA
@@ -7,6 +7,7 @@ layers, d=128, h=8, ff=256), sparse output (to_bev=False, no attached convs).  F
 (weak scaling, no data-path collective: inference has none, SURVEY.md 8e).
 
     python bench.py --gpus 1 --steps 20 --warmup 5
+    python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs DIR   # + the last timed step's outputs as DIR/*.npy
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference          # CPU port of the reference path on the host cores
 """
@@ -29,23 +30,13 @@ METRIC = "lidar_frames_per_sec_sst6_fwd_150k"
 WORKLOAD = "config2: SST-6 fwd, 150k-pt Waymo-shaped sweep, 0.32m pillars, d=128 h=8 ff=256, batch 1 per GPU, sparse output"
 
 
-def ncu_layer_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the two kernels of one SRA layer, from the committed
-    `ncu --set full` capture of the SHIPPED build (profiles/r02_ncu_layer.json, written by tools/ncu_summary.py)."""
-    p = os.path.join(ROOT, "profiles", "r02_ncu_layer.json")
-    if not os.path.exists(p):
-        return None, "no committed ncu capture of this build"
-    d = json.load(open(p))
-    return int(d["dram_bytes_per_layer"]), "profiles/r02_ncu_layer.json (ncu --set full --cache-control all: cold-L2 replay, an upper bound; " \
-                                           "in the pipeline activations stay L2-resident between launches)"
-
-
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W card; a card set to a lower power limit sustains less): 3.35 TB/s, 989 TFLOP/s dense fp16/bf16
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -280,6 +271,19 @@ def train_bench(args, world, rank, dev, frames_d):
             "loss": float(loss), "optimizer": "AdamW (fused kernel over one flat buffer)", "scaling": "weak"}
 
 
+def dump_outputs(out_dir, result):
+    """The arrays a caller of SSTEngine.run() receives from the last timed step: the voxel count, the [M, d] voxel features and
+    the [M, 4] (batch, z, y, x) coordinates of its M voxels (float64 / float32; < 64 MB for a 150k-point sweep)."""
+    import numpy as np
+    feats, coors, num = result
+    torch.cuda.synchronize()
+    M = int(num.item())
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "num_voxels.npy"), np.array([M], dtype=np.float64))
+    np.save(os.path.join(out_dir, "voxel_feats.npy"), feats[:M].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "voxel_coors.npy"), coors[:M].cpu().numpy().astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -294,6 +298,8 @@ def main():
     ap.add_argument("--train-frames", type=int, default=4, help="frames per GPU and training step (config 4: 32 frames / 8 GPUs)")
     ap.add_argument("--streams", type=int, default=int(os.environ.get("SSTB200_STREAMS", "8")),
                     help="frames in flight per GPU (independent engines on their own CUDA streams); 1 = strictly serial")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (voxel features, coordinates, count) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -361,27 +367,24 @@ def main():
     barrier()
     sampler.begin()
     main = torch.cuda.current_stream(dev)
-    REPS = int(os.environ.get("SSTB200_BENCH_REPS", "30"))   # the K-step window is repeated and the MEDIAN window reported
-    windows = []
-    ncu_range = os.environ.get("SSTB200_NCU_RANGE") == "1"   # `ncu --profile-from-start off`: profile the first timed window only
-    for rep in range(REPS):
-        if ncu_range and rep == 0:
-            torch.cuda.profiler.start()
-        if ncu_range and rep == 1:
-            torch.cuda.synchronize()
-            torch.cuda.profiler.stop()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(main)
-        for e in engs:
-            e.stream.wait_event(e0)
-        for i in range(args.steps):
-            step(rep * args.steps + i)
-        for e in engs:
-            main.wait_stream(e.stream)
-        e1.record(main)
-        windows.append((e0, e1))
+    windows = []   # one timed window of exactly --steps steps
+    last = None
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(main)
+    for e in engs:
+        e.stream.wait_event(e0)
+    for i in range(args.steps):
+        last = step(i)
+    for e in engs:
+        main.wait_stream(e.stream)
+    e1.record(main)
+    windows.append((e0, e1))
     barrier()
     sampler.end()
+    if args.dump_outputs and rank == 0:
+        if last is None:
+            raise SystemExit("--dump-outputs needs at least one timed step (--steps >= 1)")
+        dump_outputs(args.dump_outputs, last)
     wms = torch.tensor([a.elapsed_time(b) for a, b in windows], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(wms, op=dist.ReduceOp.MAX)   # per window: the slowest rank
@@ -475,12 +478,12 @@ def main():
         layer_ms = lt[len(lt) // 2] / nl
         pk = peaks()
         ach = flops / (layer_ms * 1e-3) / 1e12
-        traffic, traffic_src = ncu_layer_traffic() if precision == "bf16" else (None, None)
-        roof = {"bound": "tensor", "kernel": f"SRA encoder layer ({precision} path: window attention + fused tcgen05 chain; average over the "
+        traffic, traffic_src = None, None
+        roof = {"bound": "tensor", "kernel": f"SRA encoder layer ({precision} path: window attention + wgmma GEMMs; average over the "
                                              f"{nl}-layer stack call, L2 flushed before the call)",
                 "achieved": ach, "peak": pk["tf_sustained"], "unit": "TFLOP/s", "frac": ach / pk["tf_sustained"],
                 "traffic": traffic, "traffic_source": traffic_src,
-                "peak_source": pk["src"] + " bf16 sustained (kernel runs inside a 12-layer step)",
+                "peak_source": pk["src"] + " bf16 dense",
                 "flops_per_launch": flops, "ms_per_launch": layer_ms, "M": Mv,
                 "layer_share_of_step": nl * layer_ms / latency_ms}
 
@@ -514,7 +517,7 @@ def main():
             dist.all_reduce(t32, op=dist.ReduceOp.MAX)
         ms32 = float(t32[len(ws) // 2])
         fp32_rec = {"value": world * K32 / (ms32 / 1e3), "unit": "frames/s", "steps": K32, "ms_per_step": ms32 / K32,
-                    "frames_in_flight": len(e32), "tolerance": "1e-3 (fp32-tolerance mode, csrc/sra_fp32.cu: Linear layers as split-fp16 tcgen05 GEMMs with fp32 accumulation, fp32 SIMT window attention / LayerNorm)"}
+                    "frames_in_flight": len(e32), "tolerance": "1e-3 (fp32-tolerance mode, csrc/sra_fp32.cu: Linear layers as split-fp16 wgmma GEMMs with fp32 accumulation, fp32 SIMT window attention / LayerNorm)"}
         del e32
 
     # ---- training step (BASELINE config 4): fwd + bwd + ONE flat NCCL gradient all-reduce + fused AdamW, weak scaling ----

@@ -1,4 +1,4 @@
-/* libsstb200 - C ABI of the B200-native SST/FSD hot path.
+/* libsstb200 - C ABI of the H100-native SST/FSD hot path.
  *
  * Drop-in boundary (SURVEY.md 8b).  The reference (tusen-ai/SST @ 7c95376) reaches its native code
  * through three extension modules; each entry point below names the reference interface it replaces:
@@ -39,7 +39,7 @@ typedef struct sstb200_ctx sstb200_ctx;
                              * VFE / SIR tensor paths bf16; the API name of the mode stays 'bf16'. */
 #define SSTB200_PREC_F16 1
 #define SSTB200_PREC_FP32_TC 2 /* sstb200_spconv_forward only: fp32 tolerance on the tensor core - every operand carried as two fp16 numbers
-                                * (hi + residue, 22 significant bits), three tcgen05 products per stage, fp32 accumulation in TMEM */
+                                * (hi + residue, 22 significant bits), three wgmma products per stage, fp32 accumulation */
 
 int sstb200_version(void);
 sstb200_ctx* sstb200_create(int device);
@@ -225,7 +225,7 @@ typedef struct {
   float center_offset[3];    /* v/2 + range_min (voxel_encoder.py:160-162) */
   float rel_dist_scaler;     /* DynamicScatterVFE only, else 1 */
   float bn_eps;
-  int32_t precision;         /* SSTB200_PREC_FP32: FFMA everywhere; SSTB200_PREC_BF16: layer 1 on tcgen05 (bf16 operands) */
+  int32_t precision;         /* SSTB200_PREC_FP32: FFMA everywhere; SSTB200_PREC_BF16: layer 1 on wgmma (bf16 operands) */
   const float* weight[2];    /* vfe_layers.i.linear.weight  [C_i, in_i] */
   const float* bn_weight[2]; /* vfe_layers.i.norm.{weight,bias,running_mean,running_var} */
   const float* bn_bias[2];
@@ -304,7 +304,7 @@ int sstb200_sir_layer_forward(sstb200_ctx* ctx, const sstb200_sir_layer* layer, 
                               float* out_point, float* out_group);
 
 /* S1' as above, plus: a cached group CSR (csr_offsets [G+1], csr_order [N] from sstb200_group_csr; both NULL = built inside),
- * `precision` (SSTB200_PREC_BF16: the rel-MLP's last layer and both VFE layers run as tcgen05 GEMMs with bf16 operands and fp32
+ * `precision` (SSTB200_PREC_BF16: the rel-MLP's last layer and both VFE layers run as wgmma GEMMs with bf16 operands and fp32
  * accumulation - needs feat_channels [128,128], rel-MLP [16,32,cin], cin <= 192, else SSTB200 "unsupported" error) and a row
  * pitch for out_point (>= C_last; lets SIR.forward write block i's point features straight into block i+1's [points || feats]
  * input; bf16 path only, 0 = dense).  in_feats may likewise be a pitched matrix (in_ld floats per row, 0 = dense) whose columns
@@ -338,7 +338,7 @@ int sstb200_voxel2point(sstb200_ctx* ctx, const float* points, int point_dims, c
  * BasicShiftBlockV2.forward, models/sst/sst_basic_block_v2.py:144-169): layer l uses the windows of shift l % 2.
  * x [n,d] input (not modified), y [n,d] output, tmp [n,d] scratch; all fp32, distinct buffers.  With precision BF16 and the
  * SST-6 shape (d=128, h=8, ff=256, post-norm LayerNorm, GELU) this runs 2 launches per layer: ragged window attention and a
- * fused tcgen05 kernel (out-proj + LN1 + FFN + LN2 + the next layer's QKV); otherwise it loops sstb200_sra_layer_forward. */
+ * fused wgmma / TMA kernel (out-proj + LN1 + FFN + LN2 + the next layer's QKV); otherwise it loops sstb200_sra_layer_forward. */
 int sstb200_sra_stack_forward(sstb200_ctx* ctx, const sstb200_sra_layer* layers, int num_layers,
                               const sstb200_sra_plan* plan_shift0, const sstb200_sra_plan* plan_shift1, const float* x,
                               float* y, float* tmp, int n, const int32_t* n_dev, int precision);
@@ -399,8 +399,8 @@ int sstb200_spconv_table(sstb200_ctx* ctx, const int32_t* in_coors, int n_in, co
 /* out[o, :] = act( (sum_k feats[nbr[o][k], :] . W[k]) * scale + shift + residual[o, :] )   - one launch for conv + folded
  * BatchNorm1d (+ residual add) (+ ReLU).  feats [*, c_in] fp32, weight [KV, c_in, c_out] fp32 = the reference's parameter layout
  * (D,H,W,in,out; mmdet3d/ops/spconv/conv.py:97-98), scale / shift [c_out] or NULL (1 / 0), residual [n_out, c_out] or NULL.
- * precision FP32: FFMA implicit GEMM (c_in, c_out multiples of 4).  precision BF16 (16-bit operands, fp32 accumulation in TMEM):
- * tcgen05 implicit GEMM over weight_h16 = IEEE fp16 copy laid out [KV, c_out, c_in]; needs c_in, c_out multiples of 64, KV <= 27.
+ * precision FP32: FFMA implicit GEMM (c_in, c_out multiples of 4).  precision BF16 (16-bit operands, fp32 accumulation):
+ * wgmma implicit GEMM over weight_h16 = IEEE fp16 copy laid out [KV, c_out, c_in]; needs c_in, c_out multiples of 64, KV <= 27.
  * precision FP32_TC: the same kernel in split mode; weight_h16 = [2][KV, c_out, c_in]: the fp16 copy followed by the fp16 residue
  * (w - float(half(w))). */
 int sstb200_spconv_forward(sstb200_ctx* ctx, const float* feats, int c_in, const int32_t* nbr, int n_out, int kernel_volume,

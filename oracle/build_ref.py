@@ -29,13 +29,13 @@ def build_spconv(verbose=False):
         return None
     out = os.path.join(OUT, "spconv_build")
     os.makedirs(out, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "8")
     from torch.utils.cpp_extension import load
     srcs = [os.path.join(SPCONV_ROOT, "src", f) for f in ("all.cc", "indice.cc", "indice_cuda.cu", "reordering.cc", "reordering_cuda.cu",
                                                           "maxpool.cc", "maxpool_cuda.cu")]
     load(name=name, sources=srcs, extra_include_paths=[os.path.join(SPCONV_ROOT, "include")], extra_cflags=["-O2", "-w"],
-         extra_cuda_cflags=["-O2", "-w", "-gencode", "arch=compute_100a,code=sm_100a"], build_directory=out, verbose=verbose,
+         extra_cuda_cflags=["-O2", "-w", "-gencode", "arch=compute_90a,code=sm_90a"], build_directory=out, verbose=verbose,
          is_python_module=False)
     import shutil
     for f in glob.glob(os.path.join(out, f"{name}*.so")):
@@ -51,13 +51,13 @@ def build(verbose=False):
     if not os.path.isdir(REF_SRC):
         return None
     os.makedirs(OUT, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "6")
     from torch.utils.cpp_extension import load
     srcs = [os.path.join(REF_SRC, f) for f in ("voxelization.cpp", "voxelization_cpu.cpp", "scatter_points_cpu.cpp",
                                                "scatter_points_cuda.cu", "voxelization_cuda.cu")]
     load(name="voxel_layer_ref", sources=srcs, extra_cflags=["-DWITH_CUDA", "-O2"],
-         extra_cuda_cflags=["-DWITH_CUDA", "-O2", "-gencode", "arch=compute_100a,code=sm_100a"],
+         extra_cuda_cflags=["-DWITH_CUDA", "-O2", "-gencode", "arch=compute_90a,code=sm_90a"],
          build_directory=OUT, verbose=verbose, is_python_module=False)
     return built()[0] if built() else None
 

@@ -1,4 +1,4 @@
-"""sst_b200 - B200-native (sm_100a) implementation of the SST / FSD data-parallel hot path behind the reference's
+"""sst_b200 - H100-native (sm_90a) implementation of the SST / FSD data-parallel hot path behind the reference's
 own module / op names (tusen-ai/SST).  The arithmetic lives in libsstb200.so (csrc/*.cu, C ABI in
 include/sstb200.h); this package is the host-side mirror of the reference interface.  There is no CPU or
 PyTorch fallback: using an op without the built library or without a CUDA device raises."""

@@ -82,7 +82,7 @@ def lib():
 def ctx(device=None):
     """Per-(device, current stream) context."""
     if not torch.cuda.is_available():
-        raise SSTB200Error("sst_b200 needs a CUDA device (sm_100a); no CPU fallback exists")
+        raise SSTB200Error("sst_b200 needs a CUDA device (sm_90a); no CPU fallback exists")
     if device is None:
         device = torch.cuda.current_device()
     elif isinstance(device, torch.device):

@@ -1,4 +1,4 @@
-"""Build libsstb200.so (sm_100a only) in-tree with nvcc.  `python -m sst_b200.build [-f]`."""
+"""Build libsstb200.so (sm_90a only) in-tree with nvcc.  `python -m sst_b200.build [-f]`."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libsstb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-warn-spills"]
 
 
@@ -51,7 +51,7 @@ def build(force=False, verbose=False):
             print(f"nvcc failed on {s}", file=sys.stderr)
     if failed:
         raise RuntimeError("libsstb200 build failed")
-    subprocess.check_call([NVCC, "-shared", "-o", OUT] + objs + ["-lcudart"])
+    subprocess.check_call([NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", OUT] + objs + ["-lcudart"])
     return OUT
 
 

@@ -2,7 +2,7 @@
 // (mmdet3d/models/detectors/single_stage_fsd.py:37-81 find_connected_componets{,_gpu,_single_batch}: a dense n x n distance matrix
 // handed to scipy.sparse.csgraph.connected_components on the CPU, or TorchEx's connected_components on the GPU).
 //
-// B200 form: no n x n matrix.  Centres are binned into a uniform xy grid of cell >= dist through the bitmap-rank index (cells ->
+// Form: no n x n matrix.  Centres are binned into a uniform xy grid of cell >= dist through the bitmap-rank index (cells ->
 // CSR of their points), every centre tests only the centres of its 3 x 3 cell neighbourhood, edges are merged in a lock-free
 // union-find whose roots are always the SMALLEST index of their tree (hook the larger root under the smaller with atomicMin), and the
 // labels are the rank of (batch, root) - exactly scipy's numbering (components numbered by their first node, samples in order).

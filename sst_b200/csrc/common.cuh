@@ -1,4 +1,4 @@
-// Shared device/host helpers for libsstb200 (sm_100a only).
+// Shared device/host helpers for libsstb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -21,7 +21,7 @@
 struct sstb200_ctx {
   int device = 0;
   cudaStream_t stream = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   // bump arena for temporaries; grows (with a sync) when a call needs more.
   char* arena = nullptr;
   size_t arena_cap = 0;

@@ -1,5 +1,5 @@
 // Bitmap-rank index ("unique rows, sorted" without a sort), CSR grouping and segmented reduce.
-// Shared by voxel.cu / window.cu / vfe.cu / sir.cu.  See DESIGN.md "voxel index".
+// Shared by voxel.cu / window.cu / vfe.cu / sir.cu.
 #pragma once
 #include "common.cuh"
 

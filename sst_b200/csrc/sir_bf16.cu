@@ -1,14 +1,15 @@
-// SIRLayer on the tensor cores (precision = BF16): two persistent tcgen05 kernels per layer, tiles of 128 points taken in
+// SIRLayer on the tensor cores (precision = BF16): two persistent wgmma kernels per layer, tiles of 128 points taken in
 // group (CSR) order so that the segmented max-pool is an in-tile scan with a handful of atomics per tile.
 //   models/voxel_encoders/voxel_encoder.py:696-764 (SIRLayer.forward), ops/sst/sst_ops.py:334-361 (build_mlp)
 //
 //   kernel A (per tile):  rel-MLP layers 1,2 in registers (thread per point)            3 -> R1 -> R2, LN + act each
-//                         rel-MLP layer 3 as UMMA  [128,R2] x [cin,R2]^T -> TMEM        LN + act in the epilogue,
+//                         rel-MLP layer 3 as wgmma [128,R2] x [cin,R2]^T               LN + act in the epilogue,
 //                         x0 = [xyz/normalizer || feats] * rel  -> bf16 A operand       (gating fused into that epilogue)
-//                         layer 0 as UMMA [128,KP] x [128,KP]^T -> TMEM                  LN + act -> p0 (bf16, CSR order) + segmax g0
-//   kernel B (per tile):  layer 1 as UMMA [128,256] x [128,256]^T on [p0 || g0[group]]  LN + act -> out (fp32, original point
+//                         layer 0 as wgmma [128,KP] x [128,KP]^T                         LN + act -> p0 (bf16, CSR order) + segmax g0
+//   kernel B (per tile):  layer 1 as wgmma [128,256] x [128,256]^T on [p0 || g0[group]] LN + act -> out (fp32, original point
 //                         (the concat exists only inside the operand tile)               order) + segmax g1
-// Operands are bf16 (fp32 accumulate in TMEM); LayerNorm, activations, gating, pooling and every output stay fp32.
+// Operands are bf16 (fp32 accumulate); LayerNorm, activations, gating, pooling and every output stay fp32.  Each GEMM is split over
+// the four warpgroups (row half x column half); the fragments meet the thread-per-row epilogues in a shared-memory accumulator tile.
 // The [N, 2*C0] concat of the reference is never formed; weights are converted to bf16 operands once per CTA.
 #include <stdarg.h>
 #include "index.cuh"
@@ -99,16 +100,21 @@ __device__ __forceinline__ void ln_regs(float* v, float& mean, float& rstd, floa
 }
 
 // ------------------------------------------------------------------------------------------------------------------------
-// kernel A.  512 threads = 16 warps: warp w owns TMEM lanes 32*(w%4).. (tile rows) and column quarter w/4 in every epilogue,
+// kernel A.  512 threads = 16 warps: warp w owns tile rows 32*(w%4).. and column quarter w/4 in every epilogue,
 // so 4 warps per scheduler hide the latency of the dependent LayerNorm / activation chains.
 // ------------------------------------------------------------------------------------------------------------------------
 constexpr int NT = 512;
 
-template <int NQC>
-__device__ __forceinline__ void tmem_ld_cols(uint32_t taddr, float* v) {
-  static_assert(NQC == 32 || NQC == 48, "quarter width");
-  tmem_ld32(taddr, v);
-  if (NQC == 48) tmem_ld16(taddr + 32, v + 32);
+// C[128, N] = A . B^T over KSTEPS K-steps of 16, warpgroup w: rows 64 (w & 1).., columns N/2 (w >> 1)..; result -> acc [128][N]
+template <int N, int KSTEPS>
+__device__ __forceinline__ void sir_gemm(uint32_t a, uint32_t a_cp, uint32_t b, uint32_t b_cp, float* acc, bool sync_operands) {
+  const int w = threadIdx.x >> 7;
+  float d[N / 4];
+  wg_tile_mma<N / 2, true, KSTEPS>(d, a + (w & 1) * 64 * 128, a_cp, b + (w >> 1) * (N / 2) * 128, b_cp, false);
+  wgmma_wait<0>();
+  if (sync_operands) __syncthreads();   // acc aliases an operand: every warpgroup must be done reading it
+  wg_store_acc<N / 2>(d, acc, N, (w & 1) * 64, (w >> 1) * (N / 2));
+  __syncthreads();
 }
 
 template <int KP, int R1, int R2, int ACT>
@@ -123,36 +129,28 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
   extern __shared__ uint8_t sira_raw[];
   uint8_t* base = (uint8_t*)(((uintptr_t)sira_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* sB0 = base;                          // W0  : KP/64 chunks x SC rows x 128 B
-  uint8_t* sB3 = sB0 + (size_t)SC * KP * 2;     // Wr3 : 1 chunk x KP rows x 128 B
-  uint8_t* sA0 = sB3 + (size_t)KP * 128;        // x0  : KP/64 chunks x ST rows x 128 B
-  uint8_t* sA3 = sA0 + (size_t)ST * KP * 2;     // r2  : 1 chunk x ST rows x 128 B
+  uint8_t* sA0 = sB0 + (size_t)SC * KP * 2;     // x0  : KP/64 chunks x ST rows x 128 B
+  uint8_t* sB3 = sA0 + (size_t)ST * KP * 2;     // Wr3 : 1 chunk x KP rows x 128 B (restaged every tile: the accumulators overwrite it)
+  uint8_t* sA3 = sB3 + (size_t)KP * 128;        // r2  : 1 chunk x ST rows x 128 B
   float* sIn = reinterpret_cast<float*>(sA3 + (size_t)ST * 128);  // in_feats tile [ST][pitch_in], pitch odd (thread-per-row reads)
+  // accumulator tiles, from sB3 on: rel layer 3 one column quarter at a time [ST][64] (inside Wr3 + r2), layer 0 [ST][SC] (Wr3 + r2 +
+  // in_feats, all dead by then)
+  float* sAcc = reinterpret_cast<float*>(sB3);
   __shared__ __align__(16) float sW1[R1 * 4], sW2[R2 * R1];
   __shared__ float sG1[R1], sBt1[R1], sG2[R2], sBt2[R2], sG3[KP], sBt3[KP], sG0[SC], sBt0[SC];
   __shared__ float redA[4][ST], redB[4][ST];
   __shared__ int sRowB[2][ST], sSegB[2][ST];  // double-buffered: the next tile's point / group ids are fetched during this tile
-  __shared__ __align__(8) uint64_t mbar;
-  __shared__ uint32_t tmem_slot;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntiles = (N + ST - 1) / ST;
   if ((int)blockIdx.x >= ntiles) return;
   const int cin = d.cin;
-  constexpr uint32_t TCOLS = KP > 128 ? 256 : 128;
-  if (warp == 0) tmem_alloc(&tmem_slot, TCOLS);
-  if (tid == 0) {
-    mbar_init(smem_u32(&mbar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
   for (int i = tid; i < R1 * 4; i += NT) sW1[i] = (i % 4) < d.rel_in ? d.rw[0][(i / 4) * d.rel_in + (i % 4)] : 0.f;
   for (int i = tid; i < R2 * R1; i += NT) sW2[i] = d.rw[1][i];
   for (int i = tid; i < R1; i += NT) sG1[i] = d.rg[0][i], sBt1[i] = d.rb[0][i];
   for (int i = tid; i < R2; i += NT) sG2[i] = d.rg[1][i], sBt2[i] = d.rb[1][i];
   for (int i = tid; i < KP; i += NT) sG3[i] = i < cin ? d.rg[2][i] : 0.f, sBt3[i] = i < cin ? d.rb[2][i] : 0.f;
   for (int i = tid; i < SC; i += NT) sG0[i] = d.g0[i], sBt0[i] = d.b0[i];
-  for (int i = tid; i < ST * 8; i += NT) reinterpret_cast<int4*>(sA3)[i] = make_int4(0, 0, 0, 0);  // K columns R2..63 stay zero
   stage_weight(sB0, SC, KP, d.w0, cin, 0, SC, cin);
-  stage_weight(sB3, KP, 64, d.rw[2], R2, 0, cin, R2);
-  uint32_t parity = 0;
   const int quarter = warp >> 2;
   const int lrow = (warp & 3) * 32 + lane;
   int cur = 0;
@@ -167,7 +165,8 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
     const int nrow = min(ST, N - k0);
     const int* sRow = sRowB[cur];
     const int* sSeg = sSegB[cur];
-    __syncthreads();  // previous tile fully consumed (sIn / operands) and this tile's ids visible
+    __syncthreads();  // previous tile fully consumed (sIn / operands / accumulators) and this tile's ids visible
+    stage_weight(sB3, KP, 64, d.rw[2], R2, 0, cin, R2);
     int nx_row = -1, nx_seg = -1;
     if (tid < ST) {
       int k = (tile + (int)gridDim.x) * ST + tid;
@@ -238,32 +237,40 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
       q4.z = (int)pack_bf16(h2[4], h2[5]);
       q4.w = (int)pack_bf16(h2[6], h2[7]);
       *reinterpret_cast<int4*>(sA3 + r * 128 + ((part ^ (r & 7)) << 4)) = q4;
+      // K columns R2..63 are zero (the previous tile's accumulators overwrote them)
+      *reinterpret_cast<int4*>(sA3 + r * 128 + (((part + 4) ^ (r & 7)) << 4)) = make_int4(0, 0, 0, 0);
     }
     asm volatile("cp.async.wait_all;\n" ::: "memory");
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    if (tid == 0) {  // rel layer 3: [ST, R2] x [KP rows, R2]^T
-      const uint32_t idesc = umma_idesc(128, KP);
-      const uint32_t a0 = smem_u32(sA3), b0 = smem_u32(sB3);
+    // rel layer 3: [ST, R2] x [KP rows, R2]^T, warpgroup w: rows 64 (w & 1).., columns KP/2 (w >> 1)..; the fragments reach the
+    // thread-per-row epilogue one column quarter at a time through a [ST][64] tile
+    float v[NQC];
+    {
+      const int w = tid >> 7;
+      float dq[KP / 4];
+      wg_tile_mma<KP / 2, true, R2 / 16>(dq, smem_u32(sA3) + (w & 1) * 64 * 128, ST * 128, smem_u32(sB3) + (w >> 1) * (KP / 2) * 128, KP * 128,
+                                         false);
+      wgmma_wait<0>();
+      __syncthreads();   // the accumulator tile aliases both operands
 #pragma unroll
-      for (int s = 0; s < R2 / 16; s++) umma_bf16(tmem, umma_desc_sw128(a0 + s * 32), umma_desc_sw128(b0 + s * 32), idesc, s ? 1u : 0u);
-      umma_commit(smem_u32(&mbar));
+      for (int q = 0; q < 4; q++) {
+        if ((w >> 1) == (q >> 1)) {
+          const int c0 = (q & 1) * NQC;
+          wg_frag_pairs<KP / 2>(dq, [&](int r, int c, float v0, float v1) {
+            if (c >= c0 && c < c0 + NQC) *reinterpret_cast<float2*>(sAcc + acc_idx(64, (w & 1) * 64 + r, c - c0)) = make_float2(v0, v1);
+          });
+        }
+        __syncthreads();
+        if (quarter == q) acc_ld<NQC>(sAcc, 64, lrow, 0, v);
+        __syncthreads();
+      }
     }
-    __syncwarp();
-    mbar_wait(smem_u32(&mbar), parity);
-    parity ^= 1u;
-    tc_fence_after();
     if (nx_row >= 0) nx_seg = (int)inv[nx_row];
-    const uint32_t tlane = tmem + ((uint32_t)((warp & 3) * 32) << 16);
     {
       // epilogue rel3: LayerNorm over cin, act, gate with [xyz / normalizer || feats] -> x0 (bf16 A operand of layer 0)
       const int qb = quarter * NQC;
       const int nvalid = min(max(cin - qb, 0), NQC);  // warp-uniform: valid channels of this quarter
-      float v[NQC];
-      tmem_ld_cols<NQC>(tlane + qb, v);
       // columns >= cin are exactly 0 (zero weight rows), so plain sums work; the variance is corrected for them below
       float s = 0.f;
 #pragma unroll
@@ -310,28 +317,14 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
       }
     }
     fence_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (tid == 0) {  // layer 0: [ST, KP] x [SC, KP]^T
-      const uint32_t idesc = umma_idesc(128, SC);
-      const uint32_t a0 = smem_u32(sA0), b0 = smem_u32(sB0);
-#pragma unroll
-      for (int c = 0; c < KP / 64; c++)
-#pragma unroll
-        for (int s = 0; s < 4; s++)
-          umma_bf16(tmem, umma_desc_sw128(a0 + c * ST * 128 + s * 32), umma_desc_sw128(b0 + c * SC * 128 + s * 32), idesc, (c | s) ? 1u : 0u);
-      umma_commit(smem_u32(&mbar));
-    }
-    __syncwarp();
-    mbar_wait(smem_u32(&mbar), parity);
-    parity ^= 1u;
-    tc_fence_after();
+    __syncthreads();   // x0 complete; every thread is done reading the rel-3 accumulators
+    // layer 0: [ST, KP] x [SC, KP]^T
+    sir_gemm<SC, KP / 16>(smem_u32(sA0), ST * 128, smem_u32(sB0), SC * 128, sAcc, false);
     {
       // epilogue 0: LayerNorm over SC, act -> p0 (bf16 rows in CSR order for kernel B; fp32 tile for the pooled max)
       constexpr int H = SC / 4;
       float v[H];
-      tmem_ld32(tlane + quarter * H, v);
+      acc_ld<H>(sAcc, SC, lrow, quarter * H, v);
       float s = 0.f;
 #pragma unroll
       for (int i = 0; i < H; i++) s += v[i];
@@ -368,11 +361,7 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
       sSegB[cur ^ 1][tid] = nx_seg;
     }
     cur ^= 1;
-    tc_fence_before();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_slot, TCOLS);
 }
 
 // ------------------------------------------------------------------------------------------------------------------------
@@ -389,22 +378,15 @@ __global__ void __launch_bounds__(NT, 1) sir_b_kernel(SirDev d, const __nv_bfloa
   constexpr int K1 = 2 * SC;                 // the reference's [p0 || g0[group]] input, formed only inside the operand tile
   uint8_t* sB = base;                        // W1  : 4 chunks x SC rows x 128 B
   uint8_t* sA = sB + (size_t)SC * K1 * 2;    // [p0 || g0[group]] : 4 chunks x ST rows x 128 B
+  float* sAcc = reinterpret_cast<float*>(sA);  // accumulator tile [ST][SC] fp32, aliases the A operand
   __shared__ float sG[SC], sBt[SC];
   __shared__ float redA[4][ST], redB[4][ST];
   __shared__ int sRowB[2][ST], sSegB[2][ST];
-  __shared__ __align__(8) uint64_t mbar;
-  __shared__ uint32_t tmem_slot;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntiles = (N + ST - 1) / ST;
   if ((int)blockIdx.x >= ntiles) return;
-  if (warp == 0) tmem_alloc(&tmem_slot, SC);
-  if (tid == 0) {
-    mbar_init(smem_u32(&mbar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
   for (int i = tid; i < SC; i += NT) sG[i] = d.g1[i], sBt[i] = d.b1[i];
   stage_weight(sB, SC, K1, d.w1, K1, 0, SC, K1);
-  uint32_t parity = 0;
   const int quarter = warp >> 2;
   const int lrow = (warp & 3) * 32 + lane;
   constexpr int H = SC / 4;
@@ -464,28 +446,11 @@ __global__ void __launch_bounds__(NT, 1) sir_b_kernel(SirDev d, const __nv_bfloa
     }
     asm volatile("cp.async.wait_all;\n" ::: "memory");
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    if (tid == 0) {
-      const uint32_t idesc = umma_idesc(128, SC);
-      const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-#pragma unroll
-      for (int c = 0; c < K1 / 64; c++)
-#pragma unroll
-        for (int s = 0; s < 4; s++)
-          umma_bf16(tmem, umma_desc_sw128(a0 + c * ST * 128 + s * 32), umma_desc_sw128(b0 + c * SC * 128 + s * 32), idesc, (c | s) ? 1u : 0u);
-      umma_commit(smem_u32(&mbar));
-    }
-    __syncwarp();
-    mbar_wait(smem_u32(&mbar), parity);
-    parity ^= 1u;
-    tc_fence_after();
+    sir_gemm<SC, K1 / 16>(smem_u32(sA), ST * 128, smem_u32(sB), SC * 128, sAcc, true);
     if (nx_row >= 0) nx_seg = (int)inv[nx_row];
-    const uint32_t tlane = tmem + ((uint32_t)((warp & 3) * 32) << 16);
     float v[H];
-    tmem_ld32(tlane + quarter * H, v);
+    acc_ld<H>(sAcc, SC, lrow, quarter * H, v);
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < H; i++) s += v[i];
@@ -519,11 +484,7 @@ __global__ void __launch_bounds__(NT, 1) sir_b_kernel(SirDev d, const __nv_bfloa
       sSegB[cur ^ 1][tid] = nx_seg;
     }
     cur ^= 1;
-    tc_fence_before();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_slot, SC);
 }
 
 }  // namespace
@@ -557,7 +518,11 @@ int sstb_sir_layer_bf16(sstb200_ctx* c, const sstb200_sir_layer* L, const float*
   cudaStream_t st = c->stream;
   const int KP = cin <= 128 ? 128 : 192;
   const int pitch_in = cin | 1;
-  const size_t smemA = 1024 + (size_t)SC * KP * 2 + (size_t)KP * 128 + (size_t)ST * KP * 2 + (size_t)ST * 128 + (size_t)ST * pitch_in * 4;
+  // in_feats region at least large enough for the layer-0 accumulator tile [ST][SC] fp32 that starts at Wr3
+  size_t in_bytes = (size_t)ST * pitch_in * 4;
+  const size_t acc0 = (size_t)ST * SC * 4 - (size_t)KP * 128 - (size_t)ST * 128;
+  if (in_bytes < acc0) in_bytes = acc0;
+  const size_t smemA = 1024 + (size_t)SC * KP * 2 + (size_t)KP * 128 + (size_t)ST * KP * 2 + (size_t)ST * 128 + in_bytes;
   const size_t smemB = 1024 + (size_t)SC * 2 * SC * 2 + (size_t)ST * 2 * SC * 2;
   if (smemA + 12 * 1024 > 227 * 1024)  // + ~11 KB of static shared memory
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "SIRLayer bf16: tile of cin=%d does not fit shared memory", cin);

@@ -3,10 +3,10 @@
 // (vendored v1: mmdet3d/ops/spconv/include/spconv/geometry.h:25-301 builds the index pairs, spconv_ops.h:95-260 runs one gather ->
 // GEMM -> scatter-add per kernel offset).
 //
-// B200 form: OUTPUT-STATIONARY.  The rulebook is a neighbour table nbr[o][k] = input row that feeds output row o through kernel
+// Form: OUTPUT-STATIONARY.  The rulebook is a neighbour table nbr[o][k] = input row that feeds output row o through kernel
 // offset k (or -1), built from the bitmap-rank index of the active coordinates (no hash table, no sort, no atomics on features); a
 // convolution is then ONE implicit-GEMM launch: an output tile gathers its <= KV input rows per offset, accumulates all offsets
-// in registers / TMEM and applies the folded BatchNorm (+ residual) (+ ReLU) epilogue before its single store.  The reference's
+// in registers and applies the folded BatchNorm (+ residual) (+ ReLU) epilogue before its single store.  The reference's
 // form writes every output row KV times with atomics-free but serialised scatter-adds and keeps BN / ReLU / residual as separate
 // passes over [N, C].
 #include <stdarg.h>
@@ -306,12 +306,14 @@ __global__ void __launch_bounds__(256) spconv_dw_kernel(const float* __restrict_
 
 // ------------------------------------------------------------------------------------------------------------------------------
 // tensor-core implicit GEMM (precision 'bf16' = 16-bit operands, fp32 accumulation): 128-row output tile x NT output channels per
-// CTA, accumulators [128, NT] fp32 in TMEM across ALL kernel offsets, operands IEEE fp16 in the K-major SWIZZLE_128B layout (same
-// staging / descriptors as umma_gemm.cuh).  K is walked in stages of (kernel offset, 64 input channels): the 256 threads gather the
-// 128 neighbour rows (fp32 -> fp16 on the fly, absent neighbours = zero rows that are neither loaded nor converted) and the [NT, 64]
-// weight slab into one of NS operand buffers, one thread issues 4 tcgen05.mma (K = 16 each) and commits to the buffer's mbarrier; the
-// global loads run TWO stages ahead in two register sets (the deep levels of a U-Net are a few CTAs walking 100-200 stages each:
-// pure load latency), and a buffer is rewritten only after its commit has fired.  Offsets no row of the tile uses are skipped.  Epilogue: thread-per-row out of TMEM, y = acc * scale + shift (+ residual) (ReLU), fp32 rows.
+// CTA, accumulators [128, NT] fp32 in registers across ALL kernel offsets (warpgroup g owns rows [64 g, 64 g + 64)), operands IEEE
+// fp16 in the K-major SWIZZLE_128B layout (same staging / descriptors as umma_gemm.cuh).  K is walked in stages of (kernel offset,
+// 64 input channels): the 256 threads gather the 128 neighbour rows (fp32 -> fp16 on the fly, absent neighbours = zero rows that are
+// neither loaded nor converted) and the [NT, 64] weight slab into one of NS operand buffers, each warpgroup issues 4 wgmma (K = 16
+// each) as one commit group; the global loads run TWO stages ahead in two register sets (the deep levels of a U-Net are a few CTAs
+// walking 100-200 stages each: pure load latency), and a buffer is rewritten only after every warpgroup's group that read it has
+// completed (wgmma.wait_group before the stage barrier).  Offsets no row of the tile uses are skipped.  Epilogue straight from the
+// accumulator fragments: y = acc * scale + shift (+ residual) (ReLU), fp32 rows.
 // ------------------------------------------------------------------------------------------------------------------------------
 constexpr int SPU_TM = 128;
 constexpr int SPU_A_BYTES = SPU_TM * 128;
@@ -349,7 +351,7 @@ struct SpStageRegs {
 };
 
 // SPLIT = the fp32-tolerance mode on the tensor core: every fp32 operand is carried as two fp16 numbers (hi = rn(x), lo = rn(x - hi):
-// 22 significant bits), and a stage issues the three products hi.hi + lo.hi + hi.lo into the same fp32 TMEM accumulator (the
+// 22 significant bits), and a stage issues the three products hi.hi + lo.hi + hi.lo into the same fp32 accumulators (the
 // dropped lo.lo term is 2^-22 relative).  Same staging, same epilogue; 3x the MMAs, 2x the operand bytes.
 template <int NT, int NS, bool SPLIT>
 __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma_kernel(SpArgs g) {
@@ -361,23 +363,17 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
   constexpr int ST_BYTES = (SPLIT ? 2 : 1) * (SPU_A_BYTES + B_BYTES);   // [A_hi][A_lo][B_hi][B_lo] or [A][B]
   constexpr int OFF_ALO = SPU_A_BYTES, OFF_B = (SPLIT ? 2 : 1) * SPU_A_BYTES, OFF_BLO = OFF_B + B_BYTES;
   constexpr int BU = NT / 32;  // 16-byte weight pieces per thread and stage
-  __shared__ __align__(8) uint64_t mbar[NS];
-  __shared__ uint32_t tmem_slot;
+  static_assert(NS >= 2, "the stage barrier retires the group of the stage NS - 1 back");
   __shared__ uint32_t used_mask;
   __shared__ int sNbr[SPU_TM][SPU_MAX_KV];   // odd row pitch: conflict-free column reads
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
   const int row0 = blockIdx.x * SPU_TM, n0 = blockIdx.y * NT;
   const int n_out = g.n_dev ? min(g.n_out, *g.n_dev) : g.n_out;
-  if (row0 >= n_out) return;   // uniform per CTA, nothing allocated yet
+  if (row0 >= n_out) return;   // uniform per CTA
   const int KV = g.KV, Cin = g.Cin, Cout = g.Cout;
-  if (warp == 0) tmem_alloc(&tmem_slot, NT);
-  if (tid == 0) {
-#pragma unroll
-    for (int b = 0; b < NS; b++) mbar_init(smem_u32(&mbar[b]), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    used_mask = 0u;
-  }
+  const int wg = tid >> 7;
+  if (tid == 0) used_mask = 0u;
   __syncthreads();
   {
     uint32_t m = 0u;
@@ -392,10 +388,7 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
     for (int o = 16; o > 0; o >>= 1) m |= __shfl_xor_sync(0xffffffffu, m, o);
     if (lane == 0 && m) atomicOr(&used_mask, m);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
   const int nch = Cin >> 6;
   const int nst = __popc(used_mask) * nch;
 
@@ -429,14 +422,14 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
       ld_mask &= ld_mask - 1u;
     }
   };
+  float acc[NT / 2];
+#pragma unroll
+  for (int i = 0; i < NT / 2; i++) acc[i] = 0.f;
+  // buffer s % NS was last read by stage s - NS, whose groups the barrier of stage s - 1 has retired (see below)
   auto run_stage = [&](int s, SpStageRegs<BU, SPLIT>& R) {
-    const int b = s % NS, u_ = s / NS;
+    const int b = s % NS;
     uint8_t* sA = base + (size_t)b * ST_BYTES;
     uint8_t* sB = sA + OFF_B;
-    if (u_ >= 1) {  // the MMAs that read this buffer NS stages ago have completed
-      mbar_wait(smem_u32(&mbar[b]), (uint32_t)((u_ - 1) & 1));
-      tc_fence_after();
-    }
 #pragma unroll
     for (int u = 0; u < 4; u++) {
       const int r = my_r + 32 * u;
@@ -468,23 +461,21 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
     }
     load_next(R);         // the register set is free again: fetch the stage two ahead while this one is multiplied
     fence_async_smem();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
-    tc_fence_before();
+    wgmma_wait<NS - 2>(); // this warpgroup's groups up to stage s - NS + 1 are complete once every thread passes the barrier
     __syncthreads();
-    tc_fence_after();
-    if (tid == 0) {
-      const uint32_t idesc = umma_idesc_f16(SPU_TM, NT);
-      const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
+    {
+      const uint32_t a0 = smem_u32(sA) + wg * 64 * 128, b0 = smem_u32(sB);
+      wgmma_fence();
 #pragma unroll
-      for (int q = 0; q < 4; q++)
-        umma_f16(tmem, umma_desc_sw128(a0 + q * 32), umma_desc_sw128(b0 + q * 32), idesc, (s | q) ? 1u : 0u);
+      for (int q = 0; q < 4; q++) wgmma_ss<NT, false>(acc, wg_desc_sw128(a0 + q * 32), wg_desc_sw128(b0 + q * 32), 1);
       if (SPLIT) {
-        const uint32_t al = a0 + OFF_ALO, bl = a0 + OFF_BLO;
+        const uint32_t al = a0 + OFF_ALO, bl = smem_u32(sA) + OFF_BLO;
 #pragma unroll
-        for (int q = 0; q < 4; q++) umma_f16(tmem, umma_desc_sw128(al + q * 32), umma_desc_sw128(b0 + q * 32), idesc, 1u);   // lo . hi
+        for (int q = 0; q < 4; q++) wgmma_ss<NT, false>(acc, wg_desc_sw128(al + q * 32), wg_desc_sw128(b0 + q * 32), 1);   // lo . hi
 #pragma unroll
-        for (int q = 0; q < 4; q++) umma_f16(tmem, umma_desc_sw128(a0 + q * 32), umma_desc_sw128(bl + q * 32), idesc, 1u);   // hi . lo
+        for (int q = 0; q < 4; q++) wgmma_ss<NT, false>(acc, wg_desc_sw128(a0 + q * 32), wg_desc_sw128(bl + q * 32), 1);   // hi . lo
       }
-      umma_commit(smem_u32(&mbar[b]));  // implicit tcgen05.fence::before_thread_sync
+      wgmma_commit();
     }
   };
 
@@ -496,54 +487,25 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
     run_stage(s, R0);
     if (s + 1 < nst) run_stage(s + 1, R1);
   }
-  if (nst > 0) {
-    const int s = nst - 1;
-    mbar_wait(smem_u32(&mbar[s % NS]), (uint32_t)((s / NS) & 1));   // commit of the last stage: every MMA of the tile is done
-    tc_fence_after();
-  }
+  wgmma_wait<0>();   // every MMA of the tile is done
 
-  // ---- epilogue -------------------------------------------------------------------------------------------------------------
-  const int half = warp >> 2;                       // warps 0-3: columns [0, NT/2), warps 4-7: [NT/2, NT)
-  const int lrow = (warp & 3) * 32 + lane;          // TMEM lane == row inside the tile
-  const uint32_t tlane = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-  const int o = row0 + lrow;
-  constexpr int CB = NT / 2;
-#pragma unroll 1
-  for (int c0 = half * CB; c0 < half * CB + CB; c0 += 32) {
-    float v[32];
-    if (nst > 0) {
-      tmem_ld32(tlane + c0, v);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 32; i++) v[i] = 0.f;
+  // ---- epilogue, from the accumulator fragments -------------------------------------------------------------------------------
+  wg_frag_pairs<NT>(acc, [&](int r, int cc, float v0, float v1) {
+    const int o = row0 + wg * 64 + r;
+    if (o >= n_out) return;
+    const int col = n0 + cc;
+    float2 sc = make_float2(1.f, 1.f), sh = make_float2(0.f, 0.f);
+    if (g.scale) sc = __ldg(reinterpret_cast<const float2*>(g.scale + col));
+    if (g.shift) sh = __ldg(reinterpret_cast<const float2*>(g.shift + col));
+    float2 y = make_float2(fmaf(v0, sc.x, sh.x), fmaf(v1, sc.y, sh.y));
+    if (g.act == 2) y.x = gelu_erf(y.x), y.y = gelu_erf(y.y);   // Linear -> GELU (-> + residual)
+    if (g.residual) {
+      const float2 r2 = *reinterpret_cast<const float2*>(g.residual + (size_t)o * g.ldr + col);
+      y.x += r2.x, y.y += r2.y;
     }
-    if (o < n_out) {
-      const int col = n0 + c0;
-      float* op = g.out + (size_t)o * g.ldo + col;
-      const float* rp = g.residual ? g.residual + (size_t)o * g.ldr + col : nullptr;
-#pragma unroll
-      for (int q = 0; q < 8; q++) {
-        float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (g.scale) sc = __ldg(reinterpret_cast<const float4*>(g.scale + col) + q);
-        if (g.shift) sh = __ldg(reinterpret_cast<const float4*>(g.shift + col) + q);
-        float4 y;
-        y.x = fmaf(v[4 * q], sc.x, sh.x);
-        y.y = fmaf(v[4 * q + 1], sc.y, sh.y);
-        y.z = fmaf(v[4 * q + 2], sc.z, sh.z);
-        y.w = fmaf(v[4 * q + 3], sc.w, sh.w);
-        if (g.act == 2) y.x = gelu_erf(y.x), y.y = gelu_erf(y.y), y.z = gelu_erf(y.z), y.w = gelu_erf(y.w);   // Linear -> GELU (-> + residual)
-        if (rp) {
-          const float4 r4 = *(reinterpret_cast<const float4*>(rp) + q);
-          y.x += r4.x, y.y += r4.y, y.z += r4.z, y.w += r4.w;
-        }
-        if (g.act == 1) y.x = fmaxf(y.x, 0.f), y.y = fmaxf(y.y, 0.f), y.z = fmaxf(y.z, 0.f), y.w = fmaxf(y.w, 0.f);  // conv + BN + res -> ReLU
-        *(reinterpret_cast<float4*>(op) + q) = y;
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, NT);
+    if (g.act == 1) y.x = fmaxf(y.x, 0.f), y.y = fmaxf(y.y, 0.f);  // conv + BN + res -> ReLU
+    *reinterpret_cast<float2*>(g.out + (size_t)o * g.ldo + col) = y;
+  });
 }
 
 template <int NT, int NS, bool SPLIT>
@@ -559,12 +521,12 @@ static int launch_spconv_umma(sstb200_ctx* c, const SpArgs& g) {
 }
 
 static int dispatch_spconv_umma(sstb200_ctx* c, const SpArgs& g, bool split) {
+  // 128 output channels per CTA at most: a warpgroup's [64, NT] fp32 accumulators take NT / 2 registers per thread, beside the
+  // two register sets of staged operands
   if (split) {
-    if (g.Cout % 256 == 0) return launch_spconv_umma<256, 2, true>(c, g);
     if (g.Cout % 128 == 0) return launch_spconv_umma<128, 2, true>(c, g);
     return launch_spconv_umma<64, 3, true>(c, g);
   }
-  if (g.Cout % 256 == 0) return launch_spconv_umma<256, 2, false>(c, g);
   if (g.Cout % 128 == 0) return launch_spconv_umma<128, 3, false>(c, g);
   return launch_spconv_umma<64, 3, false>(c, g);
 }

@@ -39,7 +39,7 @@ extern "C" int sstb200_sra_stack_forward(sstb200_ctx* c, const sstb200_sra_layer
   sstb200_sra_plan plans[2] = {*plan_shift0, *plan_shift1};
   if (precision == SSTB200_PREC_BF16) {
     arena_reset(c);
-    int rc = arena_reserve(c, (size_t)n * 128 * 8 + (size_t)num_layers * (256 * 64 * 2 + 4 * 128 * 4) + (1 << 20));
+    int rc = arena_reserve(c, (size_t)n * 128 * 8 + (size_t)num_layers * 4 * 128 * 4 + (1 << 20));
     if (rc) return rc;
     rc = sstb_sra_stack_bf16(c, layers, num_layers, plans, x, y, tmp, n, n_dev);
     if (rc != SSTB_ERR_UNSUPPORTED) return rc;

@@ -463,7 +463,7 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
 static inline int sstb_win_attn_batch(sstb200_ctx* c, const __half* qkv, const int32_t* counters, const int32_t* win_offsets,
                                       const int32_t* win_batch, int n_cap, const int32_t* tok_perm, void* out_v, bool out_bf16 = false,
                                       const float* tau = nullptr, int tau_n = 0, float tau_min = 0.f) {
-  constexpr int NHL = 2;   // heads per CTA -> 4 CTAs per window batch (4 heads per CTA measured slower on B200)
+  constexpr int NHL = 2;   // heads per CTA -> 4 CTAs per window batch 
   const int rec_cap = n_cap / 32 + 2;   // bound of the record array for the smallest batch size (csrc/window.cu)
   __half* out = reinterpret_cast<__half*>(out_v);
   const int4* recs = reinterpret_cast<const int4*>(win_batch);
@@ -475,7 +475,7 @@ static inline int sstb_win_attn_batch(sstb200_ctx* c, const __half* qkv, const i
                               : ensure_smem(c, sa, win_attn_batch_kernel<NHL, false, false>, smem)));
   static int grid_mult = 0;
   if (!grid_mult) {
-    const char* e = getenv("SSTB200_ATT_GRID");  // CTAs per SM of the persistent unit loop (tuning knob; default from the B200 sweep)
+    const char* e = getenv("SSTB200_ATT_GRID");  // CTAs per SM of the persistent unit loop (tuning knob)
     grid_mult = e && atoi(e) > 0 ? atoi(e) : 9;
   }
   static int dbg_on = -1;

@@ -1,16 +1,12 @@
 // 16-bit tensor-core path of the SRA encoder layer (precision 'bf16' of the API; operands are IEEE fp16 - same tensor
 // throughput, 8x smaller operand rounding than bf16, and the reference's own mixed-precision setting is fp16,
-// configs/sst_refactor/sst_waymoD5_1x_3class_8heads_v2.py:82): tcgen05.mma (UMMA) GEMMs with TMEM accumulators.
+// configs/sst_refactor/sst_waymoD5_1x_3class_8heads_v2.py:82): wgmma GEMMs with fp32 accumulators.
 //
-// Every dense op of the layer (QKV projection, attention out-projection, FFN1, FFN2) is one launch of the same
-// kernel template:  C[128-row tile, NT] = A[128, K] . W[NT, K]^T  with the whole K extent staged once in shared
-// memory (K <= 256 on this path, so there is no K pipeline to manage), accumulated in TMEM by ONE thread issuing
-// K/16 tcgen05.mma instructions, and a fused epilogue read back with tcgen05.ld (one thread per output row):
-//     EPI_BF16      + bias, optional GELU, store bf16                       (QKV, FFN1)
-//     EPI_RES_LN    + bias + fp32 residual, LayerNorm over the row (two TMEM passes), store fp32 (+ bf16 copy)
-// A-operand prologues convert on the fly: fp32 rows (+ positional embedding from the per-axis table) -> bf16, or
-// plain bf16 rows; both write the canonical K-major SWIZZLE_128B layout the UMMA descriptors expect.
-// fp32 stays the type of the residual stream, softmax, LayerNorm and all accumulation.
+// Per layer: the QKV projection (generic GEMM kernel of csrc/umma_gemm.cuh: C[128-row tile, NT] = A[128, K] . W[NT, K]^T,
+// A converted on the fly from fp32 rows + positional embedding, fp16 q|k|v out), the ragged window attention, and the fused
+// post-attention chain of csrc/sra_chain2.cu (out-projection + LN1 + FFN + LN2, in the encoder stack also the next layer's
+// QKV), so the stack takes 2 launches per layer.  fp32 stays the type of the residual stream, softmax, LayerNorm and all
+// accumulation.
 #include <stdarg.h>
 #include <cuda_fp16.h>
 #include "sra.cuh"
@@ -19,6 +15,30 @@
 #include "umma_gemm.cuh"
 
 namespace {
+
+// QKV projection of a layer: q,k from fp16(x + pos), v from fp16(x); EPI_F16 writes fp16 rows for the tensor-core attention
+int qkv_gemm(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb200_sra_plan* P, const float* x, __half* qkv, int n_cap,
+             const int32_t* n_dev, bool f16_out) {
+  const int d = L->d_model;
+  GemmArgs g;
+  memset(&g, 0, sizeof(g));
+  g.M_cap = n_cap;
+  g.M_dev = n_dev;
+  g.A = x;
+  g.lda = d;
+  g.W = L->in_proj_w_f16;
+  g.bias = L->in_proj_b;
+  g.pos_tab = P->pos_table;
+  g.pos_code = P->pos_code;
+  g.posL = P->pos_L;
+  g.pos_maxw = P->pos_maxw;
+  g.pos_ndim = P->pos_ndim;
+  g.pos_ntiles = 2;
+  g.out_h16 = qkv;
+  g.ldo = 3 * d;
+  g.out_row_map = nullptr;  // q|k|v, att and the residual stream all live in flat token order; attention gathers its windows
+  return f16_out ? launch_umma<128, 128, PRO_F32, EPI_F16>(c, g, 3) : launch_umma<128, 128, PRO_F32, EPI_H16>(c, g, 3);
+}
 
 }  // namespace
 
@@ -35,110 +55,29 @@ int sstb_sra_layer_bf16(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb20
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "bf16 path needs the per-axis positional length (%d) to be a multiple of 8", P->pos_L);
   __half* qkv = arena_alloc<__half>(c, (size_t)n_cap * 3 * d);
   __half* att = arena_alloc<__half>(c, (size_t)n_cap * d);
-  __half* x1b = arena_alloc<__half>(c, (size_t)n_cap * d);
-  __half* hid = arena_alloc<__half>(c, (size_t)n_cap * ff);
-  float* x1 = arena_alloc<float>(c, (size_t)n_cap * d);
-  if (!qkv || !att || !x1b || !hid || !x1) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sra bf16 layer: arena too small");
-  int rc;
-  static int dbg_skip = -1;  // SSTB200_DEBUG_SKIP bitmask (timing experiments only): 1 QKV, 2 attention, 4 chain
-  if (dbg_skip < 0) {
-    const char* e = getenv("SSTB200_DEBUG_SKIP");
-    dbg_skip = e ? atoi(e) : 0;
-  }
+  if (!qkv || !att) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sra bf16 layer: arena too small");
   // tensor-core attention path: plain scaled-dot-product, 8 heads x 16, windows <= 144 tokens
   const bool tc_attn = L->nhead == 8 && (!L->tau || L->tau_n == 1 || L->tau_n == 8) && P->max_window_tokens > 0 && P->max_window_tokens <= ATT_MAXT &&
                        P->num_windows_dev && P->win_batch;
-  GemmArgs g;
-  memset(&g, 0, sizeof(g));
-  g.M_cap = n_cap;
-  g.M_dev = n_dev;
-  // 1. QKV projection: q,k from bf16(x + pos), v from bf16(x)
-  g.A = x;
-  g.lda = d;
-  g.W = L->in_proj_w_f16;
-  g.bias = L->in_proj_b;
-  g.pos_tab = P->pos_table;
-  g.pos_code = P->pos_code;
-  g.posL = P->pos_L;
-  g.pos_maxw = P->pos_maxw;
-  g.pos_ndim = P->pos_ndim;
-  g.pos_ntiles = 2;
-  g.out_h16 = qkv;
-  g.ldo = 3 * d;
-  g.out_row_map = nullptr;  // q|k|v, att and the residual stream all live in flat token order; attention gathers its windows
-  // q/k/v for the tensor-core attention are written as fp16 (softmax logits need the mantissa: with bf16 q,k the logit
-  // error dominates the layer's error budget); the SIMT fallback reads bf16.
-  rc = (dbg_skip & 1) ? 0 : (tc_attn ? launch_umma<128, 128, PRO_F32, EPI_F16>(c, g, 3) : launch_umma<128, 128, PRO_F32, EPI_H16>(c, g, 3));
+  // 1. QKV projection.  q/k/v for the tensor-core attention are written as fp16 (softmax logits need the mantissa: with bf16
+  // q,k the logit error dominates the layer's error budget); the SIMT fallback reads bf16.
+  int rc = qkv_gemm(c, L, P, x, qkv, n_cap, n_dev, tc_attn);
   if (rc) return rc;
   // 2. ragged window attention (fp32 math on bf16 q/k/v)
-  if (dbg_skip & 2)
-    rc = 0;
-  else if (tc_attn)
+  if (tc_attn)
     rc = sstb_win_attn_batch(c, qkv, P->num_windows_dev, P->win_offsets, P->win_batch, n_cap, P->tok_perm, att, false, L->tau, L->tau_n, L->tau_min);
   else  // cosine attention / unbounded windows: SIMT kernel on the bf16 operands
     rc = sstb_win_attn<__half, __half>(c, qkv, d, L->nhead, n_cap, n_dev, P->win_offsets, P->tok_perm, P->tok_win,
                                                      L->tau, L->tau_n, L->tau_min, att);
   if (rc) return rc;
-  // 3-5 fused: out-projection + LN1 + FFN1 + GELU + FFN2 + LN2 in one persistent tcgen05 kernel (csrc/sra_chain.cu)
-  {
-    static int use_chain = -1;
-    if (use_chain < 0) {
-      const char* e = getenv("SSTB200_CHAIN");
-      use_chain = e ? atoi(e) : 1;   // 0: unfused GEMM launches (bring-up reference), else the warp-specialised TMA chain
-    }
-    if (dbg_skip & 4) return SSTB_OK;
-    if (use_chain) return sstb_sra_chain2(c, L, att, x, y, n_cap, n_dev);
-  }
-  // 3. out-projection + residual + LayerNorm1 (unfused reference path, SSTB200_CHAIN=0)
-  memset(&g, 0, sizeof(g));
-  g.M_cap = n_cap;
-  g.M_dev = n_dev;
-  g.A = att;
-  g.lda = d;
-  g.W = L->out_proj_w_f16;
-  g.bias = L->out_proj_b;
-  g.res = x;
-  g.gamma = L->norm1_w;
-  g.beta = L->norm1_b;
-  g.eps = L->norm_eps;
-  g.out_f32 = x1;
-  g.out_h16 = x1b;
-  g.ldo = d;
-  rc = launch_umma<128, 128, PRO_H16, EPI_RES_LN>(c, g, 1);
-  if (rc) return rc;
-  // 4. FFN1 + GELU
-  memset(&g, 0, sizeof(g));
-  g.M_cap = n_cap;
-  g.M_dev = n_dev;
-  g.A = x1b;
-  g.lda = d;
-  g.W = L->lin1_w_f16;
-  g.bias = L->lin1_b;
-  g.out_h16 = hid;
-  g.ldo = ff;
-  rc = launch_umma<128, 128, PRO_H16, EPI_H16_GELU>(c, g, 2);
-  if (rc) return rc;
-  // 5. FFN2 + residual + LayerNorm2
-  memset(&g, 0, sizeof(g));
-  g.M_cap = n_cap;
-  g.M_dev = n_dev;
-  g.A = hid;
-  g.lda = ff;
-  g.W = L->lin2_w_f16;
-  g.bias = L->lin2_b;
-  g.res = x1;
-  g.gamma = L->norm2_w;
-  g.beta = L->norm2_b;
-  g.eps = L->norm_eps;
-  g.out_f32 = y;
-  rc = launch_umma<256, 128, PRO_H16, EPI_RES_LN>(c, g, 1);
-  return rc;
+  // 3-5 fused: out-projection + LN1 + FFN1 + GELU + FFN2 + LN2
+  return sstb_sra_chain2(c, L, att, x, y, n_cap, n_dev);
 }
 
 
 // ------------------------------------------------------------------------------------------------
 // whole encoder stack, bf16 tensor-core path: QKV(0) -> [attention(l) -> chain(l) (+ QKV(l+1) fused)] x L
-// 2 launches per layer; q/k/v, attention output and the residual stream never take a detour.
+// 2 launches per layer; q/k/v, attention output and the residual stream stay in flat token order throughout.
 // ------------------------------------------------------------------------------------------------
 static bool layer_supported_tc(const sstb200_sra_layer* L, const sstb200_sra_plan* P) {
   // LayerNorm or eval-mode BatchNorm (use_bn), plain or cosine attention (tau per layer or per head)
@@ -158,59 +97,27 @@ int sstb_sra_stack_bf16(sstb200_ctx* c, const sstb200_sra_layer* layers, int num
   if (num_layers > SSTB_MAX_STACK) return SSTB_ERR_UNSUPPORTED;
   __half* qkv = arena_alloc<__half>(c, (size_t)n_cap * 3 * d);
   __half* att = arena_alloc<__half>(c, (size_t)n_cap * d);
-  __half* pos_qk = arena_alloc<__half>(c, (size_t)num_layers * 256 * 64);
   bool any_bn = false;
   for (int l = 0; l < num_layers; l++) any_bn |= layers[l].norm1_mean != nullptr;
   float* bn_fold = any_bn ? arena_alloc<float>(c, (size_t)num_layers * 4 * 128) : nullptr;
-  if (!qkv || !att || !pos_qk || (any_bn && !bn_fold)) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sra stack: arena too small");
+  if (!qkv || !att || (any_bn && !bn_fold)) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sra stack: arena too small");
   if (any_bn) {
     int rc = sstb_sra_bn_fold(c, layers, num_layers, bn_fold);
     if (rc) return rc;
   }
-  // the positional term of every layer's q|k projection, tabulated per (axis, coordinate): B operand of the chain's one-hot K chunk
-  // (both shifts share the table: it depends on the window shape only)
-  {
-    int rc = sstb_sra_pos_qk(c, layers, num_layers, &plans[0], pos_qk);
-    if (rc) return rc;
-  }
-  // QKV of layer 0 (stand-alone GEMM, fp32 x + pos -> fp16 rows in slot order of shift 0)
-  {
-    const sstb200_sra_layer* L = &layers[0];
-    const sstb200_sra_plan* P = &plans[0];
-    GemmArgs g;
-    memset(&g, 0, sizeof(g));
-    g.M_cap = n_cap;
-    g.M_dev = n_dev;
-    g.A = x;
-    g.lda = d;
-    g.W = L->in_proj_w_f16;
-    g.bias = L->in_proj_b;
-    g.pos_tab = P->pos_table;
-    g.pos_code = P->pos_code;
-    g.posL = P->pos_L;
-    g.pos_maxw = P->pos_maxw;
-    g.pos_ndim = P->pos_ndim;
-    g.pos_ntiles = 2;
-    g.out_h16 = qkv;
-    g.ldo = 3 * d;
-    int rc = launch_umma<128, 128, PRO_F32, EPI_F16>(c, g, 3);
-    if (rc) return rc;
-  }
-  static int skip = -1;   // SSTB200_STACK_SKIP bitmask (timing experiments only): 2 attention, 4 chain
-  if (skip < 0) skip = getenv("SSTB200_STACK_SKIP") ? atoi(getenv("SSTB200_STACK_SKIP")) : 0;
+  int rc = qkv_gemm(c, &layers[0], &plans[0], x, qkv, n_cap, n_dev, true);
+  if (rc) return rc;
   const float* xin = x;
   for (int l = 0; l < num_layers; l++) {
     const sstb200_sra_plan* P = &plans[l & 1];
-    int rc = (skip & 2) ? 0 : sstb_win_attn_batch(c, qkv, P->num_windows_dev, P->win_offsets, P->win_batch, n_cap, P->tok_perm, att, false,
-                                                  layers[l].tau, layers[l].tau_n, layers[l].tau_min);
+    rc = sstb_win_attn_batch(c, qkv, P->num_windows_dev, P->win_offsets, P->win_batch, n_cap, P->tok_perm, att, false, layers[l].tau,
+                             layers[l].tau_n, layers[l].tau_min);
     if (rc) return rc;
     const bool has_next = l + 1 < num_layers;
-    if (skip & 4) continue;
     // the chain reads the residual rows of a tile before it writes the same rows of y: in-place (xin == y) is safe
     rc = sstb_sra_chain2(c, &layers[l], att, xin, y, n_cap, n_dev, has_next ? &layers[l + 1] : nullptr,
-                                has_next ? &plans[(l + 1) & 1] : nullptr, has_next ? qkv : nullptr,
-                                has_next ? pos_qk + (size_t)(l + 1) * 256 * 64 : nullptr,
-                                layers[l].norm1_mean ? bn_fold + (size_t)l * 4 * 128 : nullptr);
+                         has_next ? &plans[(l + 1) & 1] : nullptr, has_next ? qkv : nullptr,
+                         layers[l].norm1_mean ? bn_fold + (size_t)l * 4 * 128 : nullptr);
     if (rc) return rc;
     xin = y;
   }

@@ -1,733 +1,271 @@
-// Fused post-attention chain of one SRA encoder layer, warp-specialised (d_model = 128, dim_ff = 256, post-norm LayerNorm, GELU):
+// Fused post-attention chain of one SRA encoder layer (d_model = 128, dim_ff = 256, post-norm LayerNorm or eval BatchNorm, GELU):
 //
-//     x1 = LayerNorm1(x + att . Wo^T + bo)          GEMM1  [128 x 128] x [128 x 128]
+//     x1 = Norm1(x + att . Wo^T + bo)               GEMM1  [128 x 128] x [128 x 128]
 //     h  = GELU(x1 . W1^T + b1)                     GEMM2  [128 x 128] x [128 x 256]   two N = 128 chunks
-//     y  = LayerNorm2(x1 + h . W2^T + b2)           GEMM3  [128 x 256] x [256 x 128]   four K = 64 chunks
-//     q|k|v (next layer) = (y + pos | y) . Wqkv^T   GEMM4  [128 x 128] x [128 x 384]   q|k as one N = 256 GEMM, v N = 128 (optional tail)
+//     y  = Norm2(x1 + h . W2^T + b2)                GEMM3  [128 x 256] x [256 x 128]   two K = 128 chunks
+//     q|k|v (next layer) = (y + pos | y) . Wqkv^T   GEMM4  [128 x 128] x [128 x 384]   three N = 128 chunks (optional tail)
 //
 // replaces mmdet3d/models/sst/sst_basic_block_v2.py:104-126 (+ the in-projection of the following layer's
 // nn.MultiheadAttention, :70) for one 128-token tile per iteration of a persistent CTA.
 //
-// Roles (19 warps):
-//   warp 17  TMA loads (one lane): every operand tile - att, the residual x, all weights - arrives by cp.async.bulk.tensor
-//            into 128B-swizzled shared memory; weights + att stream through a ring of three 32 KB slots (full/empty mbarriers).
-//   warp 16  MMA issuer (one lane): tcgen05.mma (fp16 operands, fp32 accumulators in TMEM), tcgen05.commit -> mbarriers.
-//   warp 18  TMA stores (one lane): y (fp32) and q|k|v (fp16) tiles leave through swizzled staging buffers; the warp turns
-//            "staging written" mbarriers into bulk stores and "store has read its source" into "staging free" mbarriers, so the
-//            epilogue never executes a CTA-wide barrier.
-//   warps 0-15  epilogue: TMEM -> registers (thread per row, 4 warps per TMEM lane quadrant, each a column quarter); bias /
-//            residual / LayerNorm in packed fp32x2 arithmetic (FADD2 / FFMA2), GELU in half2 (tanh form, MUFU.TANH.F16); the
-//            operands of the next GEMM are written straight into the swizzled K-major layout.
-// GEMM2 -> GELU -> GEMM3 is pipelined: two 128-column accumulator chunks in TMEM, two 64-column hidden chunks in shared memory,
-// and two epilogue warp groups (8 warps each) that own one accumulator chunk each and feed GEMM3 its K-chunks as they finish
-// them, so GELU overlaps the MMAs and the other group.  GEMM1 of the next tile is issued while the q|k|v epilogue of this one runs.
-// All rows are in flat token order: every tile of att / x / y / q|k|v is a plain 2-D TMA box.
+// Two warpgroups, each owning 64 rows of the tile, issue wgmma.mma_async (fp16 operands, fp32 accumulators in registers).  The att
+// tile and every weight arrive by cp.async.bulk.tensor (TMA) into 128B-swizzled shared memory: weights stream as 32 KB chunks
+// ([128 rows x 128 K]) through a ring of two slots with full mbarriers, and one thread refills a slot with the chunk two ahead (also
+// across tiles) as soon as both warpgroups have retired the MMAs that read it, so weight loads overlap the next GEMM and its
+// epilogue.  Epilogues run on the accumulator fragments: a row's 128 columns sit in one lane quad, so LayerNorm statistics take
+// two xor-shuffles; x1 stays in registers from GEMM1 to GEMM3; x1, h, y and y + pos reach the next GEMM as 16-bit operands written
+// straight into the swizzled K-major layout.  Only x (residual), y and q|k|v touch global memory.  All rows are in flat token order.
 //
-// TMEM columns: [0,128) acc1 / acc3, [128,256) acc2 chunk 0 (later q), [256,384) acc2 chunk 1 (later k), [384,512) x1 fp32 (later v).
-// Shared memory: ring 3 x 32 KB | A 32 KB (x1 operand, y staging lo, q / v staging) | B 32 KB (hidden chunks, y staging hi,
-// k staging) | C 64 KB (x fp32 tile, LN statistics exchange, then the (y+pos | y) operands) | mbarriers.
+// Shared memory: A 32 KB (att, then x1, then y) | P 32 KB (y + pos) | H 64 KB (hidden, four K = 64 blocks) | ring 2 x 32 KB.
 #include <stdarg.h>
 #include <cuda_fp16.h>
 #include "sra.cuh"
 #include "tma.cuh"
+#include "umma_gemm.cuh"
 
 namespace {
 
 constexpr int TM = 128, D = 128;
-constexpr int SLOT = 32768;
-constexpr int W_MMA = 16, W_TMA = 17, W_ST = 18;
-constexpr int NTHR = 19 * 32;
-constexpr int OFF_RING = 0, OFF_A = 3 * SLOT, OFF_B = 4 * SLOT, OFF_C = 5 * SLOT, OFF_BAR = 7 * SLOT;
-constexpr int SMEM_BYTES = 7 * SLOT + 512;
-
-enum {
-  B_FULL = 0,    // [3] ring slot filled (TMA transaction bytes)
-  B_EMPTY = 3,   // [3] ring slot consumed (tcgen05.commit)
-  B_XFULL = 6,   // residual tile landed in C
-  B_CFREE = 7,   // C may be overwritten by the next residual tile
-  B_ACC1 = 8,    // GEMM1 retired
-  B_X1 = 9,      // x1 operand (A) + fp32 copy (TMEM) written              [16 warp arrivals]
-  B_ACC2F = 10,  // [2] GEMM2 chunk retired
-  B_ACC2E = 12,  // [2] acc2 chunk read back                               [8]
-  B_HIDF = 14,   // [2] hidden chunk written                               [8]
-  B_HIDE = 16,   // [2] hidden chunk consumed by GEMM3
-  B_ACC3 = 18,   // GEMM3 retired
-  B_YFULL = 19,  // LN2 done: acc3 / x1 read, y staging + (y+pos | y) operands written [16]
-  B_QKVF = 20,   // [2] q|k / v GEMM retired                               (slot 22 unused)
-  B_QKVE = 23,   // [2] q|k / v accumulator read back                      [16] (slot 25 unused)
-  B_QST = 26,    // [3] q / k / v staging written                          [16]
-  B_FREEA = 29,  // staging buffer A drained by its TMA store
-  B_FREEB = 30,  // staging buffer B drained
-  NBAR = 31
-};
+constexpr int SLOT = 32768;   // one weight chunk: 128 rows x 128 K fp16 = two 64-wide swizzle blocks of 16 KB
+constexpr int OFF_A = 0, OFF_P = SLOT, OFF_H = 2 * SLOT, OFF_RING = 4 * SLOT;
+constexpr int SMEM_BYTES = 6 * SLOT + 1024;
+constexpr int NTHR = 256;
+constexpr uint32_t OPB = TM * 128;   // byte pitch of one 64-wide K block of a 128-row operand
 
 struct Chain2Maps {
-  CUtensorMap att, x, y, qkv, wo, w1, w2, wqkv, wqk, wpos;
+  CUtensorMap att, wo, w1, w2, wqkv;
 };
 
 struct Chain2Args {
-  const float *bo, *b1, *b2, *g1, *be1, *g2, *be2;
+  const float* x;
+  float* y;
+  __half* qkv;                   // [tokens, 384] next layer's q|k|v (tail only)
+  // norm: LayerNorm (g1/be1/g2/be2 = weight, bias) or eval-mode BatchNorm (affine: g* = folded scale, be* = folded shift)
+  const float *bo, *b1, *b2, *g1, *be1, *g2, *be2, *bqkv;
   float eps;
+  int affine;
   int M_cap;
   const int32_t* M_dev;
-  int has_tail;                  // GEMM4: q|k|v of the next layer
-  // norm: LayerNorm (g1/be1/g2/be2 = weight, bias) or eval-mode BatchNorm (layer_cfg use_bn: g* = folded scale, be* = folded shift)
-  const float* bqkv;             // [384]
-  const int32_t* next_pos_code;  // [tokens]
-  int pos_maxw, pos_ndim;        // one-hot column of (axis, in-window coordinate) = axis * maxw + coordinate (< 32)
-  long long* dbg;                // optional timeline buffer [grid][3 roles][2 tiles][32] (SSTB200_CHAIN_DBG), else nullptr
+  const float* pos_tab;          // next layer's per-axis positional table, added to y for the q|k chunks
+  const int32_t* pos_code;
+  int posL, pos_maxw, pos_ndim;
 };
 
-#define DBG_T(role, it, ev)                                                                                   \
-  do {                                                                                                        \
-    if (g.dbg && (it) < 2) g.dbg[(((size_t)blockIdx.x * 3 + (role)) * 2 + (it)) * 32 + (ev)] = clock64();       \
-  } while (0)
-
-typedef unsigned long long u64;
-// packed fp32x2 arithmetic (sm_100: FADD2 / FMUL2 / FFMA2 - one issue slot for two lanes)
-__device__ __forceinline__ u64 pk2(float lo, float hi) {
-  u64 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ u64 pk2u(uint32_t lo, uint32_t hi) {
-  u64 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ void up2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ void up2u(u64 v, uint32_t& lo, uint32_t& hi) { asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(v)); }
-__device__ __forceinline__ u64 add2(u64 a, u64 b) {
-  u64 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-  u64 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-// two fp32 -> packed half2 (lo in the low half)
-__device__ __forceinline__ uint32_t cvt_h2(u64 v) {
-  float lo, hi;
-  up2(v, lo, hi);
-  uint32_t r;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
+// chunk j of a tile: 0 Wo | 1, 2 W1 rows 0-127, 128-255 | 3, 4 W2 K 0-127, 128-255 | 5, 6, 7 Wqkv rows 0-127, 128-255, 256-383
+__device__ __forceinline__ void issue_chunk(const Chain2Maps& m, int j, uint32_t dst, uint32_t bar) {
+  const CUtensorMap* map = &m.wqkv;
+  int k0 = 0, n0 = 0;
+  if (j == 0) map = &m.wo;
+  else if (j <= 2) map = &m.w1, n0 = (j - 1) * 128;
+  else if (j <= 4) map = &m.w2, k0 = (j - 3) * 128;
+  else n0 = (j - 5) * 128;
+  mbar_expect_tx(bar, SLOT);
+  tma_load_2d(dst, map, k0, n0, bar);
+  tma_load_2d(dst + SLOT / 2, map, k0 + 64, n0, bar);
 }
 
-// tanh-form GELU on two values in half2: 0.5 z (1 + tanh(z (c0 + c1 z^2))).  No clamp is needed: if z^2 overflows fp16 the
-// argument becomes +-inf and tanh returns +-1, which is the right limit (z or 0).  Deviation from the erf form plus the half2
-// arithmetic stays below 1e-3 relative - the fp16 rounding of the operand it feeds is 5e-4.
-__device__ __forceinline__ uint32_t gelu_h2(uint32_t z) {
-  const uint32_t C0 = 0x3A623A62u;   // half2(0.7978846)
-  const uint32_t C1 = 0x28912891u;   // half2(0.0356774) = 0.7978846 * 0.044715
-  const uint32_t HALF = 0x38003800u;   // 0.5
-  uint32_t z2, p, u, t, hz, r;
-  asm("mul.rn.f16x2 %0, %1, %1;" : "=r"(z2) : "r"(z));
-  asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(p) : "r"(z2), "r"(C1), "r"(C0));
-  asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(u) : "r"(p), "r"(z));
-  asm("tanh.approx.f16x2 %0, %1;" : "=r"(t) : "r"(u));
-  asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(hz) : "r"(z), "r"(HALF));
-  asm("fma.rn.f16x2 %0, %1, %2, %1;" : "=r"(r) : "r"(hz), "r"(t));
-  return r;
+// 16-bit pair (columns k, k + 1) of row `row` into a 128-row K-major SWIZZLE_128B operand
+__device__ __forceinline__ void st_op(uint8_t* buf, int row, int k, uint32_t v) {
+  *reinterpret_cast<uint32_t*>(buf + (k >> 6) * OPB + row * 128 + ((((k & 63) >> 3) ^ (row & 7)) << 4) + (k & 7) * 2) = v;
 }
 
-__device__ __forceinline__ void tmem_ld32u(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-__device__ __forceinline__ void tmem_st32u(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-      "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]),
-      "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]),
-      "r"(v[31])
-      : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
-}
-
-// One tcgen05.mma; ACC is an immediate so that the accumulate predicate folds to a constant.
-template <int ACC>
-__device__ __forceinline__ void mma1(uint32_t d_tmem, u64 adesc, u64 bdesc, uint32_t idesc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "n"(ACC)
-      : "memory");
-}
-// K-major SWIZZLE_128B descriptors differ only in the start address: constant part once, then + (bytes >> 4).
-// KSTEPS = 4 (K = 64) or 8 (K = 128: operand K-chunk c lives a_chunk / b_chunk 16-byte units further).
-template <int KSTEPS, bool ACCUM>
-__device__ __forceinline__ void mma_steps(uint32_t d_tmem, u64 adesc, u64 bdesc, uint32_t idesc, uint32_t a_chunk = 1024, uint32_t b_chunk = 1024) {
+// t = fragment of [64 rows x 128] (rows ra: t[4j], t[4j+1]; rb: t[4j+2], t[4j+3]; columns 8j + 2 (lane & 3)): per-row normalisation
+__device__ __forceinline__ void row_norm(float (&t)[64], const float* __restrict__ gam, const float* __restrict__ bet, float eps, bool affine) {
+  const int cq = 2 * (threadIdx.x & 3);
+  float mean0 = 0.f, mean1 = 0.f, rstd0 = 1.f, rstd1 = 1.f;
+  if (!affine) {
+    float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
 #pragma unroll
-  for (int s = 0; s < KSTEPS; s++) {
-    const u64 ao = (u64)((s & 3) * 2) + (u64)((s >> 2) * a_chunk), bo = (u64)((s & 3) * 2) + (u64)((s >> 2) * b_chunk);
-    if (ACCUM || s > 0) mma1<1>(d_tmem, adesc + ao, bdesc + bo, idesc);
-    else mma1<0>(d_tmem, adesc + ao, bdesc + bo, idesc);
+    for (int j = 0; j < 16; j++) {
+      s0 += t[4 * j] + t[4 * j + 1];
+      q0 += t[4 * j] * t[4 * j] + t[4 * j + 1] * t[4 * j + 1];
+      s1 += t[4 * j + 2] + t[4 * j + 3];
+      q1 += t[4 * j + 2] * t[4 * j + 2] + t[4 * j + 3] * t[4 * j + 3];
+    }
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+      s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+      q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+      q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+    }
+    mean0 = s0 * (1.f / D), mean1 = s1 * (1.f / D);
+    rstd0 = rsqrtf(fmaxf(q0 * (1.f / D) - mean0 * mean0, 0.f) + eps);
+    rstd1 = rsqrtf(fmaxf(q1 * (1.f / D) - mean1 * mean1, 0.f) + eps);
+  }
+#pragma unroll
+  for (int j = 0; j < 16; j++) {
+    const int c = 8 * j + cq;
+    const float2 g2 = __ldg(reinterpret_cast<const float2*>(gam + c)), b2 = __ldg(reinterpret_cast<const float2*>(bet + c));
+    t[4 * j] = (t[4 * j] - mean0) * rstd0 * g2.x + b2.x;
+    t[4 * j + 1] = (t[4 * j + 1] - mean0) * rstd0 * g2.y + b2.y;
+    t[4 * j + 2] = (t[4 * j + 2] - mean1) * rstd1 * g2.x + b2.x;
+    t[4 * j + 3] = (t[4 * j + 3] - mean1) * rstd1 * g2.y + b2.y;
   }
 }
-template <bool TAIL, bool BN>
-__global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_constant__ Chain2Maps maps, const Chain2Args g) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t sbase = smem_u32(smem);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + OFF_BAR + NBAR * 8);
-#define BAR(i) (sbase + OFF_BAR + (uint32_t)(i) * 8u)
 
-  if (tid == 0) {
-    if (sbase & 1023u) __trap();   // SWIZZLE_128B operands / TMA boxes need the 1024-byte alignment
-    for (int i = 0; i < NBAR; i++) {
-      uint32_t cnt = 1;
-      if (i == B_X1 || i == B_YFULL || (i >= B_QKVE && i < B_QKVE + 2) || (i >= B_QST && i < B_QST + 3)) cnt = 16;
-      if (i == B_ACC2E || i == B_ACC2E + 1 || i == B_HIDF || i == B_HIDF + 1) cnt = 8;
-      mbar_init(BAR(i), cnt);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  if (warp == W_TMA && lane == 0) {
-    tma_prefetch_desc(&maps.att);
-    tma_prefetch_desc(&maps.x);
-    tma_prefetch_desc(&maps.wo);
-    tma_prefetch_desc(&maps.w1);
-    tma_prefetch_desc(&maps.w2);
-    if (TAIL) {
-      tma_prefetch_desc(&maps.wqkv);
-      tma_prefetch_desc(&maps.wqk);
-      tma_prefetch_desc(&maps.wpos);
-    }
-  }
-  if (warp == W_ST && lane == 0) {
-    tma_prefetch_desc(&maps.y);
-    if (TAIL) tma_prefetch_desc(&maps.qkv);
-  }
-  if (warp == W_MMA) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  pdl_wait();     // everything above overlaps the tail of the producer kernel
-  pdl_launch();
-  const int M = g.M_dev ? *g.M_dev : g.M_cap;
-  const int n_tiles = (M + TM - 1) / TM;
-  constexpr bool tail = TAIL;
-  const int NI = tail ? 10 : 6;   // ring items per tile: att, Wo, W1[0:128], W1[128:256], W2[:,0:128], W2[:,128:256], Wqk K-chunks 0 / 1, Wpos, Wv
-
-  if (warp == W_TMA) {
-    // ================================================== TMA loads ==================================================
-    if (lane == 0) {
-      int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int row0 = tile * TM;
-        const int k0 = it * NI;
-        auto load_item = [&](int j, const CUtensorMap* m, int ca, int ra, int cb, int rb) {
-          const int kk = k0 + j, s = kk % 3;
-          mbar_wait(BAR(B_EMPTY + s), (uint32_t)(((kk / 3) + 1) & 1));
-          mbar_expect_tx(BAR(B_FULL + s), SLOT);
-          tma_load_2d(sbase + OFF_RING + s * SLOT, m, ca, ra, BAR(B_FULL + s));
-          tma_load_2d(sbase + OFF_RING + s * SLOT + 16384, m, cb, rb, BAR(B_FULL + s));
-        };
-        DBG_T(2, it, 0);
-        load_item(0, &maps.att, 0, row0, 64, row0);
-        load_item(1, &maps.wo, 0, 0, 64, 0);
-        DBG_T(2, it, 1);
-        mbar_wait(BAR(B_CFREE), (uint32_t)((it + 1) & 1));   // previous tile's users of C are done
-        DBG_T(2, it, 2);
-        mbar_expect_tx(BAR(B_XFULL), 4 * 16384);
-#pragma unroll
-        for (int q = 0; q < 4; q++) tma_load_2d(sbase + OFF_C + q * 16384, &maps.x, q * 32, row0, BAR(B_XFULL));
-        load_item(2, &maps.w1, 0, 0, 64, 0);
-        load_item(3, &maps.w1, 0, 128, 64, 128);
-        DBG_T(2, it, 3);
-        load_item(4, &maps.w2, 0, 0, 64, 0);
-        load_item(5, &maps.w2, 128, 0, 192, 0);
-        DBG_T(2, it, 4);
-        if (tail) {
-          // Wq|Wk as ONE N = 256 operand: a slot per 64-wide K chunk (256 rows x 128 B), then Wv (two K chunks of 128 rows)
-          // + the positional term as a third K chunk: pos . [Wq; Wk]^T tabulated per (axis, coordinate) (256 rows x 64 columns)
-          auto load_qk = [&](int j, const CUtensorMap* m, int col) {
-            const int kk = k0 + j, s2 = kk % 3;
-            mbar_wait(BAR(B_EMPTY + s2), (uint32_t)(((kk / 3) + 1) & 1));
-            mbar_expect_tx(BAR(B_FULL + s2), SLOT);
-            tma_load_2d(sbase + OFF_RING + s2 * SLOT, m, col, 0, BAR(B_FULL + s2));
-          };
-          load_qk(6, &maps.wqk, 0);
-          load_qk(7, &maps.wqk, 64);
-          load_qk(8, &maps.wpos, 0);
-          load_item(9, &maps.wqkv, 0, 256, 64, 256);
-          DBG_T(2, it, 5);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == W_MMA) {
-    // ================================================== MMA issuer ==================================================
-    if (lane == 0) {
-      const uint32_t idesc128 = umma_idesc_f16(TM, 128), idesc256 = umma_idesc_f16(TM, 256);
-      const u64 dA = umma_desc_sw128(sbase + OFF_A), dB0 = umma_desc_sw128(sbase + OFF_B), dC = umma_desc_sw128(sbase + OFF_C);
-      const u64 dR = umma_desc_sw128(sbase + OFF_RING);
-      int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int k0 = it * NI;
-        const uint32_t par = (uint32_t)(it & 1);
-        auto slot = [&](int j) { return dR + (u64)(((k0 + j) % 3) * (SLOT >> 4)); };   // descriptor of ring item j
-        auto wait_full = [&](int j) {
-          const int kk = k0 + j;
-          mbar_wait(BAR(B_FULL + kk % 3), (uint32_t)((kk / 3) & 1));
-        };
-        auto release = [&](int j) { umma_commit(BAR(B_EMPTY + (k0 + j) % 3)); };
-        // ---- GEMM1: acc1 = att . Wo^T
-        DBG_T(1, it, 0);
-        wait_full(0);
-        wait_full(1);
-        tc_fence_after();
-        DBG_T(1, it, 1);
-        mma_steps<8, false>(tmem, slot(0), slot(1), idesc128);
-        umma_commit(BAR(B_ACC1));
-        release(0);
-        release(1);
-        DBG_T(1, it, 2);
-        // ---- GEMM2: two N = 128 chunks (W1 rows 0..127 / 128..255) into acc2 buffers 0 / 1
-        mbar_wait(BAR(B_X1), par);
-        tc_fence_after();
-        DBG_T(1, it, 3);
-#pragma unroll
-        for (int j = 0; j < 2; j++) {
-          wait_full(2 + j);
-          mbar_wait(BAR(B_ACC2E + j), par ^ 1u);
-          tc_fence_after();
-          mma_steps<8, false>(tmem + 128 + j * 128, dA, slot(2 + j), idesc128);
-          umma_commit(BAR(B_ACC2F + j));
-          release(2 + j);
-          DBG_T(1, it, 4 + j);
-        }
-        // ---- GEMM3: K chunks of 64 as the GELU groups deliver them (chunks 0,1 from group 0, 2,3 from group 1)
-#pragma unroll
-        for (int c = 0; c < 4; c++) {
-          if (c == 0) wait_full(4);
-          if (c == 2) wait_full(5);
-          mbar_wait(BAR(B_HIDF + (c >> 1)), (uint32_t)(c & 1));
-          tc_fence_after();
-          const u64 ad = dB0 + (u64)((c >> 1) * (16384 >> 4)), bd = slot(4 + (c >> 1)) + (u64)((c & 1) * (16384 >> 4));
-          if (c == 0) mma_steps<4, false>(tmem, ad, bd, idesc128);
-          else mma_steps<4, true>(tmem, ad, bd, idesc128);
-          umma_commit(BAR(B_HIDE + (c >> 1)));
-          if (c == 1) release(4);
-          if (c == 3) {
-            release(5);
-            umma_commit(BAR(B_ACC3));
-          }
-          DBG_T(1, it, 8 + c);
-        }
-        // ---- LN2 done: acc3 / x1 have been read, the y operand and the one-hot position columns are in C
-        mbar_wait(BAR(B_YFULL), par);
-        tc_fence_after();
-        DBG_T(1, it, 12);
-        if (!tail) mbar_arrive(BAR(B_CFREE));   // residual consumed and the LN2 statistics exchange (which lives in C) is over
-        if (tail) {
-          // q|k = (y + pos) . [Wq; Wk]^T = y . [Wq; Wk]^T + onehot(axis, coordinate) . (pos_table . [Wq; Wk]^T) as one N = 256 GEMM
-          // with K = 128 + 32 into TMEM [128, 384): B K-chunk kc is ring item 6 + kc, item 8 the tabulated positional term
-          wait_full(6);
-          wait_full(7);
-          wait_full(8);
-          mbar_wait(BAR(B_QKVE + 0), par ^ 1u);
-          tc_fence_after();
-          mma_steps<4, false>(tmem + 128, dC, slot(6), idesc256);
-          release(6);   // as early as possible: Wv (item 9) takes this slot and must land before the q|k GEMM retires
-          mma_steps<4, true>(tmem + 128, dC + 1024, slot(7), idesc256);
-          mma_steps<2, true>(tmem + 128, dC + (u64)(32768 >> 4), slot(8), idesc256);
-          umma_commit(BAR(B_QKVF + 0));
-          release(7);
-          release(8);
-          DBG_T(1, it, 13);
-          // v = y . Wv^T into TMEM [384, 512)
-          wait_full(9);
-          mbar_wait(BAR(B_QKVE + 1), par ^ 1u);
-          tc_fence_after();
-          mma_steps<8, false>(tmem + 384, dC, slot(9), idesc128);
-          umma_commit(BAR(B_QKVF + 1));
-          release(9);
-          umma_commit(BAR(B_CFREE));
-          DBG_T(1, it, 14);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == W_ST) {
-    // ================================================== TMA stores ==================================================
-    if (lane == 0) {
-      int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int row0 = tile * TM;
-        const uint32_t par = (uint32_t)(it & 1);
-        mbar_wait(BAR(B_YFULL), par);            // y staging (A | B) written and fenced by all epilogue warps
-        tma_store_2d(&maps.y, 0, row0, sbase + OFF_A);
-        tma_store_2d(&maps.y, 32, row0, sbase + OFF_A + 16384);
-        tma_store_commit();
-        tma_store_2d(&maps.y, 64, row0, sbase + OFF_B);
-        tma_store_2d(&maps.y, 96, row0, sbase + OFF_B + 16384);
-        tma_store_commit();
-        tma_store_wait_read<1>();
-        mbar_arrive(BAR(B_FREEA));               // y[:, 0:64] has left A
-        tma_store_wait_read<0>();
-        mbar_arrive(BAR(B_FREEB));               // y[:, 64:128] has left B
-        if (tail) {
-          mbar_wait(BAR(B_QST + 0), par);
-          tma_store_2d(&maps.qkv, 0, row0, sbase + OFF_A);
-          tma_store_2d(&maps.qkv, 64, row0, sbase + OFF_A + 16384);
-          tma_store_commit();
-          mbar_wait(BAR(B_QST + 1), par);
-          tma_store_2d(&maps.qkv, 128, row0, sbase + OFF_B);
-          tma_store_2d(&maps.qkv, 192, row0, sbase + OFF_B + 16384);
-          tma_store_commit();
-          tma_store_wait_read<1>();
-          mbar_arrive(BAR(B_FREEA));             // q has left A
-          mbar_wait(BAR(B_QST + 2), par);
-          tma_store_2d(&maps.qkv, 256, row0, sbase + OFF_A);
-          tma_store_2d(&maps.qkv, 320, row0, sbase + OFF_A + 16384);
-          tma_store_commit();
-          tma_store_wait_read<1>();
-          mbar_arrive(BAR(B_FREEB));             // k has left B
-          tma_store_wait_read<0>();
-          mbar_arrive(BAR(B_FREEA));             // v has left A
-        }
-      }
-      tma_store_wait_all<0>();
-    }
-    __syncwarp();
-  } else {
-    // ================================================ epilogue warps ================================================
-    const int qd = warp & 3, cq = warp >> 2;
-    const int lrow = qd * 32 + lane;                       // tile row == TMEM lane
-    const uint32_t tlane = tmem + ((uint32_t)(qd * 32) << 16);
-    const int c0 = cq * 32;                                // this thread's 32 columns of a 128-wide row
-    const uint32_t sw = (uint32_t)(lrow & 7);
-    uint8_t* const rowA = smem + OFF_A + lrow * 128;       // + box * 16384 + ((piece ^ sw) << 4)
-    uint8_t* const rowC = smem + OFF_C + lrow * 128;
-    // LN statistics exchange: each thread parks (sum, sumsq) in the first 8 bytes of its own (dead) residual span
-    float2* const stat_own = reinterpret_cast<float2*>(rowC + cq * 16384 + (sw << 4));
-    const int ge = cq >> 1, hf = cq & 1;                   // GELU group (owns acc2 / hidden buffer ge) and column half inside a chunk
-    int nA = 0, nB = 0;                                    // phases of FREEA / FREEB consumed so far
-    int it = 0;
-#define DBG_E(ev) do { if (tid == 0) DBG_T(0, it, ev); } while (0)
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const int row0 = tile * TM;
-      const uint32_t par = (uint32_t)(it & 1);
-      DBG_E(0);
-      u64 t2[16];   // the row slice as fp32 pairs: x + acc1 + bo, then x1, later y
-      float4 ga[8];
-      // ---------------- epilogue 1: x1 = LN1(x + acc1 + bo) -> fp32 in TMEM[256..384), fp16 operand in A ----------------
-      {
-        float4 b4[8];
-#pragma unroll
-        for (int q = 0; q < 8; q++) b4[q] = __ldg(reinterpret_cast<const float4*>(g.bo + c0) + q);
-        mbar_wait(BAR(B_XFULL), par);
-        DBG_E(1);
-        mbar_wait(BAR(B_ACC1), par);
-        tc_fence_after();
-        DBG_E(2);
-        uint32_t v[32];
-        tmem_ld32u(tlane + c0, v);
-        tmem_wait_ld();
-        u64 sum2 = 0ull, sq2 = 0ull;
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-          const float4 r4 = *reinterpret_cast<const float4*>(rowC + cq * 16384 + (((uint32_t)q ^ sw) << 4));
-          const u64 a = add2(add2(pk2u(v[4 * q], v[4 * q + 1]), pk2(b4[q].x, b4[q].y)), pk2(r4.x, r4.y));
-          const u64 b = add2(add2(pk2u(v[4 * q + 2], v[4 * q + 3]), pk2(b4[q].z, b4[q].w)), pk2(r4.z, r4.w));
-          t2[2 * q] = a;
-          t2[2 * q + 1] = b;
-          sum2 = add2(sum2, add2(a, b));
-          sq2 = fma2(a, a, sq2);
-          sq2 = fma2(b, b, sq2);
-        }
-        if (!BN) {
-          float s0, s1, q0, q1;
-          up2(sum2, s0, s1);
-          up2(sq2, q0, q1);
-          *stat_own = make_float2(s0 + s1, q0 + q1);
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < 8; q++) ga[q] = __ldg(reinterpret_cast<const float4*>(g.g1 + c0) + q);
-      if (!BN) named_bar_sync(2 + qd, 128);
-      DBG_E(3);
-      {
-        u64 rs2 = 0ull, nm2 = 0ull;
-        if (!BN) {
-          const float2 s0 = *reinterpret_cast<const float2*>(rowC + 0 * 16384 + (sw << 4));
-          const float2 s1 = *reinterpret_cast<const float2*>(rowC + 1 * 16384 + (sw << 4));
-          const float2 s2 = *reinterpret_cast<const float2*>(rowC + 2 * 16384 + (sw << 4));
-          const float2 s3 = *reinterpret_cast<const float2*>(rowC + 3 * 16384 + (sw << 4));
-          const float sum = (s0.x + s1.x) + (s2.x + s3.x), sq = (s0.y + s1.y) + (s2.y + s3.y);
-          const float mean = sum * (1.0f / D);
-          const float rstd = rsqrtf(fmaxf(sq * (1.0f / D) - mean * mean, 0.f) + g.eps);
-          rs2 = pk2(rstd, rstd), nm2 = pk2(-mean * rstd, -mean * rstd);
-        }
-        uint32_t xo[32];
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-          const float4 e4 = __ldg(reinterpret_cast<const float4*>(g.be1 + c0) + q);
-          // LayerNorm: ((t - mean) rstd) w + b; eval BatchNorm: t s + t0 with the folded per-channel scale / shift
-          const u64 a = fma2(BN ? t2[2 * q] : fma2(t2[2 * q], rs2, nm2), pk2(ga[q].x, ga[q].y), pk2(e4.x, e4.y));
-          const u64 b = fma2(BN ? t2[2 * q + 1] : fma2(t2[2 * q + 1], rs2, nm2), pk2(ga[q].z, ga[q].w), pk2(e4.z, e4.w));
-          t2[2 * q] = a;
-          t2[2 * q + 1] = b;
-          up2u(a, xo[4 * q], xo[4 * q + 1]);
-          up2u(b, xo[4 * q + 2], xo[4 * q + 3]);
-        }
-        tmem_st32u(tlane + 384 + c0, xo);   // fp32 x1 stays in TMEM for the second residual
-        if (it > 0) {                       // the previous tile's v chunk has left A
-          mbar_wait(BAR(B_FREEA), (uint32_t)(nA & 1));
-          nA++;
-        }
-        const int kc = cq >> 1, j0 = (cq & 1) * 4;
-#pragma unroll
-        for (int q = 0; q < 4; q++)
-          *reinterpret_cast<int4*>(rowA + kc * 16384 + (((uint32_t)(j0 + q) ^ sw) << 4)) =
-              make_int4((int)cvt_h2(t2[4 * q]), (int)cvt_h2(t2[4 * q + 1]), (int)cvt_h2(t2[4 * q + 2]), (int)cvt_h2(t2[4 * q + 3]));
-      }
-      fence_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(BAR(B_X1));
-      DBG_E(4);
-
-      // ---------------- epilogue 2: hidden K-chunk = GELU(acc2 + b1) -> fp16 K-chunk of GEMM3's A operand in B ----------------
-      // group ge owns accumulator chunk ge (hidden columns [128 ge, 128 ge + 128)) and hidden buffer ge: it delivers K-chunks
-      // 2 ge and 2 ge + 1 one after the other; a thread covers 32 of a K-chunk's 64 columns
-      if (it > 0) {   // the previous tile's k chunk has left B
-        mbar_wait(BAR(B_FREEB), (uint32_t)(nB & 1));
-        nB++;
-      }
-#pragma unroll 1
-      for (int u = 0; u < 2; u++) {
-        const int c = 2 * ge + u;
-        float4 b4[8];
-        const float4* bp = reinterpret_cast<const float4*>(g.b1 + c * 64 + hf * 32);
-#pragma unroll
-        for (int q = 0; q < 8; q++) b4[q] = __ldg(bp + q);
-        if (u == 0) {
-          mbar_wait(BAR(B_ACC2F + ge), par);
-          tc_fence_after();
-        }
-        DBG_E(5 + u);
-        uint32_t v[32];
-        tmem_ld32u(tlane + 128 + ge * 128 + u * 64 + hf * 32, v);
-        tmem_wait_ld();
-        if (u == 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(BAR(B_ACC2E + ge));
-        }
-        uint32_t pk[16];
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-          pk[2 * q] = gelu_h2(cvt_h2(add2(pk2u(v[4 * q], v[4 * q + 1]), pk2(b4[q].x, b4[q].y))));
-          pk[2 * q + 1] = gelu_h2(cvt_h2(add2(pk2u(v[4 * q + 2], v[4 * q + 3]), pk2(b4[q].z, b4[q].w))));
-        }
-        mbar_wait(BAR(B_HIDE + ge), (uint32_t)((u + 1) & 1));   // GEMM3 has consumed the chunk that lived in this buffer
-        uint8_t* hb = smem + OFF_B + ge * 16384 + lrow * 128;
-#pragma unroll
-        for (int q = 0; q < 4; q++)
-          *reinterpret_cast<int4*>(hb + (((uint32_t)(hf * 4 + q) ^ sw) << 4)) =
-              make_int4((int)pk[4 * q], (int)pk[4 * q + 1], (int)pk[4 * q + 2], (int)pk[4 * q + 3]);
-        fence_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(BAR(B_HIDF + ge));
-        DBG_E(7 + u);
-      }
-
-      // ---------------- epilogue 3: y = LN2(x1 + acc3 + b2) -> fp32 staging (TMA store) + operands of GEMM4 ----------------
-      int pcode = 0;
-      if (tail && row0 + lrow < M) pcode = g.next_pos_code[row0 + lrow];
-      {
-        float4 b4[8];
-#pragma unroll
-        for (int q = 0; q < 8; q++) b4[q] = __ldg(reinterpret_cast<const float4*>(g.b2 + c0) + q);
-        mbar_wait(BAR(B_ACC3), par);
-        tc_fence_after();
-        DBG_E(9);
-        uint32_t v[32], r[32];
-        tmem_ld32u(tlane + c0, v);
-        tmem_ld32u(tlane + 384 + c0, r);
-        tmem_wait_ld();
-        u64 sum2 = 0ull, sq2 = 0ull;
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-          const u64 a = add2(add2(pk2u(v[4 * q], v[4 * q + 1]), pk2(b4[q].x, b4[q].y)), pk2u(r[4 * q], r[4 * q + 1]));
-          const u64 b = add2(add2(pk2u(v[4 * q + 2], v[4 * q + 3]), pk2(b4[q].z, b4[q].w)), pk2u(r[4 * q + 2], r[4 * q + 3]));
-          t2[2 * q] = a;
-          t2[2 * q + 1] = b;
-          sum2 = add2(sum2, add2(a, b));
-          sq2 = fma2(a, a, sq2);
-          sq2 = fma2(b, b, sq2);
-        }
-        if (!BN) {
-          float s0, s1, q0, q1;
-          up2(sum2, s0, s1);
-          up2(sq2, q0, q1);
-          *stat_own = make_float2(s0 + s1, q0 + q1);
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < 8; q++) ga[q] = __ldg(reinterpret_cast<const float4*>(g.g2 + c0) + q);
-      if (!BN) named_bar_sync(2 + qd, 128);
-      DBG_E(10);
-      {
-        u64 rs2 = 0ull, nm2 = 0ull;
-        if (!BN) {
-          const float2 s0 = *reinterpret_cast<const float2*>(rowC + 0 * 16384 + (sw << 4));
-          const float2 s1 = *reinterpret_cast<const float2*>(rowC + 1 * 16384 + (sw << 4));
-          const float2 s2 = *reinterpret_cast<const float2*>(rowC + 2 * 16384 + (sw << 4));
-          const float2 s3 = *reinterpret_cast<const float2*>(rowC + 3 * 16384 + (sw << 4));
-          const float sum = (s0.x + s1.x) + (s2.x + s3.x), sq = (s0.y + s1.y) + (s2.y + s3.y);
-          const float mean = sum * (1.0f / D);
-          const float rstd = rsqrtf(fmaxf(sq * (1.0f / D) - mean * mean, 0.f) + g.eps);
-          rs2 = pk2(rstd, rstd), nm2 = pk2(-mean * rstd, -mean * rstd);
-          named_bar_sync(2 + qd, 128);   // every statistic of this quadrant has been read: C may now receive the operands
-        }
-        // (global loads are kept out of the loops that store to shared memory: the compiler will not move them across the stores)
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-          const float4 e4 = __ldg(reinterpret_cast<const float4*>(g.be2 + c0) + q);
-          t2[2 * q] = fma2(BN ? t2[2 * q] : fma2(t2[2 * q], rs2, nm2), pk2(ga[q].x, ga[q].y), pk2(e4.x, e4.y));
-          t2[2 * q + 1] = fma2(BN ? t2[2 * q + 1] : fma2(t2[2 * q + 1], rs2, nm2), pk2(ga[q].z, ga[q].w), pk2(e4.z, e4.w));
-        }
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-          uint4 o;
-          up2u(t2[2 * q], o.x, o.y);
-          up2u(t2[2 * q + 1], o.z, o.w);
-          *reinterpret_cast<uint4*>(rowA + cq * 16384 + (((uint32_t)q ^ sw) << 4)) = o;   // y staging spans A | B (4 boxes of 32 columns)
-        }
-      }
-      DBG_E(11);
-      if (tail) {
-        // operands of GEMM4: y as fp16 (K chunks 0, 1 of C) and this row's one-hot position columns (third K chunk, 32 columns:
-        // column axis * maxw + coordinate is 1) - the positional embedding enters q|k through the tensor core, not through a gather
-        const int kc = cq >> 1, j0 = (cq & 1) * 4;
-#pragma unroll
-        for (int q = 0; q < 4; q++)
-          *reinterpret_cast<int4*>(rowC + kc * 16384 + (((uint32_t)(j0 + q) ^ sw) << 4)) =
-              make_int4((int)cvt_h2(t2[4 * q]), (int)cvt_h2(t2[4 * q + 1]), (int)cvt_h2(t2[4 * q + 2]), (int)cvt_h2(t2[4 * q + 3]));
-        uint32_t oh[4] = {0u, 0u, 0u, 0u};
-        if (row0 + lrow < M) {
-#pragma unroll
-          for (int a = 0; a < 3; a++) {
-            const int rel = a * g.pos_maxw + ((pcode >> (8 * a)) & 255) - 8 * cq;   // position inside this thread's 8 columns
-            if (a < g.pos_ndim && rel >= 0 && rel < 8) {
-              const uint32_t one = 0x3C00u << ((rel & 1) << 4);
-#pragma unroll
-              for (int w = 0; w < 4; w++) oh[w] |= (rel >> 1) == w ? one : 0u;
-            }
-          }
-        }
-        *reinterpret_cast<int4*>(rowC + 32768 + (((uint32_t)cq ^ sw) << 4)) = make_int4((int)oh[0], (int)oh[1], (int)oh[2], (int)oh[3]);
-      }
-      fence_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(BAR(B_YFULL));
-      DBG_E(12);
-
-      // ---------------- epilogue 4: q | k | v + bias -> fp16 staging (q, v in A; k in B) -> TMA store (warp 18) ----------------
-      if (tail) {
-#pragma unroll 1
-        for (int nt = 0; nt < 3; nt++) {
-          float4 b4[8];
-          const float4* bp = reinterpret_cast<const float4*>(g.bqkv + nt * 128 + c0);
-#pragma unroll
-          for (int q = 0; q < 8; q++) b4[q] = __ldg(bp + q);
-          if (nt != 1) {   // q|k retire together (one N = 256 GEMM), v on its own
-            mbar_wait(BAR(B_QKVF + (nt >> 1)), par);
-            tc_fence_after();
-          }
-          DBG_E(13 + nt);
-          uint32_t v[32];
-          tmem_ld32u(tlane + 128 + nt * 128 + c0, v);
-          tmem_wait_ld();
-          if (nt != 0) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(BAR(B_QKVE + (nt >> 1)));
-          }
-          uint32_t pk[16];
-#pragma unroll
-          for (int q = 0; q < 8; q++) {
-            pk[2 * q] = cvt_h2(add2(pk2u(v[4 * q], v[4 * q + 1]), pk2(b4[q].x, b4[q].y)));
-            pk[2 * q + 1] = cvt_h2(add2(pk2u(v[4 * q + 2], v[4 * q + 3]), pk2(b4[q].z, b4[q].w)));
-          }
-          // the store that last read this staging buffer has drained it
-          if (nt == 1) {
-            mbar_wait(BAR(B_FREEB), (uint32_t)(nB & 1));
-            nB++;
-          } else {
-            mbar_wait(BAR(B_FREEA), (uint32_t)(nA & 1));
-            nA++;
-          }
-          uint8_t* st = smem + (nt == 1 ? OFF_B : OFF_A) + (cq >> 1) * 16384 + lrow * 128;
-          const int j0 = (cq & 1) * 4;
-#pragma unroll
-          for (int q = 0; q < 4; q++)
-            *reinterpret_cast<int4*>(st + (((uint32_t)(j0 + q) ^ sw) << 4)) =
-                make_int4((int)pk[4 * q], (int)pk[4 * q + 1], (int)pk[4 * q + 2], (int)pk[4 * q + 3]);
-          fence_async_smem();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(BAR(B_QST + nt));
-          DBG_E(16 + nt);
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) tmem_dealloc(tmem, 512);
-#undef BAR
+__device__ __forceinline__ float2 pos_pair(const Chain2Args& g, int code, int c) {
+  const int axis = c / g.posL;   // posL % 32 == 0: the pair lies inside one axis
+  if (axis >= g.pos_ndim) return make_float2(0.f, 0.f);
+  const int cv = (code >> (8 * axis)) & 255;
+  return __ldg(reinterpret_cast<const float2*>(g.pos_tab + ((size_t)axis * g.pos_maxw + cv) * g.posL + (c - axis * g.posL)));
 }
 
-// pos_qk[l][n][axis * maxw + coordinate] = sum_j Wqk_l[n][axis * L + j] * pos_table[axis][coordinate][j]  (n < 256: q and k rows of
-// in_proj; fp32 accumulation, fp16 result, columns >= ndim * maxw zero): the B operand of the one-hot K chunk in the chain's q|k
-// GEMM.  32 blocks per layer; recomputed every frame (0.4 MFLOP per layer) so that in-place weight updates are always seen.
-struct PosQkArgs {
-  const __half* w[SSTB_MAX_STACK];   // in_proj weights [384][128] fp16 per layer
-  int num_layers;
-};
-__global__ void __launch_bounds__(256) pos_qk_kernel(PosQkArgs a, const float* __restrict__ pos_tab, int L, int maxw, int ndim,
-                                                       __half* __restrict__ out) {
+template <bool TAIL>
+__global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_constant__ Chain2Maps m, const Chain2Args g) {
   pdl_wait();
   pdl_launch();
-  // block = 8 of a layer's 256 rows (one per warp); lane = output column (axis, coordinate); table transposed in shared memory
-  __shared__ float sT[128][33];      // [j][column], j < L <= 128
-  __shared__ __half sW[8][128];
-  const int l = blockIdx.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n = (blockIdx.x & 31) * 8 + warp;
-  const int ncol = ndim * maxw;      // <= 32 (host check)
-  for (int i = threadIdx.x; i < 128 * 32; i += 256) {
-    const int j = i >> 5, col = i & 31;
-    sT[j][col] = (col < ncol && j < L) ? pos_tab[(size_t)col * L + j] : 0.f;   // pos_tab is [axis][coordinate][L] = [column][L]
+  extern __shared__ uint8_t chain_raw[];
+  uint8_t* base = (uint8_t*)(((uintptr_t)chain_raw + 1023) & ~(uintptr_t)1023);
+  uint8_t* pA = base + OFF_A;
+  uint8_t* pP = base + OFF_P;
+  uint8_t* pH = base + OFF_H;
+  const uint32_t sA = smem_u32(pA), sP = smem_u32(pP), sH = smem_u32(pH), sR = smem_u32(base + OFF_RING);
+  __shared__ __align__(8) uint64_t bar_full[2], bar_att;
+  constexpr int NCH = TAIL ? 8 : 5;
+
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
+  const int M = g.M_dev ? *g.M_dev : g.M_cap;
+  const int ntiles = (M + TM - 1) / TM;
+  if ((int)blockIdx.x >= ntiles) return;   // uniform per CTA, nothing issued yet
+  // chunk `n` (counted over the CTA's whole tile sequence) belongs to a tile this CTA will process
+  auto chunk_live = [&](int n) { return (int)blockIdx.x + (n / NCH) * (int)gridDim.x < ntiles; };
+  if (tid == 0) {
+    mbar_init(smem_u32(&bar_full[0]), 1);
+    mbar_init(smem_u32(&bar_full[1]), 1);
+    mbar_init(smem_u32(&bar_att), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    for (int n = 0; n < 2; n++)
+      if (chunk_live(n)) issue_chunk(m, n % NCH, sR + n * SLOT, smem_u32(&bar_full[n]));
   }
-  reinterpret_cast<uint2*>(sW[warp])[lane] = reinterpret_cast<const uint2*>(a.w[l] + (size_t)n * 128)[lane];
   __syncthreads();
-  const int axis = min(lane / maxw, ndim - 1);
-  float acc = 0.f;
-  if ((axis + 1) * L <= 128)
-    for (int j = 0; j < L; j++) acc = fmaf(__half2float(sW[warp][axis * L + j]), sT[j][lane], acc);
-  __half* o = out + ((size_t)l * 256 + n) * 64;
-  o[lane] = __float2half_rn(lane < ncol ? acc : 0.f);
-  o[32 + lane] = __float2half_rn(0.f);
+
+  int gc = 0;   // weight chunks consumed
+  auto wait_chunk = [&]() -> uint32_t {
+    mbar_wait(smem_u32(&bar_full[gc & 1]), (uint32_t)((gc >> 1) & 1));
+    return sR + (gc & 1) * SLOT;
+  };
+  // after wgmma_wait<0> in every thread: the slot is free once all threads pass the barrier; refill it with the chunk two ahead
+  auto release_chunk = [&]() {
+    __syncthreads();
+    if (tid == 0 && chunk_live(gc + 2)) issue_chunk(m, (gc + 2) % NCH, sR + (gc & 1) * SLOT, smem_u32(&bar_full[gc & 1]));
+    gc++;
+  };
+
+  const int rl = 64 * wg + 16 * ((tid >> 5) & 3) + (lane >> 2);   // fragment rows rl, rl + 8 of the tile
+  const int cq = 2 * (lane & 3);
+  uint32_t att_par = 0;
+  float acc[64], x1[64];
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int row0 = tile * TM;
+    const int rowA = row0 + rl, rowB = rowA + 8;
+    const bool okA = rowA < M, okB = rowB < M;
+    fence_async_smem();   // the previous tile's generic-proxy writes of A precede the TMA that overwrites it
+    __syncthreads();
+    if (tid == 0) {
+      mbar_expect_tx(smem_u32(&bar_att), SLOT);
+      tma_load_2d(sA, &m.att, 0, row0, smem_u32(&bar_att));
+      tma_load_2d(sA + SLOT / 2, &m.att, 64, row0, smem_u32(&bar_att));
+    }
+    mbar_wait(smem_u32(&bar_att), att_par);
+    att_par ^= 1u;
+
+    // ---- GEMM1 + bias + residual + Norm1 -> x1 (registers, and fp16 into A) -----------------------------------------------------
+    wg_tile_mma<128, false, 8>(acc, sA + wg * 64 * 128, OPB, wait_chunk(), OPB, false);
+    wgmma_wait<0>();
+    release_chunk();   // also: both warpgroups are done with att in A
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+      const int c = 8 * j + cq;
+      const float2 b = __ldg(reinterpret_cast<const float2*>(g.bo + c));
+      const float2 ra = okA ? *reinterpret_cast<const float2*>(g.x + (size_t)rowA * D + c) : make_float2(0.f, 0.f);
+      const float2 rb = okB ? *reinterpret_cast<const float2*>(g.x + (size_t)rowB * D + c) : make_float2(0.f, 0.f);
+      x1[4 * j] = acc[4 * j] + b.x + ra.x;
+      x1[4 * j + 1] = acc[4 * j + 1] + b.y + ra.y;
+      x1[4 * j + 2] = acc[4 * j + 2] + b.x + rb.x;
+      x1[4 * j + 3] = acc[4 * j + 3] + b.y + rb.y;
+    }
+    row_norm(x1, g.g1, g.be1, g.eps, g.affine);
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+      const int c = 8 * j + cq;
+      st_op(pA, rl, c, pack_f16(x1[4 * j], x1[4 * j + 1]));
+      st_op(pA, rl + 8, c, pack_f16(x1[4 * j + 2], x1[4 * j + 3]));
+    }
+    fence_async_smem();
+    __syncthreads();
+
+    // ---- GEMM2 + bias + GELU -> h (fp16 into H) -----------------------------------------------------------------------------------
+#pragma unroll 1
+    for (int h = 0; h < 2; h++) {
+      wg_tile_mma<128, false, 8>(acc, sA + wg * 64 * 128, OPB, wait_chunk(), OPB, false);
+      wgmma_wait<0>();
+      release_chunk();
+#pragma unroll
+      for (int j = 0; j < 16; j++) {
+        const int c = 8 * j + cq;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(g.b1 + 128 * h + c));
+        st_op(pH, rl, 128 * h + c, pack_f16(gelu_fast(acc[4 * j] + b.x), gelu_fast(acc[4 * j + 1] + b.y)));
+        st_op(pH, rl + 8, 128 * h + c, pack_f16(gelu_fast(acc[4 * j + 2] + b.x), gelu_fast(acc[4 * j + 3] + b.y)));
+      }
+    }
+    fence_async_smem();
+    __syncthreads();
+
+    // ---- GEMM3 + bias + x1 + Norm2 -> y (fp32 rows; fp16 y and y + pos into A / P for the tail) -----------------------------------
+#pragma unroll 1
+    for (int kc = 0; kc < 2; kc++) {
+      wg_tile_mma<128, false, 8>(acc, sH + kc * 2 * OPB + wg * 64 * 128, OPB, wait_chunk(), OPB, kc > 0);
+      wgmma_wait<0>();
+      release_chunk();
+    }
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+      const int c = 8 * j + cq;
+      const float2 b = __ldg(reinterpret_cast<const float2*>(g.b2 + c));
+      acc[4 * j] += b.x + x1[4 * j];
+      acc[4 * j + 1] += b.y + x1[4 * j + 1];
+      acc[4 * j + 2] += b.x + x1[4 * j + 2];
+      acc[4 * j + 3] += b.y + x1[4 * j + 3];
+    }
+    row_norm(acc, g.g2, g.be2, g.eps, g.affine);
+    int codeA = 0, codeB = 0;
+    if (TAIL) {
+      codeA = okA ? g.pos_code[rowA] : 0;
+      codeB = okB ? g.pos_code[rowB] : 0;
+    }
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+      const int c = 8 * j + cq;
+      if (okA) *reinterpret_cast<float2*>(g.y + (size_t)rowA * D + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      if (okB) *reinterpret_cast<float2*>(g.y + (size_t)rowB * D + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      if (TAIL) {
+        st_op(pA, rl, c, pack_f16(acc[4 * j], acc[4 * j + 1]));
+        st_op(pA, rl + 8, c, pack_f16(acc[4 * j + 2], acc[4 * j + 3]));
+        const float2 pa = pos_pair(g, codeA, c), pb = pos_pair(g, codeB, c);
+        st_op(pP, rl, c, pack_f16(acc[4 * j] + pa.x, acc[4 * j + 1] + pa.y));
+        st_op(pP, rl + 8, c, pack_f16(acc[4 * j + 2] + pb.x, acc[4 * j + 3] + pb.y));
+      }
+    }
+    if (!TAIL) continue;
+    fence_async_smem();
+    __syncthreads();
+
+    // ---- GEMM4: next layer's q|k (from y + pos) and v (from y) + bias -> fp16 rows ------------------------------------------------
+#pragma unroll 1
+    for (int q = 0; q < 3; q++) {
+      wg_tile_mma<128, false, 8>(acc, (q < 2 ? sP : sA) + wg * 64 * 128, OPB, wait_chunk(), OPB, false);
+      wgmma_wait<0>();
+      release_chunk();
+#pragma unroll
+      for (int j = 0; j < 16; j++) {
+        const int c = 8 * j + cq;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(g.bqkv + 128 * q + c));
+        if (okA) *reinterpret_cast<uint32_t*>(g.qkv + (size_t)rowA * 3 * D + 128 * q + c) = pack_f16(acc[4 * j] + b.x, acc[4 * j + 1] + b.y);
+        if (okB) *reinterpret_cast<uint32_t*>(g.qkv + (size_t)rowB * 3 * D + 128 * q + c) = pack_f16(acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y);
+      }
+    }
+  }
 }
 
 // eval-mode BatchNorm of layer_cfg use_bn folded to y = x s + t per channel: out[l][4][128] = {s1, t1, s2, t2}
@@ -751,17 +289,6 @@ __global__ void __launch_bounds__(128) bn_fold_kernel(BnFoldArgs a, float* __res
 
 }  // namespace
 
-int sstb_sra_pos_qk(sstb200_ctx* c, const sstb200_sra_layer* layers, int num_layers, const sstb200_sra_plan* plan, __half* out) {
-  if (num_layers > SSTB_MAX_STACK) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "encoder stacks deeper than %d layers are not built", SSTB_MAX_STACK);
-  PosQkArgs a;
-  memset(&a, 0, sizeof(a));
-  a.num_layers = num_layers;
-  for (int l = 0; l < num_layers; l++) a.w[l] = reinterpret_cast<const __half*>(layers[l].in_proj_w_f16);
-  CUDA_TRY(c, launch_pdl(pos_qk_kernel, dim3(num_layers * 32), dim3(256), (size_t)0, c->stream, a, (const float*)plan->pos_table, plan->pos_L, plan->pos_maxw,
-                         plan->pos_ndim, out));
-  return SSTB_OK;
-}
-
 int sstb_sra_bn_fold(sstb200_ctx* c, const sstb200_sra_layer* layers, int num_layers, float* out) {
   for (int l0 = 0; l0 < num_layers; l0 += 8) {
     BnFoldArgs a;
@@ -779,35 +306,33 @@ int sstb_sra_bn_fold(sstb200_ctx* c, const sstb200_sra_layer* layers, int num_la
 }
 
 int sstb_sra_chain2(sstb200_ctx* c, const sstb200_sra_layer* L, const __half* att, const float* x, float* y, int n_cap, const int32_t* n_dev,
-                    const sstb200_sra_layer* next, const sstb200_sra_plan* next_plan, void* next_qkv, const __half* next_pos_qk,
-                    const float* bn_fold) {
+                    const sstb200_sra_layer* next, const sstb200_sra_plan* next_plan, void* next_qkv, const float* bn_fold) {
   Chain2Maps maps;
   Chain2Args g;
   memset(&g, 0, sizeof(g));
   memset(&maps, 0, sizeof(maps));
   const bool tail = next && next_plan && next_qkv;
-  if (tail && (!next_pos_qk || !next_plan->pos_code || next_plan->pos_ndim < 1 || next_plan->pos_ndim > 3 ||
-               next_plan->pos_ndim * next_plan->pos_maxw > 32))
-    return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "fused QKV tail needs the next plan's pos_code and ndim * max window extent <= 32");
+  if (tail && (!next_plan->pos_table || !next_plan->pos_code || next_plan->pos_L % 32 != 0 || next_plan->pos_ndim < 1 ||
+               next_plan->pos_ndim > 3))
+    return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "fused QKV tail needs the next plan's positional table with a per-axis length that is a multiple of 32");
   int rc = 0;
   rc |= tmap_2d_sw128(&maps.att, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, att, 128, (uint64_t)n_cap, 256, 64, 128);
-  rc |= tmap_2d_sw128(&maps.x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, 128, (uint64_t)n_cap, 512, 32, 128);
-  rc |= tmap_2d_sw128(&maps.y, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, y, 128, (uint64_t)n_cap, 512, 32, 128);
   rc |= tmap_2d_sw128(&maps.wo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L->out_proj_w_f16, 128, 128, 256, 64, 128);
   rc |= tmap_2d_sw128(&maps.w1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L->lin1_w_f16, 128, 256, 256, 64, 128);
   rc |= tmap_2d_sw128(&maps.w2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L->lin2_w_f16, 256, 128, 512, 64, 128);
   if (tail) {
     rc |= tmap_2d_sw128(&maps.wqkv, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, next->in_proj_w_f16, 128, 384, 256, 64, 128);
-    rc |= tmap_2d_sw128(&maps.wqk, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, next->in_proj_w_f16, 128, 256, 256, 64, 256);
-    rc |= tmap_2d_sw128(&maps.wpos, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, next_pos_qk, 64, 256, 128, 64, 256);
-    rc |= tmap_2d_sw128(&maps.qkv, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, next_qkv, 384, (uint64_t)n_cap, 768, 64, 128);
-    g.has_tail = 1;
+    g.qkv = reinterpret_cast<__half*>(next_qkv);
     g.bqkv = next->in_proj_b;
-    g.next_pos_code = next_plan->pos_code;
+    g.pos_tab = next_plan->pos_table;
+    g.pos_code = next_plan->pos_code;
+    g.posL = next_plan->pos_L;
     g.pos_maxw = next_plan->pos_maxw;
     g.pos_ndim = next_plan->pos_ndim;
   }
   if (rc) return sstb_fail(c, SSTB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d): operands must be 16-byte aligned", rc);
+  g.x = x;
+  g.y = y;
   g.bo = L->out_proj_b;
   g.b1 = L->lin1_b;
   g.b2 = L->lin2_b;
@@ -817,46 +342,15 @@ int sstb_sra_chain2(sstb200_ctx* c, const sstb200_sra_layer* L, const __half* at
   g.be1 = bn ? bn_fold + 128 : L->norm1_b;
   g.g2 = bn ? bn_fold + 256 : L->norm2_w;
   g.be2 = bn ? bn_fold + 384 : L->norm2_b;
+  g.affine = bn;
   g.eps = L->norm_eps;
   g.M_cap = n_cap;
   g.M_dev = n_dev;
-  static SmemAttr sa[4];
-  void (*kern)(const Chain2Maps, const Chain2Args) = tail ? (bn ? sra_chain2_kernel<true, true> : sra_chain2_kernel<true, false>)
-                                                          : (bn ? sra_chain2_kernel<false, true> : sra_chain2_kernel<false, false>);
-  CUDA_TRY(c, ensure_smem(c, sa[(tail ? 2 : 0) + (bn ? 1 : 0)], kern, (size_t)SMEM_BYTES));
+  static SmemAttr sa[2];
+  void (*kern)(const Chain2Maps, const Chain2Args) = tail ? sra_chain2_kernel<true> : sra_chain2_kernel<false>;
+  CUDA_TRY(c, ensure_smem(c, sa[tail ? 1 : 0], kern, (size_t)SMEM_BYTES));
   const int tiles_cap = (n_cap + TM - 1) / TM;
   const int grid = c->num_sms < tiles_cap ? c->num_sms : tiles_cap;
-  static int dbg_on = -1;
-  if (dbg_on < 0) dbg_on = getenv("SSTB200_CHAIN_DBG") ? atoi(getenv("SSTB200_CHAIN_DBG")) : 0;
-  static long long* dbg_buf = nullptr;
-  const size_t dbg_n = (size_t)grid * 3 * 2 * 32;
-  if (dbg_on) {   // timeline dump of CTA 0 and one mid CTA (profiling aid; synchronises)
-    if (!dbg_buf) CUDA_TRY(c, cudaMalloc(&dbg_buf, (size_t)1024 * 3 * 2 * 32 * 8));
-    CUDA_TRY(c, cudaMemsetAsync(dbg_buf, 0, dbg_n * 8, c->stream));
-    g.dbg = dbg_buf;
-  }
   CUDA_TRY(c, launch_pdl(kern, dim3(grid), dim3(NTHR), (size_t)SMEM_BYTES, c->stream, maps, g));
-  if (dbg_on) {
-    std::vector<long long> h(dbg_n);
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    CUDA_TRY(c, cudaMemcpy(h.data(), dbg_buf, dbg_n * 8, cudaMemcpyDeviceToHost));
-    static int dumps = 0;
-    if (dumps++ % dbg_on == 0) {
-      const char* roles[3] = {"epi", "mma", "tma"};
-      for (int cta : {0, grid / 2}) {
-        long long t0 = h[(((size_t)cta * 3 + 2) * 2 + 0) * 32 + 0];
-        for (int role = 0; role < 3; role++)
-          for (int it = 0; it < 2; it++) {
-            printf("[chain2 dbg] cta %3d %s tile %d:", cta, roles[role], it);
-            for (int e = 0; e < 22; e++) {
-              long long v = h[(((size_t)cta * 3 + role) * 2 + it) * 32 + e];
-              printf(" %d:%lld", e, v ? v - t0 : -1);
-            }
-            printf("\n");
-          }
-      }
-      fflush(stdout);
-    }
-  }
   return SSTB_OK;
 }

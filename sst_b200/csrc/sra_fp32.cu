@@ -192,7 +192,7 @@ void sstb_add_norm(cudaStream_t st, const float* a, const float* b, const float*
 
 // ------------------------------------------------------------------------------------------------
 // fp32-tolerance GEMMs on the tensor core (SSTB200_FP32_TC, default on): every Linear of the layer runs through sstb_gemm_rows_x3
-// (split-fp16 operands: hi.hi + lo.hi + hi.lo in one fp32 TMEM accumulator, ~2^-22 relative) instead of the FFMA kernel above; the
+// (split-fp16 operands: hi.hi + lo.hi + hi.lo in one set of fp32 accumulators, ~2^-22 relative) instead of the FFMA kernel above; the
 // positional term of q|k is added to a copy of the input first.  Shapes that do not fit fall back to the FFMA kernel.
 // ------------------------------------------------------------------------------------------------
 static int fp32_tc_enabled() {

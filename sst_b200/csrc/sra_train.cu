@@ -8,13 +8,13 @@
 // operands and saved activations are bf16 (gradients need the fp32 exponent range, so no loss scaling), accumulation, softmax,
 // LayerNorm, residual stream, weight gradients and the optimizer state are fp32.
 //
-// Per layer, forward:   qkv = [x+pos | x] Wqkv^T        tcgen05 GEMM (csrc/umma_gemm.cuh), q|k|v fp16 for the attention kernel
+// Per layer, forward:   qkv = [x+pos | x] Wqkv^T        wgmma GEMM (csrc/umma_gemm.cuh)  , q|k|v fp16 for the attention kernel
 //                       att = windowed softmax(q k^T) v  csrc/sra_attn.cuh (bf16 output)
-//                       x1 = LN1(x + att Wo^T + bo)      tcgen05 GEMM + LN epilogue, keeps t1 = pre-LN sum
-//                       h  = GELU(z), z = x1 W1^T + b1   tcgen05 GEMM, keeps z
-//                       y  = LN2(x1 + h W2^T + b2)       tcgen05 GEMM + LN epilogue, keeps t2
+//                       x1 = LN1(x + att Wo^T + bo)      wgmma GEMM + LN epilogue, keeps t1   = pre-LN sum
+//                       h  = GELU(z), z = x1 W1^T + b1   wgmma GEMM, keeps z  
+//                       y  = LN2(x1 + h W2^T + b2)       wgmma GEMM + LN epilogue, keeps t2  
 // backward:  LN2' -> dW2, dz = (dt2 W2) * gelu'(z) -> dW1, dx1 = dt2 + dz W1 -> LN1' -> dWo, datt = dt1 Wo -> attention' ->
-//            dWqkv, dx = dt1 + dqkv Wqkv.  dX-type GEMMs run on tcgen05 (transposed bf16 weight copies), dW-type GEMMs (reduction
+//            dWqkv, dx = dt1 + dqkv Wqkv.  dX-type GEMMs run on wgmma (transposed bf16 weight copies), dW-type GEMMs (reduction
 //            over the ~30 k tokens) on mma.sync tiles (per-split partial blocks + a deterministic reduce), attention' as a two-pass SIMT kernel per window batch.
 #include <stdarg.h>
 #include <cuda_fp16.h>

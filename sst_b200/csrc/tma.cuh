@@ -1,7 +1,7 @@
 // TMA (cp.async.bulk.tensor) + mbarrier helpers: host-side tensor-map encoding and the device-side PTX wrappers.
 //   SASS evidence: cp.async.bulk.tensor loads -> UTMALDG, stores -> UTMASTG, expect_tx -> SYNCS.ARRIVE.TRANS64.
 // Every tile that crosses the HBM/L2 <-> shared-memory boundary of the tensor-core kernels is one of these bulk copies,
-// landing in (or leaving from) the 128-byte-swizzled layout the UMMA descriptors read, so no thread spends
+// landing in (or leaving from) the 128-byte-swizzled layout the wgmma descriptors read, so no thread spends
 // instructions on address arithmetic for operand staging.
 #pragma once
 #include <cuda.h>

@@ -1,7 +1,7 @@
-// Generic tcgen05 GEMM tile kernel shared by the SRA forward (csrc/sra_bf16.cu) and the training path (csrc/sra_train.cu):
-//     C[128-row tile, NT] = A[128, K] . W[NT, K]^T      (whole K staged once, K <= 384; accumulators in TMEM)
+// Generic wgmma GEMM tile kernel shared by the SRA forward (csrc/sra_bf16.cu) and the training path (csrc/sra_train.cu):
+//     C[128-row tile, NT] = A[128, K] . W[NT, K]^T      (whole K staged once, K <= 384; fp32 accumulators)
 // A-operand prologues: plain 16-bit rows, or fp32 rows (+ positional embedding from the per-axis table) converted on the fly.
-// Epilogues (thread per row out of TMEM, then coalesced through an XOR-swizzled staging tile):
+// Epilogues (thread per row out of the shared-memory accumulator tile, then coalesced through an XOR-swizzled staging tile):
 //     EPI_H16 / EPI_F16  + bias, store 16-bit (operand format / always fp16)
 //     EPI_H16_GELU       + bias, GELU, store 16-bit (optionally also the pre-activation, for the backward pass)
 //     EPI_RES_LN         + bias + fp32 residual, LayerNorm, store fp32 (+ 16-bit copy, + the pre-LayerNorm sum)
@@ -83,9 +83,10 @@ struct GemmArgs {
 constexpr int TILE_M = 128;
 
 // Persistent over (row tile, n tile) items.  Per item: stage W and A (16-byte chunks, 8 loads in flight per thread) in
-// the K-major SWIZZLE_128B layout -> one thread issues the MMAs -> commit/mbarrier -> epilogue.  The epilogue goes through
-// shared memory (the operand buffers are free once the MMA has completed) so that every global access is a coalesced row
-// segment: thread-per-row TMEM reads meet warp-per-row global traffic in an XOR-swizzled staging tile.
+// the K-major SWIZZLE_128B layout -> each of the two warpgroups runs the wgmma chain of its 64 rows -> the register fragments
+// go to a shared-memory accumulator tile -> epilogue.  The epilogue goes through shared memory (the operand buffers are free
+// once the MMAs have completed) so that every global access is a coalesced row segment: thread-per-row accumulator reads
+// meet warp-per-row global traffic in an XOR-swizzled staging tile.
 template <int K, int NT, int PRO, int EPI, int FMT>
 __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
   pdl_wait();
@@ -95,25 +96,18 @@ __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
   uint8_t* sA = base;                           // K/64 chunks x 128 rows x 128 B
   uint8_t* sW = sA + (size_t)TILE_M * K * 2;    // K/64 chunks x NT rows x 128 B
   uint8_t* sE = base;                           // epilogue staging (aliases the operands)
-  __shared__ __align__(8) uint64_t mbar;
-  __shared__ uint32_t tmem_slot;
+  constexpr int STAGE = (EPI == EPI_RES_LN || EPI == EPI_ADD_F32) ? TILE_M * NT * 4 : TILE_M * NT * 2;
+  float* sAcc = reinterpret_cast<float*>(base + STAGE);   // [128][NT] fp32 accumulators (aliases the operands, not the staging)
   __shared__ float red[2][TILE_M][2];
   __shared__ int sRow[TILE_M];
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int M = g.M_dev ? *g.M_dev : g.M_cap;
   const int n_items = ((M + TILE_M - 1) / TILE_M) * g.ny;
-  if ((int)blockIdx.x >= n_items) return;  // uniform per CTA: nothing allocated yet
+  if ((int)blockIdx.x >= n_items) return;  // uniform per CTA
 
-  if (warp == 0) tmem_alloc(&tmem_slot, NT);
-  if (tid == 0) {
-    mbar_init(smem_u32(&mbar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
   constexpr int CH = K / 8;  // 16-byte chunks per operand row
   constexpr int NTH = 256, UNR = 8;
-  uint32_t parity = 0;
-  uint32_t tmem = 0;
   for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
     const int ytile = item % g.ny;
     const int row0 = (item / g.ny) * TILE_M;
@@ -212,37 +206,24 @@ __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
         }
       }
     }
-    // generic-proxy smem writes -> visible to the tensor core (async proxy); TMEM address visible to all
+    // generic-proxy smem writes -> visible to the tensor core (async proxy)
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    tmem = tmem_slot;
 
-    // ---- MMA issue: one thread ------------------------------------------------------------------------------------------
-    if (tid == 0) {
-      const uint32_t idesc = FMT == FMT_BF16 ? umma_idesc(TILE_M, NT) : umma_idesc_f16(TILE_M, NT);
-      const uint32_t a0 = smem_u32(sA), w0 = smem_u32(sW);
-#pragma unroll
-      for (int c = 0; c < K / 64; c++) {
-#pragma unroll
-        for (int s = 0; s < 4; s++) {
-          uint64_t ad = umma_desc_sw128(a0 + c * TILE_M * 128 + s * 32);
-          uint64_t bd = umma_desc_sw128(w0 + c * NT * 128 + s * 32);
-          umma_f16(tmem, ad, bd, idesc, (c | s) ? 1u : 0u);
-        }
-      }
-      umma_commit(smem_u32(&mbar));  // implicit tcgen05.fence::before_thread_sync
+    // ---- MMA: warpgroup g computes rows [64 g, 64 g + 64) x NT ------------------------------------------------------------
+    {
+      const int wg = tid >> 7;
+      float acc[NT / 2];
+      wg_tile_mma<NT, FMT == FMT_BF16, K / 16>(acc, smem_u32(sA) + wg * 64 * 128, TILE_M * 128, smem_u32(sW), NT * 128, false);
+      wgmma_wait<0>();
+      __syncthreads();   // both warpgroups are done reading the operands the accumulator tile aliases
+      wg_store_acc<NT>(acc, sAcc, NT, wg * 64, 0);
+      __syncthreads();
     }
-    __syncwarp();
-    mbar_wait(smem_u32(&mbar), parity);
-    parity ^= 1u;
-    tc_fence_after();
 
     // ---- epilogue ----------------------------------------------------------------------------------------------------------
     const int half = warp >> 2;                      // warps 0-3: columns [0,NT/2), warps 4-7: [NT/2,NT)
-    const int lrow = (warp & 3) * 32 + (tid & 31);   // TMEM lane == row inside the tile
-    const uint32_t tlane = tmem + ((uint32_t)((warp & 3) * 32) << 16);
+    const int lrow = (warp & 3) * 32 + (tid & 31);   // row inside the tile
     constexpr int CB = NT / 2;
     const int cbeg = half * CB;
     if (EPI == EPI_H16 || EPI == EPI_H16_GELU || EPI == EPI_F16 || EPI == EPI_GELUGRAD) {
@@ -254,7 +235,7 @@ __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
 #pragma unroll 1
         for (int c0 = cbeg; c0 < cbeg + CB; c0 += 32) {
           float v[32];
-          tmem_ld32(tlane + c0, v);
+          acc_ld<32>(sAcc, NT, lrow, c0, v);
           uint32_t pk[16];
           const int grow = sRow[lrow];
           if (EPI == EPI_GELUGRAD) {
@@ -292,7 +273,6 @@ __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
                 make_int4((int)pk[4 * q], (int)pk[4 * q + 1], (int)pk[4 * q + 2], (int)pk[4 * q + 3]);
           }
         }
-        tc_fence_before();
         __syncthreads();
         __half* dst = pass == 0 ? out16 : reinterpret_cast<__half*>(g.out_pre16);
         for (int idx = tid; idx < TILE_M * ECH; idx += NTH) {
@@ -331,7 +311,7 @@ __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
 #pragma unroll 1
       for (int c0 = cbeg; c0 < cbeg + CB; c0 += 32) {
         float v[32];
-        tmem_ld32(tlane + c0, v);
+        acc_ld<32>(sAcc, NT, lrow, c0, v);
 #pragma unroll
         for (int q = 0; q < 8; q++) {
           int ch = (c0 >> 2) + q;
@@ -349,7 +329,6 @@ __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
       }
       red[half][lrow][0] = sum;
       red[half][lrow][1] = sq;
-      tc_fence_before();
       __syncthreads();
       if (EPI == EPI_RES_LN && g.out_pre) {   // training: keep the pre-LayerNorm sum for the backward pass
         for (int idx = tid; idx < TILE_M * ECH; idx += NTH) {
@@ -400,17 +379,16 @@ __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
         }
       }
     }
-    // TMEM fully read and the staging tile stored before the next item overwrites operands / accumulators
-    tc_fence_before();
+    // accumulator tile fully read and the staging tile stored before the next item overwrites them
     __syncthreads();
   }  // item loop
-  if (warp == 0) tmem_dealloc(tmem, NT);
 }
 
 template <int K, int NT, int PRO, int EPI, int FMT = FMT_F16>
 int launch_umma(sstb200_ctx* c, const GemmArgs& g, int n_tiles_y) {
   size_t ops = (size_t)TILE_M * K * 2 + (size_t)NT * K * 2;
   size_t stage = (EPI == EPI_RES_LN || EPI == EPI_ADD_F32) ? (size_t)TILE_M * NT * 4 : (size_t)TILE_M * NT * 2;
+  stage += (size_t)TILE_M * NT * 4;   // + the accumulator tile
   size_t smem = (ops > stage ? ops : stage) + 1024;
   auto kern = umma_gemm_kernel<K, NT, PRO, EPI, FMT>;
   static SmemAttr sa;
@@ -420,7 +398,6 @@ int launch_umma(sstb200_ctx* c, const GemmArgs& g, int n_tiles_y) {
   int items_cap = ((g.M_cap + TILE_M - 1) / TILE_M) * n_tiles_y;
   int per_sm = (int)((220 * 1024) / (smem + 6144));
   if (per_sm < 1) per_sm = 1;
-  if (per_sm > 512 / NT) per_sm = 512 / NT;   // TMEM columns
   int grid = c->num_sms * per_sm;
   if (grid > items_cap) grid = items_cap;
   launch_pdl(kern, dim3(grid), dim3(256), (size_t)(smem), c->stream, ga);

@@ -333,8 +333,8 @@ __global__ void __launch_bounds__(256) vfe_fused_kernel(VfeDev v, const float* _
 // Tile path (max pooling): points are visited in CSR (voxel-sorted) order in tiles of 128.
 //   vfe_mean_kernel     per-voxel xyz mean (4 lanes per voxel, fp64 accumulate)
 //   vfe_l0_tile_kernel  decorate + layer 0 (FFMA, fp32 exact) + in-tile segmented max -> vf0 [M,C0]
-//   vfe_l1_umma_kernel  A = bf16([y0 || vf0[voxel]]) [128 x 2*C0], B = bf16(W1) -> tcgen05.mma into TMEM,
-//                       epilogue BN+ReLU, post-activation tile to smem, in-tile segmented max -> vf1 [M,C1]
+//   vfe_l1_umma_kernel  A = bf16([y0 || vf0[voxel]]) [128 x 2*C0], B = bf16(W1) -> wgmma (two warpgroups of 64 rows),
+//                       epilogue BN+ReLU from the accumulator fragments into an smem tile, in-tile segmented max -> vf1 [M,C1]
 // Post-ReLU values are >= 0, so the max across tile edges is an integer atomicMax on the float bits
 // (exact, order independent); segments interior to a tile are written with plain stores.
 // =====================================================================================================
@@ -501,7 +501,7 @@ __global__ void __launch_bounds__(256) vfe_l1_umma_kernel(VfeDev v, const float*
   pdl_wait();
   pdl_launch();
   constexpr int K = 2 * C0;
-  static_assert(K % 64 == 0 && C1 % 16 == 0 && C1 <= 256, "shape");
+  static_assert(K % 64 == 0 && (C1 == 32 || C1 == 64 || C1 == 128), "shape: wgmma_ss is instantiated for N = 32 / 64 / 128 here");
   extern __shared__ uint8_t l1_smem_raw[];
   uint8_t* base = (uint8_t*)(((uintptr_t)l1_smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* sB = base;                       // K/64 chunks x C1 rows x 128 B - staged ONCE per CTA (persistent over tiles)
@@ -511,9 +511,7 @@ __global__ void __launch_bounds__(256) vfe_l1_umma_kernel(VfeDev v, const float*
   __shared__ int sVox[VT];
   __shared__ float sW0[VFE_MAXD][C0];
   __shared__ float sS0[C0], sT0[C0], sS1[C1], sT1[C1];
-  __shared__ __align__(8) uint64_t mbar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int D0 = v.D0;
   const int M = *nvox_dev;
   const int nvalid = M > 0 ? (int)offsets[M] : 0;
@@ -526,11 +524,6 @@ __global__ void __launch_bounds__(256) vfe_l1_umma_kernel(VfeDev v, const float*
   for (int i = tid; i < C1; i += blockDim.x) {
     sS1[i] = v.s1[i];
     sT1[i] = v.t1[i];
-  }
-  if (warp == 0) tmem_alloc(&tmem_slot, C1 < 32 ? 32 : C1);
-  if (tid == 0) {
-    mbar_init(smem_u32(&mbar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   // B operand: W1 [C1, K] fp32 -> bf16, K-major SWIZZLE_128B, once per CTA (4 pieces in flight per thread)
   for (int i0 = tid; i0 < C1 * (K / 8); i0 += blockDim.x * 4) {
@@ -559,7 +552,6 @@ __global__ void __launch_bounds__(256) vfe_l1_umma_kernel(VfeDev v, const float*
       }
     }
   }
-  uint32_t parity = 0;
   for (int k0 = blockIdx.x * VT; k0 < nvalid; k0 += gridDim.x * VT) {
     const int nrow = min(VT, nvalid - k0);
     __syncthreads();  // previous tile's smem (sTile aliases sA) fully consumed
@@ -607,44 +599,23 @@ __global__ void __launch_bounds__(256) vfe_l1_umma_kernel(VfeDev v, const float*
     }
     asm volatile("cp.async.wait_all;\n" ::: "memory");
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    if (tid == 0) {
-      const uint32_t idesc = umma_idesc(128, C1);
-      const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-#pragma unroll
-      for (int c = 0; c < K / 64; c++)
-#pragma unroll
-        for (int s = 0; s < 4; s++)
-          umma_bf16(tmem, umma_desc_sw128(a0 + c * VT * 128 + s * 32), umma_desc_sw128(b0 + c * C1 * 128 + s * 32), idesc,
-                    (c | s) ? 1u : 0u);
-      umma_commit(smem_u32(&mbar));
+    {
+      const int wg = tid >> 7;
+      float acc[C1 / 2];
+      wg_tile_mma<C1, true, K / 16>(acc, smem_u32(sA) + wg * 64 * 128, VT * 128, smem_u32(sB), C1 * 128, false);
+      wgmma_wait<0>();
+      __syncthreads();   // sTile aliases the A operand that both warpgroups read
+      // epilogue: BN + ReLU into the fp32 tile
+      wg_frag_pairs<C1>(acc, [&](int r, int cc, float v0, float v1) {
+        float* t = sTile + (wg * 64 + r) * (C1 + 1) + cc;
+        t[0] = fmaxf(fmaf(v0, sS1[cc], sT1[cc]), 0.f);
+        t[1] = fmaxf(fmaf(v1, sS1[cc + 1], sT1[cc + 1]), 0.f);
+      });
     }
-    __syncwarp();
-    mbar_wait(smem_u32(&mbar), parity);
-    parity ^= 1u;
-    tc_fence_after();
-    // epilogue: BN + ReLU, tile to smem (operand buffers are free now: the MMA has completed)
-    const int half = warp >> 2;
-    const int lrow = (warp & 3) * 32 + (tid & 31);
-    const uint32_t tlane = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-    constexpr int CB = C1 / 2;
-#pragma unroll 1
-    for (int c0 = half * CB; c0 < half * CB + CB; c0 += 32) {
-      float acc[32];
-      tmem_ld32(tlane + c0, acc);
-#pragma unroll
-      for (int i = 0; i < 32; i++) sTile[lrow * (C1 + 1) + c0 + i] = fmaxf(fmaf(acc[i], sS1[c0 + i], sT1[c0 + i]), 0.f);
-    }
-    tc_fence_before();
     __syncthreads();
     tile_segmax(sTile, C1 + 1, sVox, nrow, C1, vf1);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_slot, C1 < 32 ? 32 : C1);
 }
 
 
@@ -817,7 +788,7 @@ static int vfe_forward_impl(sstb200_ctx* c, const sstb200_vfe_cfg* cfg, const fl
   float* vmean = arena_alloc<float>(c, (size_t)P * 3);
   float* vf0 = arena_alloc<float>(c, (size_t)P * C0);
   float* fold = arena_alloc<float>(c, 2 * (size_t)(C0 + C1) + 8);
-  __nv_bfloat16* y0buf = arena_alloc<__nv_bfloat16>(c, (size_t)P * C0 + 64);  // layer-0 point features (bf16, CSR order) for the tcgen05 layer 1
+  __nv_bfloat16* y0buf = arena_alloc<__nv_bfloat16>(c, (size_t)P * C0 + 64);  // layer-0 point features (bf16, CSR order) for the tensor-core layer 1
   if (!count || !vmean || !vf0 || !fold || !y0buf) return sstb_fail(c, SSTB_ERR_WORKSPACE, "vfe: arena");
   CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)P + 2) * 4, c->stream));
   int nb = (P + 255) / 256;
@@ -881,7 +852,7 @@ static int vfe_forward_impl(sstb200_ctx* c, const sstb200_vfe_cfg* cfg, const fl
                                                              cfg->bn_eps, C1, fold + 2 * C0, fold + 2 * C0 + C1);
   LAUNCH_CHECK(c);
   {
-    // tile path (max pooling, the configurations on the hot path): layer 0 FFMA tiles; layer 1 on tcgen05 when bf16
+    // tile path (max pooling, the configurations on the hot path): layer 0 FFMA tiles; layer 1 on the tensor cores (wgmma) when bf16
     bool l1_done = false, tiled = false;
     const bool umma = cfg->precision == SSTB200_PREC_BF16;
 #define VFE_TILE(a, b)                                                                                                          \

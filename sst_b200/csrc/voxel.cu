@@ -1,6 +1,6 @@
 // Voxel-id ranking, DynamicScatter (fwd/bwd), unique rows, segmented reduce, in-group ranks.
 //
-// B200-first design note (DESIGN.md "voxel index"): instead of the reference's row sort
+// Design note (voxel index): instead of the reference's row sort
 // (at::unique_dim, scatter_points_cuda.cu:202-205) every "unique rows, sorted" on this path is a
 // *bitmap rank*: rows are linearised into a bounded grid, the grid's occupancy bitmap is built with one
 // atomicOr per row, a popcount prefix-scan over the bitmap words gives every occupied cell its rank in

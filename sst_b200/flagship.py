@@ -110,7 +110,7 @@ def fsd_unet_bench(dev, reps=5, precisions=("bf16", "fp32_tc", "fp32")):
             b.record()
             torch.cuda.synchronize(dev)
             ms = a.elapsed_time(b) / reps
-            rec[{"bf16": "f16_tcgen05", "fp32_tc": "fp32_split_tcgen05", "fp32": "fp32_ffma"}[prec]] = {"ms_per_sweep": ms, "sweeps_per_s": 1e3 / ms}
+            rec[{"bf16": "f16_wgmma", "fp32_tc": "fp32_split_wgmma", "fp32": "fp32_ffma"}[prec]] = {"ms_per_sweep": ms, "sweeps_per_s": 1e3 / ms}
     return rec
 
 
@@ -143,5 +143,5 @@ def sir_bench(dev, reps=5, precisions=("bf16", "fp32")):
             b.record()
             torch.cuda.synchronize(dev)
             ms = a.elapsed_time(b) / reps
-            rec["bf16_tcgen05" if prec == "bf16" else "fp32_ffma"] = {"ms": ms, "tflops": flops / ms / 1e9}
+            rec["bf16_wgmma" if prec == "bf16" else "fp32_ffma"] = {"ms": ms, "tflops": flops / ms / 1e9}
     return rec

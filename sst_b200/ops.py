@@ -1,5 +1,5 @@
 """Python face of the op surface the reference exports from `mmdet3d.ops`
-(mmdet3d/ops/__init__.py:23-30), backed by libsstb200 (CUDA, sm_100a).  Same names, argument meaning
+(mmdet3d/ops/__init__.py:23-30), backed by libsstb200 (CUDA, sm_90a).  Same names, argument meaning
 and error behaviour; no CPU path - CPU tensors raise.
 
     Voxelization / voxelization       ops/voxel/voxelize.py:11-130          (dynamic branch only, V1)
@@ -26,7 +26,7 @@ _REDUCE = {"sum": 0, "mean": 1, "max": 2}
 def _need_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
-            raise L.SSTB200Error("sst_b200 ops need CUDA tensors (B200); there is no CPU implementation")
+            raise L.SSTB200Error("sst_b200 ops need CUDA tensors (H100); there is no CPU implementation")
 
 
 # ----------------------------------------------------------------------------------------------

@@ -115,7 +115,7 @@ class SIRLayer(nn.Module):
         s.rel_dist_scaler = float(self.rel_dist_scaler)
         return s
 
-    precision = "fp32"  # 'bf16': rel-MLP layer 3 and both VFE layers on tcgen05 (bf16 operands, fp32 accumulate / LN / pooling)
+    precision = "fp32"  # 'bf16': rel-MLP layer 3 and both VFE layers on the tensor cores (bf16 operands, fp32 accumulate / LN / pooling)
 
     def _forward_composed(self, features, coors, f_cluster, return_inv, return_both, unq_inv_once, new_coors_once):
         """voxel_encoder.py:696-764 as a composition when a gradient is needed: torch Linear / LayerNorm / activation modules (autograd)

@@ -342,7 +342,7 @@ class ToDense(SparseModule):
 # convolution layers
 # ------------------------------------------------------------------------------------------------------------------------
 class SparseConvolution(SparseModule):
-    """conv.py:45-206.  precision: 'fp32' (FFMA, exact path), 'bf16' (tcgen05, 16-bit operands) or 'fp32_tc' (tcgen05 with split-fp16
+    """conv.py:45-206.  precision: 'fp32' (FFMA, exact path), 'bf16' (wgmma, 16-bit operands) or 'fp32_tc' (wgmma with split-fp16
     operands: fp32 tolerance at tensor-core speed; channels % 64) - module attribute, also settable for a whole model with
     set_spconv_precision()."""
 

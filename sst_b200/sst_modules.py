@@ -463,7 +463,7 @@ class SSTv2(nn.Module):
 
     def _run_stack(self, x, plans, precision):
         """All encoder layers through ONE C call (sstb200_sra_stack_forward): with precision 'bf16' and the SST-6 shape this
-        is 2 launches per layer (window attention + fused tcgen05 chain incl. the next layer's QKV)."""
+        is 2 launches per layer (window attention + fused wgmma / TMA chain incl. the next layer's QKV)."""
         layers = [l for blk in self.block_list for l in blk.encoder_list]
         if not layers:
             return x

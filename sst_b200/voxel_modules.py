@@ -62,7 +62,7 @@ L.SIGNATURES["sstb200_dynamic_scatter_vfe_forward"] = (C.c_int, [L.vp, C.POINTER
 @VOXEL_ENCODERS.register_module()
 class DynamicVFE(nn.Module):
     """voxel_encoder.py:92-298."""
-    _drop_first = 1  # DynamicScatter semantics (scatter_points_cuda.cu:207-210), see DESIGN.md "reference quirks"
+    _drop_first = 1  # DynamicScatter semantics (scatter_points_cuda.cu:207-210)
 
     def __init__(self, in_channels=4, feat_channels=[], with_distance=False, with_cluster_center=False,
                  with_voxel_center=False, voxel_size=(0.2, 0.2, 4), point_cloud_range=(0, -40, -3, 70.4, 40, 1),

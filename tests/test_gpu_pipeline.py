@@ -37,7 +37,7 @@ def test_vfe_matches_oracle(cuda, P, batch, extra, precision):
     assert torch.equal(vc.cpu(), vc_o)
     if precision == "fp32":
         torch.testing.assert_close(vf.cpu(), vf_o, rtol=1e-4, atol=1e-4)
-    else:  # second VFE layer with bf16 operands on tcgen05: north_star bf16 tolerance
+    else:  # second VFE layer with bf16 operands on the tensor cores: north_star bf16 tolerance
         assert (vf.cpu() - vf_o).abs().max().item() / vf_o.abs().max().item() < 1e-2
 
 

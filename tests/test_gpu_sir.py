@@ -81,7 +81,7 @@ def test_sir_layer_without_f_cluster_and_shortcut(cuda):
 
 @pytest.mark.parametrize("N,G", [(20000, 64), (150000, 256), (300, 7), (129, 1)])
 def test_sir_config3_bf16_parity(cuda, N, G):
-    """Tensor-core path (tcgen05, bf16 operands / fp32 accumulate): 1e-2 of the fp32 oracle (north_star tolerance for bf16);
+    """Tensor-core path (wgmma, bf16 operands / fp32 accumulate): 1e-2 of the fp32 oracle (north_star tolerance for bf16);
     group coordinates stay bit-exact.  Also covers the in-place [points || feats] hand-over between blocks."""
     g = torch.Generator().manual_seed(N + 1)
     points = torch.cat([torch.randn(N, 3, generator=g) * 10, torch.rand(N, 2, generator=g)], 1)

@@ -135,7 +135,7 @@ def test_unet_and_mixer_reference_golden(cuda):
 
 @pytest.mark.parametrize("cin,cout", [(64, 64), (128, 64), (64, 128), (256, 256), (512, 256)])
 def test_conv_epilogue_both_precisions(cuda, cin, cout):
-    """one launch = gather-GEMM + scale/shift + residual + ReLU; FFMA path and tcgen05 path against the fp64 table oracle"""
+    """one launch = gather-GEMM + scale/shift + residual + ReLU; FFMA path and wgmma path against the fp64 table oracle"""
     from sst_b200 import spconv_modules as SP
     shape = [6, 24, 24]
     feats, coors = SO.synth_sparse(cin + cout, 2, shape, 450, cin)
@@ -184,7 +184,7 @@ def _live_init(net, seed):
 
 
 def test_unet_fsd_channels_both_precisions(cuda):
-    """a SimpleSparseUNet with the channel widths of configs/fsd (64 / 128) against the oracle: fp32 path 1e-4, tcgen05 path 1e-2"""
+    """a SimpleSparseUNet with the channel widths of configs/fsd (64 / 128) against the oracle: fp32 path 1e-4, wgmma path 1e-2"""
     from sst_b200 import registry, spconv_modules as SP
     torch.manual_seed(11)
     net = registry.MODELS.build(dict(type="SimpleSparseUNet", **UNET64)).eval()
@@ -279,7 +279,7 @@ def test_vs_reference_cuda_spconv(cuda):
         (outids, pairs, num), t_ref_pairs = timed(lambda: ext.get_indice_pairs_3d(coors, 1, shape, shape, [3, 3, 3], [1, 1, 1], [1, 1, 1],
                                                                                    [1, 1, 1], [0, 0, 0], 1, 0))
         ref, t_ref_conv = timed(lambda: ext.indice_conv_fp32(feats, w, pairs, num, coors.shape[0], 0, 1))
-    except Exception as e:   # the 2019 kernels are not guaranteed to run on sm_100a / this torch
+    except Exception as e:   # the 2019 kernels are not guaranteed to run on sm_90a / this torch
         pytest.skip(f"reference CUDA spconv did not run here: {type(e).__name__}: {e}")
     (nbr, _), t_tab = timed(lambda: SP.conv_table(coors, coors, 1, shape, shape, [3, 3, 3], [1, 1, 1], [1, 1, 1]))
     w27 = w.reshape(27, 64, 64)
@@ -290,7 +290,7 @@ def test_vs_reference_cuda_spconv(cuda):
     _close(out32, ref, 1e-4)
     _close(out16, ref, 5e-3)
     print(f"\n[spconv SubM 3x3x3 64->64, {coors.shape[0]} voxels, pairs {pairs_ref} / {pairs_here}] reference CUDA: pairs {t_ref_pairs:.0f} us + conv {t_ref_conv:.0f} us | "
-          f"sst_b200: table {t_tab:.0f} us + conv fp32 {t32:.0f} us / tcgen05 {t16:.0f} us")
+          f"sst_b200: table {t_tab:.0f} us + conv fp32 {t32:.0f} us / wgmma {t16:.0f} us")
 
 
 def _gclose(a, b, tol):

@@ -144,7 +144,7 @@ def test_sstv2_fp32_parity(cuda, cfg):
 
 @pytest.mark.parametrize("P,blocks", [(20000, 1), (150000, 6)])
 def test_sstv2_bf16_parity(cuda, P, blocks):
-    """bf16 tensor-core path (tcgen05 GEMMs, fp32 accumulate/softmax/LN): <= 1e-2 relative (north_star tolerance)."""
+    """bf16 tensor-core path (wgmma GEMMs, fp32 accumulate/softmax/LN): <= 1e-2 relative (north_star tolerance)."""
     from sst_b200.sst_modules import SSTInputLayerV2
     feats, coors = _voxels((1000,), P, C=128)
     m = _sst_pair(128, 8, 256, blocks)

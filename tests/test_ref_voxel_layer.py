@@ -1,8 +1,8 @@
 """The reference's OWN compiled voxel_layer (oracle/_ref/voxel_layer_ref.so: /root/reference/mmdet3d/ops/voxel/src/*.cpp,*.cu
-built unmodified for sm_100a by oracle/build_ref.py) as the checker:
+built unmodified for sm_90a by oracle/build_ref.py) as the checker:
 
   * CPU (not gpu): pins oracle.dynamic_voxelize to the reference C++ `dynamic_voxelize` (voxelization_cpu.cpp:7-41).
-  * GPU: libsstb200 vs the reference CUDA kernels on the same B200 - `dynamic_voxelize_gpu` (voxelization_cuda.cu:332-375)
+  * GPU: libsstb200 vs the reference CUDA kernels on the same GPU - `dynamic_voxelize_gpu` (voxelization_cuda.cu:332-375)
     and `dynamic_point_to_voxel_forward/backward_gpu` (scatter_points_cuda.cu:183-303); indices bit-exact.
 
 Skipped when the prebuilt extension is absent (it is git-ignored, travels with gpurun, and is rebuilt by
@@ -79,7 +79,7 @@ def test_dynamic_scatter_vs_reference_cuda(cuda, ref, reduce, P, C, lo):
 
 @pytest.mark.gpu
 def test_speed_vs_reference_cuda(cuda, ref):
-    """SURVEY 8(d): "also time the reference CUDA voxel_layer built for sm_100a - the in-tree GPU kernel to beat for V1/V2".
+    """SURVEY 8(d): "also time the reference CUDA voxel_layer built for sm_90a - the in-tree GPU kernel to beat for V1/V2".
     Same device tensors, CUDA events, L2 flushed before every call, median of 15.  The gate is deliberately loose (2x); the
     measured ratios are printed (run with -s) and written to gpurun_out/ref_cuda_timing.json when that directory exists."""
     import json

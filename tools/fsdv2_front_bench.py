@@ -1,10 +1,10 @@
 """BASELINE config 5 (front part): FSDv2 virtual-voxel front at nuScenes shape - 30k real points x batch 16 (+ 2k voted centres per
 sample), 67-dim point features into DynamicScatterVFE [64,128], multiscale fusion with three coarse levels - through
-sst_b200.fsdv2_modules.VirtualVoxelFront on one B200: first everything `SingleStageFSDV2.extract_feat` does before and after its
+sst_b200.fsdv2_modules.VirtualVoxelFront on one GPU: first everything `SingleStageFSDV2.extract_feat` does before and after its
 `self.backbone(...)` call (identity mixer), then the whole extract_feat with the configs/fsdv2 VirtualVoxelMixer (sparse-conv U-Net,
 SURVEY 8f next-1; spconv_modules.py) in both precisions.
 
-    python tools/fsdv2_front_bench.py > profiles/r02_fsdv2_config5.json     (GPU box)"""
+    python tools/fsdv2_front_bench.py > fsdv2_config5.json"""
 import json
 import os
 import sys

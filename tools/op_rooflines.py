@@ -1,7 +1,7 @@
 """Per-op latency + roofline table for every SURVEY.md 8(a) row, through the public Python ops / modules (the calls a
 reference user makes), on config-2 / config-3 shapes.  CUDA events on the current stream, L2 flushed before every call,
 median of `--iters`.  Ops that return data-dependent shapes read one int32 back (like the reference) - that sync is inside
-the timing, so these are API latencies, not kernel sums (kernel sums: ncu launch lists under profiles/).  The reference's own
+the timing, so these are API latencies, not kernel sums (kernel sums: torch.profiler launch lists).  The reference's own
 CUDA voxel_layer is timed on the same tensors by tests/test_ref_voxel_layer.py::test_speed_vs_reference_cuda.
 
     python tools/op_rooflines.py [--iters 20] [--out gpurun_out/op_rooflines.json]

@@ -1,8 +1,8 @@
-"""FSD sparse U-Net (SURVEY 8f next-1) on one B200: SimpleSparseUNet with the configs/fsd/fsd_waymoD1_1x.py backbone shape on a
+"""FSD sparse U-Net (SURVEY 8f next-1) on one GPU: SimpleSparseUNet with the configs/fsd/fsd_waymoD1_1x.py backbone shape on a
 150k-point synthetic sweep voxelised at 0.2 m (grid 32 x 640 x 640), eval mode.  Reports table building + forward time for the
-FFMA path and the tcgen05 path, per-convolution FLOPs / bytes and the achieved rates.  No oracle import.
+FFMA path and the wgmma path, per-convolution FLOPs / bytes and the achieved rates.  No oracle import.
 
-    python tools/spconv_bench.py [--reps 10] [--out profiles/r02_spconv_bench.json] [--once precision]   (--once: one forward, for ncu)"""
+    python tools/spconv_bench.py [--reps 10] [--out FILE.json] [--once precision]   (--once: one forward, for ncu)"""
 import argparse
 import json
 import os
