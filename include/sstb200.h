@@ -33,7 +33,8 @@ typedef struct sstb200_ctx sstb200_ctx;
 #define SSTB200_REDUCE_SUM 0
 #define SSTB200_REDUCE_MEAN 1
 #define SSTB200_REDUCE_MAX 2
-#define SSTB200_PREC_FP32 0 /* fp32 FFMA everywhere */
+#define SSTB200_PREC_FP32 0 /* fp32 tolerance: fp32 math, except that the SRA encoder layer runs its Linears as split-fp16 tensor-core GEMMs
+                             * (as SSTB200_PREC_FP32_TC below) when d_model and dim_ff are multiples of 64, fp32 FFMA otherwise */
 #define SSTB200_PREC_BF16 1 /* 16-bit tensor-core GEMMs, fp32 accumulate / softmax / LayerNorm / residual.  The SRA encoder uses
                              * IEEE fp16 operands (the reference's own mixed-precision mode, `fp16 = dict(loss_scale=32.0)`), the
                              * VFE / SIR tensor paths bf16; the API name of the mode stays 'bf16'. */

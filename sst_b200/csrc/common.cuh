@@ -107,41 +107,21 @@ static inline cudaError_t ensure_smem(const sstb200_ctx* c, SmemAttr& a, K kern,
 // and its writes are visible) followed by pdl_launch() (griddepcontrol.launch_dependents: allow the next kernel of the
 // stream / graph to be scheduled while this one still runs).  Launches carry the programmatic-stream-serialization
 // attribute, so inside the per-frame CUDA graph consecutive kernels are linked by programmatic edges and the launch
-// latency of kernel N+1 overlaps the execution of kernel N.  SSTB200_PDL=0 disables the attribute (plain launches).
+// latency of kernel N+1 overlaps the execution of kernel N.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-inline int sstb_pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SSTB200_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v;
-}
-
 // All kernels of the library ask for the same shared-memory carveout (max shared): consecutive kernels with different
 // carveouts force the SMs to drain and re-partition L1/shared between launches, which costs more than any L1 hit here.
-inline int sstb_uniform_carveout() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SSTB200_CARVEOUT");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v;
-}
-
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   static void* seen[32];  // per kernel signature & TU; the attribute is sticky per function -> set once, before any capture
   static int nseen = 0;
-  if (sstb_uniform_carveout()) {
-    bool found = false;
-    for (int i = 0; i < nseen; i++) found |= (seen[i] == (void*)kern);
-    if (!found) {
-      cudaFuncSetAttribute((const void*)kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-      if (nseen < 32) seen[nseen++] = (void*)kern;
-    }
+  bool found = false;
+  for (int i = 0; i < nseen; i++) found |= (seen[i] == (void*)kern);
+  if (!found) {
+    cudaFuncSetAttribute((const void*)kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    if (nseen < 32) seen[nseen++] = (void*)kern;
   }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -151,11 +131,22 @@ static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 blo
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = sstb_pdl_enabled();
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
+
+// ---- window batches of the batched attention kernels ---------------------------------------------------------------------
+// Batch b = the windows whose first slot lies in [b * ATT_CHUNK, (b + 1) * ATT_CHUNK) (win_batch_kernel, window.cu); with
+// windows of at most ATT_MAXT tokens it holds at most ATT_CHUNK - 1 + ATT_MAXT rows, which the kernels stage in ATT_BT rows.
+#define ATT_MAXT 144
+#define ATT_CHUNK 112
+#define ATT_BT 256
+static_assert(ATT_CHUNK - 1 + ATT_MAXT <= ATT_BT, "a window batch must fit the staged rows");
+// Record-array bound for a plan over n tokens.  At most n / ATT_CHUNK + 1 records are written, but the caller's win_batch buffer
+// is documented (include/sstb200.h) and allocated (ops.py, engine.py) for n / 32 + 2, so that stays the bound.
+static inline int att_rec_cap(int n) { return n / 32 + 2; }
 
 // ---- device helpers ------------------------------------------------------
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }

@@ -142,7 +142,6 @@ int sstb_win_attn(sstb200_ctx* c, const TI* qkv, int d, int nhead, int n_cap, co
 // ------------------------------------------------------------------------------------------------
 // Tensor-core ragged window attention helpers (mma.sync.m16n8k16, fp32 accumulate) shared by the kernels below.
 // ------------------------------------------------------------------------------------------------
-#define ATT_MAXT 144
 
 __device__ __forceinline__ void mma_bf16_16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
@@ -190,8 +189,6 @@ __device__ __forceinline__ uint32_t ex2_h2(float a, float b) {
 // sums come out of the tensor core as well (a constant "ones" B fragment).  A further chunk rescales the running accumulators
 // by 2^(old max - new max).  ~0.15 instructions per score; the two-pass form this replaces needed ~0.7.
 // ------------------------------------------------------------------------------------------------
-#define ATT_CHUNK 112
-#define ATT_BT 256   // >= ATT_CHUNK - 1 + 144 rows per batch
 #define ATT_KCHUNK 64
 
 // m0 / m1: running row maxima in log2 units; o / ol: running numerators / denominators.  kaddr / vaddr: this lane's ldmatrix
@@ -280,9 +277,8 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
                                                                        const int4* __restrict__ batch_rec, int rec_cap,
                                                                        const int32_t* __restrict__ tok_perm, float scale,
                                                                        const float* __restrict__ tau, int tau_n, float tau_min,
-                                                                       __half* __restrict__ out, long long* dbg) {
+                                                                       __half* __restrict__ out) {
   pdl_launch();
-  int dbg_n = 0;
   constexpr int D = 128, DH = 16, LD = NHL * 16 + 8, HSPLIT = 8 / NHL, PPR = NHL * 2;  // PPR: 16-byte pieces per row per matrix
   constexpr int NROW = ATT_BT + 16;
   extern __shared__ __align__(16) uint8_t att_smem[];
@@ -295,8 +291,7 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
   __shared__ short sTileKe[ATT_BT];
   __shared__ int sNumTiles;
   __shared__ float sInvQ[COS ? NHL * NROW : 1], sInvK[COS ? NHL * NROW : 1];   // [head][row]: 1 / max(|q|, 1e-12), 1 / max(|k|, 1e-12)
-  // batch b = the windows whose first slot lies in [b*ATT_CHUNK, (b+1)*ATT_CHUNK) (win_batch_kernel, csrc/window.cu); it holds
-  // at most ATT_CHUNK - 1 + 144 <= ATT_BT rows.  record = {first window, end window, first slot, end slot}
+  // record of window batch b (see ATT_CHUNK in common.cuh) = {first window, end window, first slot, end slot}
   int4 rc = batch_rec[min((int)blockIdx.x / HSPLIT, rec_cap - 1)];
   const int nbatch = counters[17];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -308,7 +303,6 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
   const uint32_t klane = (uint32_t)((((lane & 7) + ((lane >> 4) & 1) * 8) * LD + ((lane >> 3) & 1) * 8) * 2);
   const uint32_t vlane = (uint32_t)((((lane & 7) + ((lane >> 3) & 1) * 8) * LD + (lane >> 4) * 8) * 2);
   const float sl2 = scale * 1.4426950408889634f;   // exp(x) = 2^(x log2 e)
-  bool waited = false;
   for (int unit = blockIdx.x; unit < nbatch * HSPLIT; unit += gridDim.x) {
     const int b = unit / HSPLIT, hs = unit % HSPLIT;
     if (unit != (int)blockIdx.x) rc = batch_rec[b];
@@ -316,7 +310,6 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
     if (wb == we) continue;  // a big window covers this chunk entirely (uniform per CTA)
     const int nrow = min(s1 - s0, ATT_BT);
     const int nfill = min(((nrow + 15) & ~15) + 16, NROW);  // key chunks may run up to 15 rows past the batch: keep them finite (0)
-    if (dbg && threadIdx.x == 0 && dbg_n < 4) dbg[(blockIdx.x * 4 + dbg_n) * 4 + 0] = clock64();
     __syncthreads();  // previous batch fully consumed
     // staging role: lane = (row of an 8-row group, 16-byte piece p of the NHL heads' columns); a warp covers 8 rows x {K, V, Q} per
     // step, the CTA 64 rows -> <= 5 steps, all of whose token loads are in flight together
@@ -358,10 +351,7 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
       }
       if (lane == 0) sNumTiles = min(cnt, ATT_BT);
     }
-    if (!waited) {   // q|k|v of this layer are complete and visible from here on
-      pdl_wait();
-      waited = true;
-    }
+    pdl_wait();   // q|k|v of this layer are complete and visible from here on (returns at once after the first unit)
     // K | V | Q rows (gathered through the window permutation): 16-byte pieces with cp.async, zero fill beyond the batch
 #pragma unroll
     for (int j = 0; j < SSTEPS; j++) {
@@ -382,10 +372,8 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
         }
       }
     }
-    if (dbg && threadIdx.x == 0 && dbg_n < 4) dbg[(blockIdx.x * 4 + dbg_n) * 4 + 1] = clock64();
     asm volatile("cp.async.wait_all;\n" ::: "memory");
     __syncthreads();
-    if (dbg && threadIdx.x == 0 && dbg_n < 4) dbg[(blockIdx.x * 4 + dbg_n) * 4 + 2] = clock64();
     if (COS) {   // F.normalize(q), F.normalize(k) per head (eps 1e-12) as fp32 factors
       for (int idx = threadIdx.x; idx < nfill * NHL * 2; idx += 256) {
         const int r = idx / (NHL * 2), rem = idx - r * (NHL * 2), hl = rem >> 1, isk = rem & 1;
@@ -402,9 +390,8 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
       }
       __syncthreads();
     }
-    const int ntiles = sNumTiles;
 #pragma unroll 1
-    for (int item = warp; item < ntiles * NHL; item += 8) {   // (q-tile, head) items, round-robin over the warps
+    for (int item = warp; item < sNumTiles * NHL; item += 8) {   // (q-tile, head) items, round-robin over the warps
       const int tk = item / NHL, hl = item - tk * NHL;
       const int row = sTileRow[tk], kb = sTileKb[tk], ke = sTileKe[tk];
       const int n = ke - kb;
@@ -450,10 +437,6 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
         op1[t4 + 4] = (OUT_BF16 ? pack2_bf16 : pack2_f16)(o[1][2] * i1, o[1][3] * i1);
       }
     }
-    if (dbg && threadIdx.x == 0 && dbg_n < 4) {
-      dbg[(blockIdx.x * 4 + dbg_n) * 4 + 3] = clock64() * 1000 + ntiles;
-      dbg_n++;
-    }
   }
 }
 
@@ -463,8 +446,9 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
 static inline int sstb_win_attn_batch(sstb200_ctx* c, const __half* qkv, const int32_t* counters, const int32_t* win_offsets,
                                       const int32_t* win_batch, int n_cap, const int32_t* tok_perm, void* out_v, bool out_bf16 = false,
                                       const float* tau = nullptr, int tau_n = 0, float tau_min = 0.f) {
-  constexpr int NHL = 2;   // heads per CTA -> 4 CTAs per window batch 
-  const int rec_cap = n_cap / 32 + 2;   // bound of the record array for the smallest batch size (csrc/window.cu)
+  constexpr int NHL = 2;   // heads per CTA -> 4 CTAs per window batch
+  constexpr int CTAS_PER_SM = 9;   // grid of the persistent unit loop
+  const int rec_cap = att_rec_cap(n_cap);
   __half* out = reinterpret_cast<__half*>(out_v);
   const int4* recs = reinterpret_cast<const int4*>(win_batch);
   if (tau && out_bf16) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "cosine attention is not built for the training path");
@@ -473,47 +457,15 @@ static inline int sstb_win_attn_batch(sstb200_ctx* c, const __half* qkv, const i
   CUDA_TRY(c, out_bf16 ? ensure_smem(c, sb, win_attn_batch_kernel<NHL, true, false>, smem)
                        : (tau ? ensure_smem(c, sc, win_attn_batch_kernel<NHL, false, true>, smem)
                               : ensure_smem(c, sa, win_attn_batch_kernel<NHL, false, false>, smem)));
-  static int grid_mult = 0;
-  if (!grid_mult) {
-    const char* e = getenv("SSTB200_ATT_GRID");  // CTAs per SM of the persistent unit loop (tuning knob)
-    grid_mult = e && atoi(e) > 0 ? atoi(e) : 9;
-  }
-  static int dbg_on = -1;
-  if (dbg_on < 0) dbg_on = getenv("SSTB200_ATT_DBG") ? atoi(getenv("SSTB200_ATT_DBG")) : 0;
-  static long long* dbg_buf = nullptr;
-  const int grid = c->num_sms * grid_mult;
-  if (dbg_on && !dbg_buf) CUDA_TRY(c, cudaMalloc(&dbg_buf, (size_t)4096 * 16 * 8));
-  if (dbg_on) CUDA_TRY(c, cudaMemsetAsync(dbg_buf, 0, (size_t)grid * 16 * 8, c->stream));
-  long long* dbg = dbg_on ? dbg_buf : (long long*)nullptr;
+  const int grid = c->num_sms * CTAS_PER_SM;
   if (out_bf16)
     CUDA_TRY(c, launch_pdl(win_attn_batch_kernel<NHL, true, false>, dim3(grid), dim3(256), smem, c->stream, qkv, counters, win_offsets, recs, rec_cap,
-                           tok_perm, 0.25f, tau, tau_n, tau_min, out, dbg));
+                           tok_perm, 0.25f, tau, tau_n, tau_min, out));
   else if (tau)
     CUDA_TRY(c, launch_pdl(win_attn_batch_kernel<NHL, false, true>, dim3(grid), dim3(256), smem, c->stream, qkv, counters, win_offsets, recs, rec_cap,
-                           tok_perm, 0.25f, tau, tau_n, tau_min, out, dbg));
+                           tok_perm, 0.25f, tau, tau_n, tau_min, out));
   else
     CUDA_TRY(c, launch_pdl(win_attn_batch_kernel<NHL, false, false>, dim3(grid), dim3(256), smem, c->stream, qkv, counters, win_offsets, recs, rec_cap,
-                           tok_perm, 0.25f, tau, tau_n, tau_min, out, dbg));
-  if (dbg_on) {
-    static int dumps = 0;
-    std::vector<long long> h((size_t)grid * 16);
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    CUDA_TRY(c, cudaMemcpy(h.data(), dbg_buf, h.size() * 8, cudaMemcpyDeviceToHost));
-    if (dumps++ % dbg_on == 0) {
-      long long tmin = 1LL << 62;
-      for (int b = 0; b < grid; b++) if (h[b * 16]) tmin = std::min(tmin, h[b * 16]);
-      for (int b : {0, 1, 147, 148, 300, 443, 444, 600, 887}) {
-        if (b >= grid) continue;
-        printf("[attn dbg] cta %3d:", b);
-        for (int u = 0; u < 4; u++) {
-          const long long* e = &h[(b * 4 + u) * 4];
-          if (!e[0]) continue;
-          printf("  unit%d start %lld staged+%lld sync+%lld done+%lld tiles %lld |", u, e[0] - tmin, e[1] - e[0], e[2] - e[0], e[3] / 1000 - e[0], e[3] % 1000);
-        }
-        printf("\n");
-      }
-      fflush(stdout);
-    }
-  }
+                           tok_perm, 0.25f, tau, tau_n, tau_min, out));
   return SSTB_OK;
 }

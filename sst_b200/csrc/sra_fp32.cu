@@ -191,19 +191,11 @@ void sstb_add_norm(cudaStream_t st, const float* a, const float* b, const float*
 }
 
 // ------------------------------------------------------------------------------------------------
-// fp32-tolerance GEMMs on the tensor core (SSTB200_FP32_TC, default on): every Linear of the layer runs through sstb_gemm_rows_x3
-// (split-fp16 operands: hi.hi + lo.hi + hi.lo in one set of fp32 accumulators, ~2^-22 relative) instead of the FFMA kernel above; the
-// positional term of q|k is added to a copy of the input first.  Shapes that do not fit fall back to the FFMA kernel.
+// fp32-tolerance GEMMs on the tensor core: every Linear of the layer runs through sstb_gemm_rows_x3 (split-fp16 operands:
+// hi.hi + lo.hi + hi.lo in one set of fp32 accumulators, ~2^-22 relative) instead of the FFMA kernel above; the positional term of
+// q|k is added to a copy of the input first.  Shapes sstb_gemm_rows_x3 does not take (d_model or dim_ff not a multiple of 64) run
+// on the FFMA kernel.
 // ------------------------------------------------------------------------------------------------
-static int fp32_tc_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SSTB200_FP32_TC");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v;
-}
-
 __global__ void add_pos_kernel(const float* __restrict__ x, int d, PosTab pos, float* __restrict__ out, int n, const int32_t* __restrict__ n_dev) {
   pdl_wait();
   pdl_launch();
@@ -216,10 +208,8 @@ __global__ void add_pos_kernel(const float* __restrict__ x, int d, PosTab pos, f
 
 static int linear_fp32(sstb200_ctx* c, const float* A, int lda, const float* W, const float* bias, const float* res, int ldr, float* out,
                        int ldo, int n_cap, const int32_t* n_dev, int N, int K, int act) {
-  if (fp32_tc_enabled()) {
-    const int rc = sstb_gemm_rows_x3(c, A, lda, W, bias, res, ldr, out, ldo, n_cap, n_dev, N, K, act);
-    if (rc != SSTB_ERR_UNSUPPORTED) return rc;
-  }
+  const int rc = sstb_gemm_rows_x3(c, A, lda, W, bias, res, ldr, out, ldo, n_cap, n_dev, N, K, act);
+  if (rc != SSTB_ERR_UNSUPPORTED) return rc;
   sstb_gemm_rows_ex(c->stream, A, lda, W, K, bias, res, ldr, nullptr, out, ldo, n_cap, n_dev, N, K, act, nullptr, nullptr, 0, 0, 0, 0);
   return SSTB_OK;
 }
@@ -245,7 +235,7 @@ int sstb_sra_layer_fp32(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb20
   }
   // q,k from (x + pos); v from x
   int rc = SSTB_OK;
-  if (fp32_tc_enabled() && d % 64 == 0 && ff % 64 == 0) {
+  if (d % 64 == 0 && ff % 64 == 0) {
     const float* xqk = xin;
     if (P->pos_table) {
       float* xpos = arena_alloc<float>(c, (size_t)n_cap * d);

@@ -189,22 +189,21 @@ __global__ void tok_finish_kernel(int n, const int32_t* __restrict__ n_dev, cons
   if (flat2win) flat2win[i] = (long long)win_rank[w] * lv.maxtok[slot] + tok_inner[i];
 }
 
-// Window batches for the batched attention kernel: batch b = the windows whose first slot lies in [b*chunk, (b+1)*chunk).
+// Window batches for the batched attention kernels: batch b = the windows whose first slot lies in [b*ATT_CHUNK, (b+1)*ATT_CHUNK).
 // One int4 record per batch {first window, end window, first slot, end slot} (two lower bounds over offsets[0..R) per thread), so
 // that a consumer CTA learns everything about its batch from ONE load; counters[17] = number of batches.
-// A batch holds at most chunk - 1 + max_window_tokens rows.
-__global__ void win_batch_kernel(const uint32_t* __restrict__ offsets, const int32_t* __restrict__ nwin_dev, int chunk,
+__global__ void win_batch_kernel(const uint32_t* __restrict__ offsets, const int32_t* __restrict__ nwin_dev,
                                  int4* __restrict__ batch_rec, int rec_cap, int32_t* __restrict__ counters, const int32_t* __restrict__ flags) {
   pdl_wait();
   pdl_launch();
   const int R = *nwin_dev;
   const int ntok = (int)offsets[R];
-  const int nb = (ntok + chunk - 1) / chunk;
+  const int nb = (ntok + ATT_CHUNK - 1) / ATT_CHUNK;
   for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < nb && b < rec_cap; b += gridDim.x * blockDim.x) {
     int w[2];
 #pragma unroll
     for (int e = 0; e < 2; e++) {
-      const uint32_t t0 = (uint32_t)(b + e) * (uint32_t)chunk;
+      const uint32_t t0 = (uint32_t)(b + e) * (uint32_t)ATT_CHUNK;
       int lo = 0, hi = R;
       while (lo < hi) {
         int mid = (lo + hi) >> 1;
@@ -293,14 +292,8 @@ static int window_plan_impl(sstb200_ctx* c, const TC* coors, int n, const int32_
                (long long*)o->drop_level, (long long*)o->flat2win_inds, r.offsets, o->tok_slot);
   }
   if (o->win_batch) {
-    static int chunk = 0;   // slots per window batch (tuning knob SSTB200_ATT_CHUNK, 32..112; a batch holds <= chunk - 1 + 144 <= 255 rows)
-    if (!chunk) {
-      const char* e = getenv("SSTB200_ATT_CHUNK");
-      chunk = e ? atoi(e) : 112;
-      if (chunk < 32 || chunk > 112) chunk = 112;
-    }
-    launch_pdl(win_batch_kernel, dim3((n / chunk + 256) / 256), dim3(256), (size_t)0, c->stream, (const uint32_t*)r.offsets, (const int32_t*)nwin,
-               chunk, reinterpret_cast<int4*>(o->win_batch), n / 32 + 2, o->counters, (const int32_t*)k.flags);
+    launch_pdl(win_batch_kernel, dim3((n / ATT_CHUNK + 256) / 256), dim3(256), (size_t)0, c->stream, (const uint32_t*)r.offsets, (const int32_t*)nwin,
+               reinterpret_cast<int4*>(o->win_batch), att_rec_cap(n), o->counters, (const int32_t*)k.flags);
   }
   LAUNCH_CHECK(c);
   if (err_host) {
