@@ -347,6 +347,8 @@ int sstb200_sra_stack_forward(sstb200_ctx* ctx, const sstb200_sra_layer* layers,
 /* ---- training (BASELINE config 4): SSTv2's encoder stack with everything the backward pass needs kept in `workspace`, and the
  * backward pass (the autograd graph torch builds over sst_basic_block_v2.py:100-126 / backbones/sst_v2.py:129-133 in the reference).
  * Shape: d_model 128, 8 heads, dim_ff 256, post-norm LayerNorm, GELU, windows <= 144 tokens (all configs/sst_refactor models).
+ * Attention: plain scaled dot product, or cosine attention (layer.tau non-NULL: tau_n 1 or 8 temperatures, tau_min > 0; the
+ * gradient of tau is 0 where tau < tau_min, as torch's clamp(min=) gives it).  BatchNorm layers (norm1_mean non-NULL) are refused.
  * GEMM operands and saved activations are bf16, accumulation / softmax / LayerNorm / residual stream / gradients of the
  * parameters fp32.  For these two entry points the `*_w_f16` fields of sstb200_sra_layer hold BF16 copies of the weights. */
 typedef struct {
@@ -354,6 +356,7 @@ typedef struct {
 } sstb200_sra_layer_wt;
 typedef struct { /* fp32 accumulators in the layout of the parameters; the call ADDS to them */
   float *in_proj_w, *in_proj_b, *out_proj_w, *out_proj_b, *lin1_w, *lin1_b, *lin2_w, *lin2_b, *norm1_w, *norm1_b, *norm2_w, *norm2_b;
+  float* tau; /* [tau_n] for a cosine-attention layer, NULL for plain attention */
 } sstb200_sra_layer_grads;
 
 size_t sstb200_sra_train_workspace_bytes(int n, int num_layers);

@@ -451,21 +451,14 @@ static inline int sstb_win_attn_batch(sstb200_ctx* c, const __half* qkv, const i
   const int rec_cap = att_rec_cap(n_cap);
   __half* out = reinterpret_cast<__half*>(out_v);
   const int4* recs = reinterpret_cast<const int4*>(win_batch);
-  if (tau && out_bf16) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "cosine attention is not built for the training path");
   size_t smem = (size_t)3 * (ATT_BT + 16) * (NHL * 16 + 8) * sizeof(__half);
-  static SmemAttr sa, sb, sc;
-  CUDA_TRY(c, out_bf16 ? ensure_smem(c, sb, win_attn_batch_kernel<NHL, true, false>, smem)
-                       : (tau ? ensure_smem(c, sc, win_attn_batch_kernel<NHL, false, true>, smem)
-                              : ensure_smem(c, sa, win_attn_batch_kernel<NHL, false, false>, smem)));
+  static SmemAttr sa, sb, sc, sd;
+  auto* kern = out_bf16 ? (tau ? win_attn_batch_kernel<NHL, true, true> : win_attn_batch_kernel<NHL, true, false>)
+                        : (tau ? win_attn_batch_kernel<NHL, false, true> : win_attn_batch_kernel<NHL, false, false>);
+  SmemAttr& attr = out_bf16 ? (tau ? sd : sb) : (tau ? sc : sa);
+  CUDA_TRY(c, ensure_smem(c, attr, kern, smem));
   const int grid = c->num_sms * CTAS_PER_SM;
-  if (out_bf16)
-    CUDA_TRY(c, launch_pdl(win_attn_batch_kernel<NHL, true, false>, dim3(grid), dim3(256), smem, c->stream, qkv, counters, win_offsets, recs, rec_cap,
-                           tok_perm, 0.25f, tau, tau_n, tau_min, out));
-  else if (tau)
-    CUDA_TRY(c, launch_pdl(win_attn_batch_kernel<NHL, false, true>, dim3(grid), dim3(256), smem, c->stream, qkv, counters, win_offsets, recs, rec_cap,
-                           tok_perm, 0.25f, tau, tau_n, tau_min, out));
-  else
-    CUDA_TRY(c, launch_pdl(win_attn_batch_kernel<NHL, false, false>, dim3(grid), dim3(256), smem, c->stream, qkv, counters, win_offsets, recs, rec_cap,
-                           tok_perm, 0.25f, tau, tau_n, tau_min, out));
+  CUDA_TRY(c, launch_pdl(kern, dim3(grid), dim3(256), smem, c->stream, qkv, counters, win_offsets, recs, rec_cap, tok_perm, 0.25f, tau, tau_n,
+                         tau_min, out));
   return SSTB_OK;
 }

@@ -9,7 +9,7 @@
 // LayerNorm, residual stream, weight gradients and the optimizer state are fp32.
 //
 // Per layer, forward:   qkv = [x+pos | x] Wqkv^T        wgmma GEMM (csrc/umma_gemm.cuh)  , q|k|v fp16 for the attention kernel
-//                       att = windowed softmax(q k^T) v  csrc/sra_attn.cuh (bf16 output)
+//                       att = windowed softmax(q k^T) v  csrc/sra_attn.cuh (bf16 output; plain or cosine logits)
 //                       x1 = LN1(x + att Wo^T + bo)      wgmma GEMM + LN epilogue, keeps t1   = pre-LN sum
 //                       h  = GELU(z), z = x1 W1^T + b1   wgmma GEMM, keeps z  
 //                       y  = LN2(x1 + h W2^T + b2)       wgmma GEMM + LN epilogue, keeps t2  
@@ -335,6 +335,13 @@ static int launch_dw(sstb200_ctx* c, const __nv_bfloat16* dY, int ldy, int n_out
 // ds_ij = p_ij (dO_i . v_j - D_i).  Pass B, one thread per (key, head): dk_j = scale * sum_i ds_ij q_i, dv_j = sum_i p_ij dO_i
 // using the row statistics pass A left in shared memory.  No atomics, fp32 math; dq | dk | dv leave as bf16 rows in flat
 // token order.
+// COS: cosine attention (models/sst/cosine_msa.py:123-185), logits s_ij = c qh_i . kh_j with qh = q iq, kh = k ik,
+// iq = 1 / max(|q|, 1e-12), ik likewise, c = 1 / max(tau_h, tau_min).  iq / ik per (row, head) are recomputed from the staged
+// fp16 q | k into shared memory, as the forward kernel does.  With g_ij = p_ij (dO_i . v_j - D_i): dqh_i = c sum_j g_ij kh_j and
+// dq_i = iq (dqh_i - qh_i (qh_i . dqh_i)), the gradient of F.normalize (q = 0 is the only way the clamp engages for an fp16
+// row, and there qh = 0, so the same formula gives dqh / 1e-12); dk symmetrically in pass B.  Pass A also sums g_ij (qh_i . kh_j)
+// per head (d loss / d c); each CTA writes its per-head sums to tau_part[blockIdx.x][8] (fixed thread -> row mapping, fixed
+// reduction tree), and tau_grad_kernel turns them into d tau.
 // ------------------------------------------------------------------------------------------------
 constexpr int AB_LD = 40;   // halfs per staged row and tensor (2 heads x 16 + 8 pad)
 
@@ -366,21 +373,38 @@ __device__ __forceinline__ void store16_bf16(__nv_bfloat16* p, const float* v) {
   reinterpret_cast<uint4*>(p)[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 
+constexpr int AB_NHL = 2, AB_NROW = ATT_BT;   // heads per CTA, staged rows
+
+static size_t attn_bwd_smem(bool cos) {
+  size_t b = (size_t)4 * AB_NROW * AB_LD * 2 + (size_t)AB_NROW * AB_NHL * 3 * 4;
+  if (cos) b += (size_t)2 * AB_NHL * AB_NROW * 4 + (size_t)8 * AB_NHL * 4 + 8 * 4;   // sInvQ, sInvK, sTRed, sTAcc
+  return b;
+}
+
+// Parameters after dqkv are read by the COS instantiation only (they come last so that the plain kernel's code is unchanged).
+template <bool COS>
 __global__ void __launch_bounds__(256) win_attn_bwd_kernel(const __half* __restrict__ qkv, const __nv_bfloat16* __restrict__ att,
                                                            const __nv_bfloat16* __restrict__ datt, const int32_t* __restrict__ counters,
                                                            const int32_t* __restrict__ win_offsets, const int32_t* __restrict__ win_batch,
-                                                           const int32_t* __restrict__ tok_perm, float scale, __nv_bfloat16* __restrict__ dqkv) {
+                                                           const int32_t* __restrict__ tok_perm, float scale, __nv_bfloat16* __restrict__ dqkv,
+                                                           const float* __restrict__ tau, int tau_n, float tau_min, float* __restrict__ tau_part) {
   pdl_wait();
   pdl_launch();
-  constexpr int D = 128, DH = 16, NHL = 2, HSPLIT = 4, NROW = ATT_BT;
+  constexpr int D = 128, DH = 16, NHL = AB_NHL, HSPLIT = 4, NROW = AB_NROW;
   extern __shared__ __align__(16) uint8_t ab_smem[];
   __half* sQ = reinterpret_cast<__half*>(ab_smem);
   __half* sK = sQ + NROW * AB_LD;
   __half* sV = sK + NROW * AB_LD;
   __nv_bfloat16* sG = reinterpret_cast<__nv_bfloat16*>(sV + NROW * AB_LD);   // dO
   float* sStat = reinterpret_cast<float*>(sG + NROW * AB_LD);                 // [NROW][NHL][3]: max, 1/sum, D
+  // COS only (dynamic shared memory, so that the plain kernel's static layout is unchanged)
+  float* sInvQ = sStat + NROW * NHL * 3;   // [NHL][NROW] 1 / max(|q|, 1e-12)
+  float* sInvK = sInvQ + NHL * NROW;       // [NHL][NROW] 1 / max(|k|, 1e-12)
+  float* sTRed = sInvK + NHL * NROW;       // [8 warps][NHL] per-warp temperature sums of the current unit
+  float* sTAcc = sTRed + 8 * NHL;          // [8 heads] this CTA's temperature sums over all its units
   __shared__ int sTok[NROW];
   __shared__ short sKb[NROW], sKe[NROW];   // window key range of every local row
+  if (COS && threadIdx.x < 8) sTAcc[threadIdx.x] = 0.f;
   const int nbatch = counters[17];
   for (int unit = blockIdx.x; unit < nbatch * HSPLIT; unit += gridDim.x) {
     const int b = unit / HSPLIT, hs = unit % HSPLIT;
@@ -414,17 +438,42 @@ __global__ void __launch_bounds__(256) win_attn_bwd_kernel(const __half* __restr
     }
     asm volatile("cp.async.wait_all;\n" ::: "memory");
     __syncthreads();
+    if (COS) {   // F.normalize(q), F.normalize(k) per head (eps 1e-12) as fp32 factors
+      for (int idx = threadIdx.x; idx < nrow * NHL * 2; idx += blockDim.x) {
+        const int r = idx >> 2, hl = (idx >> 1) & 1, isk = idx & 1;
+        float f[16];
+        load16_f16((isk ? sK : sQ) + r * AB_LD + hl * DH, f);
+        float ss = 0.f;
+#pragma unroll
+        for (int d = 0; d < 16; d++) ss = fmaf(f[d], f[d], ss);
+        (isk ? sInvK : sInvQ)[hl * NROW + r] = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
+      }
+      __syncthreads();
+    }
     // ---- pass A: per (query row, head)
+    float tsum = 0.f;   // COS: sum of g_ij (qh_i . kh_j) over this thread's rows; its head is hl = threadIdx.x & 1
     for (int it = threadIdx.x; it < nrow * NHL; it += blockDim.x) {
       const int r = it >> 1, hl = it & 1;
       const int kb = sKb[r], ke = sKe[r];
-      float q[16], g[16], o[16];
+      float q[16], g[16];
       load16_f16(sQ + r * AB_LD + hl * DH, q);
       load16_bf16(sG + r * AB_LD + hl * DH, g);
-      load16_bf16(att + (size_t)sTok[r] * D + (hs * NHL + hl) * DH, o);
       float Dv = 0.f;
+      if (!COS) {
+        float o[16];
+        load16_bf16(att + (size_t)sTok[r] * D + (hs * NHL + hl) * DH, o);
 #pragma unroll
-      for (int d = 0; d < 16; d++) Dv = fmaf(g[d], o[d], Dv);
+        for (int d = 0; d < 16; d++) Dv = fmaf(g[d], o[d], Dv);
+      }
+      // COS: logit = (q . k ik) sc with sc = c iq (the query's factors), so s below is q . kh after the key's factor.  D = dO . O
+      // is formed from the recomputed fp32 probabilities (sum_j p_ij dO_i . v_j) rather than from the bf16 output: then
+      // sum_j g_ij = 0 holds to fp32 rounding, which d tau - a sum of g_ij (qh_i . kh_j) over every window - depends on.
+      float sc = scale, iq = 1.f, cinv = 1.f;
+      if (COS) {
+        cinv = 1.0f / fmaxf(tau_n > 1 ? tau[hs * NHL + hl] : tau[0], tau_min);
+        iq = sInvQ[hl * NROW + r];
+        sc = cinv * iq;
+      }
       float m = -INFINITY;
       for (int j = kb; j < ke; j++) {
         float k[16];
@@ -432,7 +481,8 @@ __global__ void __launch_bounds__(256) win_attn_bwd_kernel(const __half* __restr
         float s = 0.f;
 #pragma unroll
         for (int d = 0; d < 16; d++) s = fmaf(q[d], k[d], s);
-        m = fmaxf(m, s * scale);
+        if (COS) s *= sInvK[hl * NROW + j];
+        m = fmaxf(m, s * sc);
       }
       float l = 0.f;
       for (int j = kb; j < ke; j++) {
@@ -441,9 +491,22 @@ __global__ void __launch_bounds__(256) win_attn_bwd_kernel(const __half* __restr
         float s = 0.f;
 #pragma unroll
         for (int d = 0; d < 16; d++) s = fmaf(q[d], k[d], s);
-        l += __expf(s * scale - m);
+        if (COS) {
+          float v[16];
+          load16_f16(sV + j * AB_LD + hl * DH, v);
+          float dp = 0.f;
+#pragma unroll
+          for (int d = 0; d < 16; d++) dp = fmaf(g[d], v[d], dp);
+          s *= sInvK[hl * NROW + j];
+          const float e = __expf(s * sc - m);
+          l += e;
+          Dv = fmaf(e, dp, Dv);
+        } else {
+          l += __expf(s * sc - m);
+        }
       }
       const float il = 1.0f / l;
+      if (COS) Dv *= il;
       float dq[16];
 #pragma unroll
       for (int d = 0; d < 16; d++) dq[d] = 0.f;
@@ -457,17 +520,46 @@ __global__ void __launch_bounds__(256) win_attn_bwd_kernel(const __half* __restr
           s = fmaf(q[d], k[d], s);
           dp = fmaf(g[d], v[d], dp);
         }
-        const float p = __expf(s * scale - m) * il;
-        const float ds = p * (dp - Dv) * scale;
+        float ds;
+        if (COS) {
+          const float ik = sInvK[hl * NROW + j];
+          s *= ik;
+          const float p = __expf(s * sc - m) * il;
+          const float gij = p * (dp - Dv);
+          tsum = fmaf(gij, s * iq, tsum);   // g_ij (qh_i . kh_j)
+          ds = gij * cinv * ik;             // dqh_i = c sum_j g_ij kh_j = sum_j (g_ij c ik_j) k_j
+        } else {
+          const float p = __expf(s * scale - m) * il;
+          ds = p * (dp - Dv) * scale;
+        }
 #pragma unroll
         for (int d = 0; d < 16; d++) dq[d] = fmaf(ds, k[d], dq[d]);
+      }
+      if (COS) {   // dq = iq (dqh - qh (qh . dqh))
+        float qd = 0.f;
+#pragma unroll
+        for (int d = 0; d < 16; d++) qd = fmaf(q[d], dq[d], qd);
+        const float t = qd * iq * iq;
+#pragma unroll
+        for (int d = 0; d < 16; d++) dq[d] = iq * fmaf(-q[d], t, dq[d]);
       }
       sStat[(r * NHL + hl) * 3 + 0] = m;
       sStat[(r * NHL + hl) * 3 + 1] = il;
       sStat[(r * NHL + hl) * 3 + 2] = Dv;
       store16_bf16(dqkv + (size_t)sTok[r] * (3 * D) + (hs * NHL + hl) * DH, dq);
     }
+    if (COS) {   // per-warp sums of the two heads (lanes of equal parity share a head)
+#pragma unroll
+      for (int o2 = 2; o2 < 32; o2 <<= 1) tsum += __shfl_xor_sync(0xffffffffu, tsum, o2);
+      if ((threadIdx.x & 31) < NHL) sTRed[(threadIdx.x >> 5) * NHL + (threadIdx.x & 31)] = tsum;
+    }
     __syncthreads();
+    if (COS && threadIdx.x < NHL) {
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; w++) t += sTRed[w * NHL + threadIdx.x];
+      sTAcc[hs * NHL + threadIdx.x] += t;
+    }
     // ---- pass B: per (key row, head)
     for (int it = threadIdx.x; it < nrow * NHL; it += blockDim.x) {
       const int r = it >> 1, hl = it & 1;
@@ -475,6 +567,11 @@ __global__ void __launch_bounds__(256) win_attn_bwd_kernel(const __half* __restr
       float k[16], v[16], dk[16], dv[16];
       load16_f16(sK + r * AB_LD + hl * DH, k);
       load16_f16(sV + r * AB_LD + hl * DH, v);
+      float ik = 1.f, cinv = 1.f;
+      if (COS) {
+        cinv = 1.0f / fmaxf(tau_n > 1 ? tau[hs * NHL + hl] : tau[0], tau_min);
+        ik = sInvK[hl * NROW + r];
+      }
 #pragma unroll
       for (int d = 0; d < 16; d++) dk[d] = dv[d] = 0.f;
       for (int i = kb; i < ke; i++) {
@@ -488,28 +585,85 @@ __global__ void __launch_bounds__(256) win_attn_bwd_kernel(const __half* __restr
           dp = fmaf(g[d], v[d], dp);
         }
         const float* st = sStat + (i * NHL + hl) * 3;
-        const float p = __expf(s * scale - st[0]) * st[1];
-        const float ds = p * (dp - st[2]) * scale;
+        float p, ds;
+        if (COS) {   // the logit exactly as pass A formed it: (q . k ik) (c iq)
+          const float iq = sInvQ[hl * NROW + i];
+          p = __expf((s * ik) * (cinv * iq) - st[0]) * st[1];
+          ds = p * (dp - st[2]) * (cinv * iq);   // dkh_j = c sum_i g_ij qh_i = sum_i (g_ij c iq_i) q_i
+        } else {
+          p = __expf(s * scale - st[0]) * st[1];
+          ds = p * (dp - st[2]) * scale;
+        }
 #pragma unroll
         for (int d = 0; d < 16; d++) {
           dk[d] = fmaf(ds, q[d], dk[d]);
           dv[d] = fmaf(p, g[d], dv[d]);
         }
       }
+      if (COS) {   // dk = ik (dkh - kh (kh . dkh))
+        float kd = 0.f;
+#pragma unroll
+        for (int d = 0; d < 16; d++) kd = fmaf(k[d], dk[d], kd);
+        const float t = kd * ik * ik;
+#pragma unroll
+        for (int d = 0; d < 16; d++) dk[d] = ik * fmaf(-k[d], t, dk[d]);
+      }
       __nv_bfloat16* dst = dqkv + (size_t)sTok[r] * (3 * D) + (hs * NHL + hl) * DH;
       store16_bf16(dst + D, dk);
       store16_bf16(dst + 2 * D, dv);
     }
   }
+  if (COS) {
+    __syncthreads();
+    if (threadIdx.x < 8) tau_part[blockIdx.x * 8 + threadIdx.x] = sTAcc[threadIdx.x];
+  }
+}
+
+// d tau[h] += -c_h^2 sum over the CTAs' partials (sum over all 8 heads when one tau is shared), c_h = 1 / max(tau_h, tau_min);
+// 0 where tau_h < tau_min (torch's clamp(min=) passes the gradient at equality).  Fixed summation order: reproducible.
+__global__ void tau_grad_kernel(const float* __restrict__ part, int nparts, const float* __restrict__ tau, int tau_n, float tau_min,
+                                float* __restrict__ dtau) {
+  pdl_wait();
+  pdl_launch();
+  const int h = threadIdx.x;
+  if (h >= tau_n) return;
+  const int h0 = tau_n > 1 ? h : 0, h1 = tau_n > 1 ? h + 1 : 8;
+  float s = 0.f;
+  for (int hh = h0; hh < h1; hh++) {
+    float sh = 0.f;
+    for (int b = 0; b < nparts; b++) sh += part[(size_t)b * 8 + hh];
+    s += sh;
+  }
+  const float t = tau[h];
+  if (t >= tau_min) {
+    const float cinv = 1.0f / t;
+    dtau[h] += -cinv * cinv * s;
+  }
 }
 
 static int launch_attn_bwd(sstb200_ctx* c, const __half* qkv, const __nv_bfloat16* att, const __nv_bfloat16* datt, const sstb200_sra_plan* P,
-                           __nv_bfloat16* dqkv) {
-  const size_t smem = (size_t)4 * ATT_BT * AB_LD * 2 + (size_t)ATT_BT * 2 * 3 * 4;
-  static SmemAttr sa;
-  CUDA_TRY(c, ensure_smem(c, sa, win_attn_bwd_kernel, smem));
-  CUDA_TRY(c, launch_pdl(win_attn_bwd_kernel, dim3(c->num_sms * 2), dim3(256), smem, c->stream, qkv, att, datt, P->num_windows_dev,
-                         P->win_offsets, P->win_batch, P->tok_perm, 0.25f, dqkv));
+                           const sstb200_sra_layer* L, float* dtau, __nv_bfloat16* dqkv) {
+  const int grid = c->num_sms * 2;
+  if (!L->tau) {
+    const size_t smem = attn_bwd_smem(false);
+    static SmemAttr sa;
+    CUDA_TRY(c, ensure_smem(c, sa, win_attn_bwd_kernel<false>, smem));
+    CUDA_TRY(c, launch_pdl(win_attn_bwd_kernel<false>, dim3(grid), dim3(256), smem, c->stream, qkv, att, datt, P->num_windows_dev, P->win_offsets,
+                           P->win_batch, P->tok_perm, 0.25f, dqkv, (const float*)nullptr, 0, 0.f, (float*)nullptr));
+    return SSTB_OK;
+  }
+  // per-CTA temperature partials in the arena; the reduce is enqueued before any later arena_reset can hand the memory out again
+  arena_reset(c);
+  int rc = arena_reserve(c, (size_t)grid * 8 * 4);
+  if (rc) return rc;
+  float* part = arena_alloc<float>(c, (size_t)grid * 8);
+  if (!part) return sstb_fail(c, SSTB_ERR_WORKSPACE, "tau partials: arena");
+  const size_t smem = attn_bwd_smem(true);
+  static SmemAttr sb;
+  CUDA_TRY(c, ensure_smem(c, sb, win_attn_bwd_kernel<true>, smem));
+  CUDA_TRY(c, launch_pdl(win_attn_bwd_kernel<true>, dim3(grid), dim3(256), smem, c->stream, qkv, att, datt, P->num_windows_dev, P->win_offsets,
+                         P->win_batch, P->tok_perm, 0.25f, dqkv, L->tau, (int)L->tau_n, L->tau_min, part));
+  CUDA_TRY(c, launch_pdl(tau_grad_kernel, dim3(1), dim3(32), (size_t)0, c->stream, (const float*)part, grid, L->tau, (int)L->tau_n, L->tau_min, dtau));
   return SSTB_OK;
 }
 
@@ -532,9 +686,10 @@ __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ p, const
 }
 
 static bool layer_ok(const sstb200_sra_layer* L, const sstb200_sra_plan* P) {
-  return L->d_model == DM && L->dim_ff == DFF && L->post_norm && !L->norm1_mean && L->act == 2 && !L->tau && L->nhead == 8 && L->in_proj_w_f16 &&
-         L->out_proj_w_f16 && L->lin1_w_f16 && L->lin2_w_f16 && P->max_window_tokens > 0 && P->max_window_tokens <= ATT_MAXT &&
-         P->num_windows_dev && P->win_batch && (!P->pos_table || P->pos_L % 8 == 0);
+  return L->d_model == DM && L->dim_ff == DFF && L->post_norm && !L->norm1_mean && L->act == 2 &&
+         (!L->tau || ((L->tau_n == 1 || L->tau_n == 8) && L->tau_min > 0.f)) && L->nhead == 8 && L->in_proj_w_f16 && L->out_proj_w_f16 &&
+         L->lin1_w_f16 && L->lin2_w_f16 && P->max_window_tokens > 0 && P->max_window_tokens <= ATT_MAXT && P->num_windows_dev && P->win_batch &&
+         (!P->pos_table || P->pos_L % 8 == 0);
 }
 
 }  // namespace
@@ -550,7 +705,9 @@ extern "C" int sstb200_sra_stack_forward_train(sstb200_ctx* c, const sstb200_sra
   const sstb200_sra_plan plans[2] = {*plan_shift0, *plan_shift1};
   for (int l = 0; l < num_layers; l++)
     if (!layer_ok(&layers[l], &plans[l & 1]))
-      return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "training path is built for d_model=128, dim_ff=256, 8 heads, post-norm LayerNorm, gelu, windows <= 144 tokens");
+      return sstb_fail(c, SSTB_ERR_UNSUPPORTED,
+                       "training path is built for d_model=128, dim_ff=256, 8 heads, post-norm LayerNorm, gelu, plain or cosine attention "
+                       "(1 or 8 temperatures, tau_min > 0), windows <= 144 tokens");
   const TrainWs w = train_ws(n, num_layers);
   uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
   const float* xin = x;
@@ -569,7 +726,7 @@ extern "C" int sstb200_sra_stack_forward_train(sstb200_ctx* c, const sstb200_sra
     if ((rc = launch_umma<128, 128, PRO_F32, EPI_F16, FMT_BF16>(c, g, 3))) return rc;
     // 2. attention (bf16 output)
     if ((rc = sstb_win_attn_batch(c, reinterpret_cast<const __half*>(lw + w.qkv), P->num_windows_dev, P->win_offsets, P->win_batch, n, P->tok_perm,
-                                  lw + w.att, /*out_bf16=*/true)))
+                                  lw + w.att, /*out_bf16=*/true, L->tau, L->tau_n, L->tau_min)))
       return rc;
     // 3. x1 = LN1(x + att Wo^T + bo), keep t1
     memset(&g, 0, sizeof(g));
@@ -596,6 +753,7 @@ extern "C" int sstb200_sra_stack_backward(sstb200_ctx* c, const sstb200_sra_laye
                                           const sstb200_sra_plan* plan_shift1, const float* x, void* workspace, const float* dy, float* dx,
                                           int n) {
   CHECK_ARG(c, c && layers && wt && grads && num_layers >= 1 && plan_shift0 && plan_shift1 && x && workspace && dy && dx && n >= 0);
+  for (int l = 0; l < num_layers; l++) CHECK_ARG(c, !layers[l].tau || grads[l].tau);   // cosine layers need their d tau accumulator
   if (n == 0) return SSTB_OK;
   const sstb200_sra_plan plans[2] = {*plan_shift0, *plan_shift1};
   const TrainWs w = train_ws(n, num_layers);
@@ -644,7 +802,8 @@ extern "C" int sstb200_sra_stack_backward(sstb200_ctx* c, const sstb200_sra_laye
     g.M_cap = n, g.A = dtb, g.lda = DM, g.W = T->out_proj_wt, g.bias = nullptr, g.out_h16 = dattb, g.ldo = DM;
     if ((rc = launch_umma<128, 128, PRO_H16, EPI_H16, FMT_BF16>(c, g, 1))) return rc;
     // attention'
-    if ((rc = launch_attn_bwd(c, reinterpret_cast<const __half*>(lw + w.qkv), reinterpret_cast<const __nv_bfloat16*>(lw + w.att), dattb, P, dqkv)))
+    if ((rc = launch_attn_bwd(c, reinterpret_cast<const __half*>(lw + w.qkv), reinterpret_cast<const __nv_bfloat16*>(lw + w.att), dattb, P, L, G->tau,
+                              dqkv)))
       return rc;
     // dWq|k += [dq|dk]^T (x + pos) ;  dWv += dv^T x ;  d bqkv += colsum(dqkv)
     if ((rc = launch_dw(c, dqkv, 3 * DM, 2 * DM, nullptr, xin, DM, DM, P->pos_table ? P : nullptr, G->in_proj_w, n, G->in_proj_b))) return rc;

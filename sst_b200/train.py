@@ -13,16 +13,13 @@ import torch
 
 from . import _lib as L
 
-_PARAMS_PER_LAYER = 12
-
-
 class _LayerWt(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in ("in_proj_wt", "out_proj_wt", "lin1_wt", "lin2_wt")]
 
 
 class _LayerGrads(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in ("in_proj_w", "in_proj_b", "out_proj_w", "out_proj_b", "lin1_w", "lin1_b", "lin2_w", "lin2_b",
-                                          "norm1_w", "norm1_b", "norm2_w", "norm2_b")]
+                                          "norm1_w", "norm1_b", "norm2_w", "norm2_b", "tau")]
 
 
 def _register():
@@ -40,10 +37,23 @@ _register()
 
 
 def layer_params(layer):
-    """The 12 parameters of an EncoderLayer in the order of sstb200_sra_layer_grads."""
+    """The parameters of an EncoderLayer in the order of sstb200_sra_layer_grads: 12, plus win_attn.self_attn.tau last for a
+    cosine-attention layer."""
     sa = layer.win_attn.self_attn
-    return [sa.in_proj_weight, sa.in_proj_bias, sa.out_proj.weight, sa.out_proj.bias, layer.linear1.weight, layer.linear1.bias,
-            layer.linear2.weight, layer.linear2.bias, layer.norm1.weight, layer.norm1.bias, layer.norm2.weight, layer.norm2.bias]
+    ps = [sa.in_proj_weight, sa.in_proj_bias, sa.out_proj.weight, sa.out_proj.bias, layer.linear1.weight, layer.linear1.bias,
+          layer.linear2.weight, layer.linear2.bias, layer.norm1.weight, layer.norm1.bias, layer.norm2.weight, layer.norm2.bias]
+    if layer.win_attn.cosine:
+        ps.append(sa.tau)
+    return ps
+
+
+def _param_offsets(layers):
+    """Start of every layer's parameters in the flat argument list of SraStackFunction."""
+    offs, o = [], 0
+    for layer in layers:
+        offs.append(o)
+        o += len(layer_params(layer))
+    return offs, o
 
 
 class SraStackFunction(torch.autograd.Function):
@@ -53,7 +63,8 @@ class SraStackFunction(torch.autograd.Function):
     def forward(ctx, x, layers, plans, make_plan, *params):
         from .sst_modules import _SraLayer
         _register()
-        assert len(params) == _PARAMS_PER_LAYER * len(layers)
+        offs, total = _param_offsets(layers)
+        assert len(params) == total
         dev = x.device
         x = x.detach().float().contiguous()
         n = x.shape[0]
@@ -61,7 +72,7 @@ class SraStackFunction(torch.autograd.Function):
         structs, keep = [], []
         for i, layer in enumerate(layers):
             s = layer._struct(0)                        # fp32 pointers, shapes, eps
-            w16 = [params[_PARAMS_PER_LAYER * i + j].detach().to(torch.bfloat16).contiguous() for j in (0, 2, 4, 6)]
+            w16 = [params[offs[i] + j].detach().to(torch.bfloat16).contiguous() for j in (0, 2, 4, 6)]
             s.in_proj_w_f16, s.out_proj_w_f16, s.lin1_w_f16, s.lin2_w_f16 = [w.data_ptr() for w in w16]
             structs.append(s)
             keep.append(w16)
@@ -85,6 +96,7 @@ class SraStackFunction(torch.autograd.Function):
         n = x.shape[0]
         lib, c = L.lib(), L.ctx(dev)
         dy = dy.detach().float().contiguous()
+        offs, _ = _param_offsets(layers)
         structs, wts, grads, gstructs, keep = [], [], [], [], []
         for i, layer in enumerate(layers):
             s = layer._struct(0)
@@ -94,7 +106,7 @@ class SraStackFunction(torch.autograd.Function):
             wt = [w.t().contiguous() for w in w16]          # bf16 [in, out]
             keep.append(wt)
             wts.append(_LayerWt(*[w.data_ptr() for w in wt]))
-            g = [torch.zeros_like(params[_PARAMS_PER_LAYER * i + j], dtype=torch.float32) for j in range(_PARAMS_PER_LAYER)]
+            g = [torch.zeros_like(params[offs[i] + j], dtype=torch.float32) for j in range(len(layer_params(layer)))]
             grads.extend(g)
             gstructs.append(_LayerGrads(*[t.data_ptr() for t in g]))
         arr = (_SraLayer * len(layers))(*structs)
@@ -111,25 +123,28 @@ class SraStackFunction(torch.autograd.Function):
 class FlatAdamW:
     """AdamW over ONE flat fp32 buffer that the parameters are views of (so a single NCCL all-reduce covers every gradient and a
     single kernel does the update).  `params`: iterable of leaf tensors on one CUDA device; after construction each p.data and
-    p.grad is a view into .flat / .flat_grad."""
+    p.grad is a view into .flat / .flat_grad.  Every view starts on a 16-byte boundary (the kernels read parameters such as LayerNorm
+    weights as float4), so a parameter whose size is not a multiple of 4 (e.g. a cosine-attention layer's one-element tau) is followed
+    by zero padding; padding has zero gradient and stays zero under the update."""
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01):
         _register()
         self.params = [p for p in params if p.requires_grad]
         dev = self.params[0].device
-        n = sum(p.numel() for p in self.params)
-        self.flat = torch.empty((n,), dtype=torch.float32, device=dev)
+        offs, n = [], 0
+        for p in self.params:
+            offs.append(n)
+            n += (p.numel() + 3) // 4 * 4
+        self.flat = torch.zeros((n,), dtype=torch.float32, device=dev)
         self.flat_grad = torch.zeros((n,), dtype=torch.float32, device=dev)
         self.m = torch.zeros_like(self.flat)
         self.v = torch.zeros_like(self.flat)
-        o = 0
         with torch.no_grad():
-            for p in self.params:
+            for p, o in zip(self.params, offs):
                 k = p.numel()
                 self.flat[o:o + k].copy_(p.detach().reshape(-1))
                 p.data = self.flat[o:o + k].view_as(p)
                 p.grad = self.flat_grad[o:o + k].view_as(p)
-                o += k
         self.lr, self.betas, self.eps, self.wd, self.t = lr, betas, eps, weight_decay, 0
 
     def zero_grad(self):
