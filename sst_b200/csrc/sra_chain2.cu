@@ -8,15 +8,24 @@
 // replaces mmdet3d/models/sst/sst_basic_block_v2.py:104-126 (+ the in-projection of the following layer's
 // nn.MultiheadAttention, :70) for one 128-token tile per iteration of a persistent CTA.
 //
-// Two warpgroups, each owning 64 rows of the tile, issue wgmma.mma_async (fp16 operands, fp32 accumulators in registers).  The att
-// tile and every weight arrive by cp.async.bulk.tensor (TMA) into 128B-swizzled shared memory: weights stream as 32 KB chunks
-// ([128 rows x 128 K]) through a ring of two slots with full mbarriers, and one thread refills a slot with the chunk two ahead (also
-// across tiles) as soon as both warpgroups have retired the MMAs that read it, so weight loads overlap the next GEMM and its
-// epilogue.  Epilogues run on the accumulator fragments: a row's 128 columns sit in one lane quad, so LayerNorm statistics take
-// two xor-shuffles; x1 stays in registers from GEMM1 to GEMM3; x1, h, y and y + pos reach the next GEMM as 16-bit operands written
-// straight into the swizzled K-major layout.  Only x (residual), y and q|k|v touch global memory.  All rows are in flat token order.
+// Two warpgroups, each owning 64 rows of the tile, issue wgmma.mma_async (fp16 operands, fp32 accumulators in registers) in
+// ping-pong: both consume one sequence of weight chunks in the same order, and warpgroup 1 issues its MMA on a chunk only after
+// warpgroup 0's MMA on it has retired, so one warpgroup's epilogue (bias, residual, LayerNorm, GELU, positional add, stores) runs
+// while the other's MMA occupies the tensor core.  Weights arrive by cp.async.bulk.tensor (TMA) as 32 KB chunks ([128 rows x
+// 128 K]) into a ring of three 128B-swizzled slots with per-slot mbarriers: "full" (TMA bytes landed) and "warpgroup 0 done".
+// Warpgroup 1 is the last reader of every slot; one of its threads refills the slot with the chunk three ahead (also across
+// tiles), which by itself bounds how far warpgroup 0 runs ahead.  Each warpgroup streams its own 64-row half of the attention
+// tile by TMA, issued one tile ahead, and loads its residual rows and positional codes while its GEMM1 is in flight.  The
+// scheduling unit stays the 128-row tile: both warpgroups walk every tile of the CTA and wait on and release every chunk, also
+// when their half has no valid rows.  Inside a warpgroup, epilogue writes that feed the next wgmma are ordered by
+// fence.proxy.async and a named barrier; the tile loop has no CTA-wide barrier.
+// Epilogues run on the accumulator fragments: a row's 128 columns sit in one lane quad, so LayerNorm statistics take two
+// xor-shuffles; x1 stays in registers from GEMM1 to GEMM3; x1, h, y and y + pos reach the next GEMM as 16-bit operands written
+// straight into the swizzled K-major layout.  Only x (residual), y and q|k|v touch global memory; q|k|v leave as 16-byte stores
+// after a transpose inside each lane quad (whole 32-byte sectors per warp store).  All rows are in flat token order.
 //
-// Shared memory: A 32 KB (att, then x1, then y) | P 32 KB (y + pos) | H 64 KB (hidden, four K = 64 blocks) | ring 2 x 32 KB.
+// Shared memory, per warpgroup (64 rows, K-major, 128B swizzle, 8 KB per 64-wide K block): X 16 KB (x1, then y) | T 16 KB (att) |
+// H 32 KB (hidden, four K blocks; y + pos aliased onto its first 16 KB once GEMM3 has retired); then the ring, 3 x 32 KB.
 #include <stdarg.h>
 #include <cuda_fp16.h>
 #include "sra.cuh"
@@ -25,12 +34,16 @@
 
 namespace {
 
-constexpr int TM = 128, D = 128;
+constexpr int TM = 128, HM = 64, D = 128;
 constexpr int SLOT = 32768;   // one weight chunk: 128 rows x 128 K fp16 = two 64-wide swizzle blocks of 16 KB
-constexpr int OFF_A = 0, OFF_P = SLOT, OFF_H = 2 * SLOT, OFF_RING = 4 * SLOT;
-constexpr int SMEM_BYTES = 6 * SLOT + 1024;
+constexpr int NSLOT = 3;
+constexpr int WG_BYTES = 2 * SLOT;   // one warpgroup's operands
+constexpr int OFF_X = 0, OFF_T = SLOT / 2, OFF_H = SLOT, OFF_RING = 2 * WG_BYTES;
+constexpr int SMEM_BYTES = OFF_RING + NSLOT * SLOT + 1024;
+static_assert(SMEM_BYTES <= 232448, "sra_chain2 shared memory exceeds the sm_90 per-block limit");
 constexpr int NTHR = 256;
-constexpr uint32_t OPB = TM * 128;   // byte pitch of one 64-wide K block of a 128-row operand
+constexpr uint32_t OPB = TM * 128;   // byte pitch of one 64-wide K block of a weight chunk (128 rows)
+constexpr uint32_t OPH = HM * 128;   // byte pitch of one 64-wide K block of a warpgroup's 64-row operand
 
 struct Chain2Maps {
   CUtensorMap att, wo, w1, w2, wqkv;
@@ -64,9 +77,9 @@ __device__ __forceinline__ void issue_chunk(const Chain2Maps& m, int j, uint32_t
   tma_load_2d(dst + SLOT / 2, map, k0 + 64, n0, bar);
 }
 
-// 16-bit pair (columns k, k + 1) of row `row` into a 128-row K-major SWIZZLE_128B operand
-__device__ __forceinline__ void st_op(uint8_t* buf, int row, int k, uint32_t v) {
-  *reinterpret_cast<uint32_t*>(buf + (k >> 6) * OPB + row * 128 + ((((k & 63) >> 3) ^ (row & 7)) << 4) + (k & 7) * 2) = v;
+// 16-bit pair (columns k, k + 1) of row `row` into a 64-row K-major SWIZZLE_128B operand
+__device__ __forceinline__ void st_op(uint32_t buf, int row, int k, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(buf + (k >> 6) * OPH + row * 128 + ((((k & 63) >> 3) ^ (row & 7)) << 4) + (k & 7) * 2), "r"(v) : "memory");
 }
 
 // t = fragment of [64 rows x 128] (rows ra: t[4j], t[4j+1]; rb: t[4j+2], t[4j+3]; columns 8j + 2 (lane & 3)): per-row normalisation
@@ -104,6 +117,28 @@ __device__ __forceinline__ void row_norm(float (&t)[64], const float* __restrict
   }
 }
 
+// One row's 128 fp16 outputs held by a lane quad as 16 packed pairs (pair j: columns 8j + 2 (lane & 3), 8j + 2 (lane & 3) + 1).
+// A 4 x 4 transpose of each group of four pairs inside the quad gives every lane 8 consecutive columns, so each lane stores 16 B
+// and a warp writes whole 32-byte sectors instead of 4-byte pieces of them.  All lanes shuffle; `ok` only gates the stores.
+__device__ __forceinline__ void st_row_f16(__half* row, const uint32_t (&p)[16], bool ok) {
+  const int qd = threadIdx.x & 3;
+  const bool o = qd & 1, t = qd & 2;
+#pragma unroll
+  for (int m = 0; m < 4; m++) {
+    uint32_t v0 = p[4 * m], v1 = p[4 * m + 1], v2 = p[4 * m + 2], v3 = p[4 * m + 3];
+    // exchange across lane bit 0, then bit 1: afterwards slot k of lane qd holds lane k's pair of group 4m + qd
+    uint32_t r = __shfl_xor_sync(0xffffffffu, o ? v0 : v1, 1);
+    if (o) v0 = r; else v1 = r;
+    r = __shfl_xor_sync(0xffffffffu, o ? v2 : v3, 1);
+    if (o) v2 = r; else v3 = r;
+    r = __shfl_xor_sync(0xffffffffu, t ? v0 : v2, 2);
+    if (t) v0 = r; else v2 = r;
+    r = __shfl_xor_sync(0xffffffffu, t ? v1 : v3, 2);
+    if (t) v1 = r; else v3 = r;
+    if (ok) *reinterpret_cast<uint4*>(row + 8 * (4 * m + qd)) = make_uint4(v0, v1, v2, v3);
+  }
+}
+
 __device__ __forceinline__ float2 pos_pair(const Chain2Args& g, int code, int c) {
   const int axis = c / g.posL;   // posL % 32 == 0: the pair lies inside one axis
   if (axis >= g.pos_ndim) return make_float2(0.f, 0.f);
@@ -117,107 +152,148 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
   pdl_launch();
   extern __shared__ uint8_t chain_raw[];
   uint8_t* base = (uint8_t*)(((uintptr_t)chain_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* pA = base + OFF_A;
-  uint8_t* pP = base + OFF_P;
-  uint8_t* pH = base + OFF_H;
-  const uint32_t sA = smem_u32(pA), sP = smem_u32(pP), sH = smem_u32(pH), sR = smem_u32(base + OFF_RING);
-  __shared__ __align__(8) uint64_t bar_full[2], bar_att;
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
+  const uint32_t sX = smem_u32(base + wg * WG_BYTES + OFF_X), sT = smem_u32(base + wg * WG_BYTES + OFF_T);
+  const uint32_t sH = smem_u32(base + wg * WG_BYTES + OFF_H), sR = smem_u32(base + OFF_RING);
+  __shared__ __align__(8) uint64_t bar_full[NSLOT], bar_wg0[NSLOT], bar_att[2];
   constexpr int NCH = TAIL ? 8 : 5;
 
-  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
   const int M = g.M_dev ? *g.M_dev : g.M_cap;
   const int ntiles = (M + TM - 1) / TM;
   if ((int)blockIdx.x >= ntiles) return;   // uniform per CTA, nothing issued yet
   // chunk `n` (counted over the CTA's whole tile sequence) belongs to a tile this CTA will process
   auto chunk_live = [&](int n) { return (int)blockIdx.x + (n / NCH) * (int)gridDim.x < ntiles; };
+  const bool leader = (tid & 127) == 0;   // one elected thread per warpgroup
+  // this warpgroup's half of the attention tile `tile`; a half that lies wholly past the tensor's rows only completes the phase
+  auto issue_att = [&](int tile) {
+    const uint32_t bar = smem_u32(&bar_att[wg]);
+    const int r0 = tile * TM + wg * HM;
+    if (r0 < g.M_cap) {
+      mbar_expect_tx(bar, SLOT / 2);
+      tma_load_2d(sT, &m.att, 0, r0, bar);
+      tma_load_2d(sT + OPH, &m.att, 64, r0, bar);
+    } else {
+      mbar_arrive(bar);
+    }
+  };
   if (tid == 0) {
-    mbar_init(smem_u32(&bar_full[0]), 1);
-    mbar_init(smem_u32(&bar_full[1]), 1);
-    mbar_init(smem_u32(&bar_att), 1);
+    for (int s = 0; s < NSLOT; s++) {
+      mbar_init(smem_u32(&bar_full[s]), 1);
+      mbar_init(smem_u32(&bar_wg0[s]), 1);
+    }
+    mbar_init(smem_u32(&bar_att[0]), 1);
+    mbar_init(smem_u32(&bar_att[1]), 1);
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    for (int n = 0; n < 2; n++)
+    for (int n = 0; n < NSLOT; n++)
       if (chunk_live(n)) issue_chunk(m, n % NCH, sR + n * SLOT, smem_u32(&bar_full[n]));
   }
   __syncthreads();
+  if (leader) issue_att(blockIdx.x);
 
   int gc = 0;   // weight chunks consumed
-  auto wait_chunk = [&]() -> uint32_t {
-    mbar_wait(smem_u32(&bar_full[gc & 1]), (uint32_t)((gc >> 1) & 1));
-    return sR + (gc & 1) * SLOT;
+  // slot of chunk gc + i once it has landed; warpgroup 1 also waits until warpgroup 0's MMA on it has retired
+  auto acquire = [&](int i) -> uint32_t {
+    const int n = gc + i, s = n % NSLOT;
+    const uint32_t par = (uint32_t)((n / NSLOT) & 1);
+    mbar_wait(smem_u32(&bar_full[s]), par);
+    if (wg == 1) mbar_wait(smem_u32(&bar_wg0[s]), par);
+    return sR + s * SLOT;
   };
-  // after wgmma_wait<0> in every thread: the slot is free once all threads pass the barrier; refill it with the chunk two ahead
-  auto release_chunk = [&]() {
-    __syncthreads();
-    if (tid == 0 && chunk_live(gc + 2)) issue_chunk(m, (gc + 2) % NCH, sR + (gc & 1) * SLOT, smem_u32(&bar_full[gc & 1]));
-    gc++;
+  // after wgmma_wait<0>: once every warp of the warpgroup has passed the barrier, its MMAs have retired, so its own operand
+  // buffers may be overwritten and the next `cnt` chunks released.  Warpgroup 0 signals it is done with them; warpgroup 1,
+  // their last reader, refills each slot with the chunk three ahead.
+  auto release = [&](int cnt) {
+    named_bar_sync(1 + wg, 128);
+    if (wg == 0) {
+      if (leader)
+        for (int i = 0; i < cnt; i++) mbar_arrive(smem_u32(&bar_wg0[(gc + i) % NSLOT]));
+    } else {
+      if (leader)
+        for (int i = 0; i < cnt; i++)
+          if (chunk_live(gc + i + NSLOT)) {
+            const int s = (gc + i) % NSLOT;
+            issue_chunk(m, (gc + i + NSLOT) % NCH, sR + s * SLOT, smem_u32(&bar_full[s]));
+          }
+    }
+    gc += cnt;
+  };
+  auto wg_sync = [&]() {   // this warpgroup's generic-proxy shared-memory writes -> its next wgmma
+    fence_async_smem();
+    named_bar_sync(1 + wg, 128);
   };
 
-  const int rl = 64 * wg + 16 * ((tid >> 5) & 3) + (lane >> 2);   // fragment rows rl, rl + 8 of the tile
+  const int rl = 16 * ((tid >> 5) & 3) + (lane >> 2);   // fragment rows rl, rl + 8 of this warpgroup's half
   const int cq = 2 * (lane & 3);
   uint32_t att_par = 0;
   float acc[64], x1[64];
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int row0 = tile * TM;
-    const int rowA = row0 + rl, rowB = rowA + 8;
+    const int rowA = tile * TM + wg * HM + rl, rowB = rowA + 8;
     const bool okA = rowA < M, okB = rowB < M;
-    fence_async_smem();   // the previous tile's generic-proxy writes of A precede the TMA that overwrites it
-    __syncthreads();
-    if (tid == 0) {
-      mbar_expect_tx(smem_u32(&bar_att), SLOT);
-      tma_load_2d(sA, &m.att, 0, row0, smem_u32(&bar_att));
-      tma_load_2d(sA + SLOT / 2, &m.att, 64, row0, smem_u32(&bar_att));
-    }
-    mbar_wait(smem_u32(&bar_att), att_par);
-    att_par ^= 1u;
 
-    // ---- GEMM1 + bias + residual + Norm1 -> x1 (registers, and fp16 into A) -----------------------------------------------------
-    wg_tile_mma<128, false, 8>(acc, sA + wg * 64 * 128, OPB, wait_chunk(), OPB, false);
+    // ---- GEMM1 + bias + residual + Norm1 -> x1 (registers, and fp16 into X) -----------------------------------------------------
+    {
+      const uint32_t w = acquire(0);
+      mbar_wait(smem_u32(&bar_att[wg]), att_par);
+      att_par ^= 1u;
+      wg_tile_mma<128, false, 8>(acc, sT, OPH, w, OPB, false);
+    }
+    // residual rows and positional codes load while the MMA runs
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+      const int c = 8 * j + cq;
+      const float2 ra = okA ? *reinterpret_cast<const float2*>(g.x + (size_t)rowA * D + c) : make_float2(0.f, 0.f);
+      const float2 rb = okB ? *reinterpret_cast<const float2*>(g.x + (size_t)rowB * D + c) : make_float2(0.f, 0.f);
+      x1[4 * j] = ra.x, x1[4 * j + 1] = ra.y, x1[4 * j + 2] = rb.x, x1[4 * j + 3] = rb.y;
+    }
+    int codeA = 0, codeB = 0;
+    if (TAIL) {
+      codeA = okA ? g.pos_code[rowA] : 0;
+      codeB = okB ? g.pos_code[rowB] : 0;
+    }
     wgmma_wait<0>();
-    release_chunk();   // also: both warpgroups are done with att in A
+    release(1);
 #pragma unroll
     for (int j = 0; j < 16; j++) {
       const int c = 8 * j + cq;
       const float2 b = __ldg(reinterpret_cast<const float2*>(g.bo + c));
-      const float2 ra = okA ? *reinterpret_cast<const float2*>(g.x + (size_t)rowA * D + c) : make_float2(0.f, 0.f);
-      const float2 rb = okB ? *reinterpret_cast<const float2*>(g.x + (size_t)rowB * D + c) : make_float2(0.f, 0.f);
-      x1[4 * j] = acc[4 * j] + b.x + ra.x;
-      x1[4 * j + 1] = acc[4 * j + 1] + b.y + ra.y;
-      x1[4 * j + 2] = acc[4 * j + 2] + b.x + rb.x;
-      x1[4 * j + 3] = acc[4 * j + 3] + b.y + rb.y;
+      x1[4 * j] = acc[4 * j] + b.x + x1[4 * j];
+      x1[4 * j + 1] = acc[4 * j + 1] + b.y + x1[4 * j + 1];
+      x1[4 * j + 2] = acc[4 * j + 2] + b.x + x1[4 * j + 2];
+      x1[4 * j + 3] = acc[4 * j + 3] + b.y + x1[4 * j + 3];
     }
     row_norm(x1, g.g1, g.be1, g.eps, g.affine);
 #pragma unroll
     for (int j = 0; j < 16; j++) {
       const int c = 8 * j + cq;
-      st_op(pA, rl, c, pack_f16(x1[4 * j], x1[4 * j + 1]));
-      st_op(pA, rl + 8, c, pack_f16(x1[4 * j + 2], x1[4 * j + 3]));
+      st_op(sX, rl, c, pack_f16(x1[4 * j], x1[4 * j + 1]));
+      st_op(sX, rl + 8, c, pack_f16(x1[4 * j + 2], x1[4 * j + 3]));
     }
-    fence_async_smem();
-    __syncthreads();
+    wg_sync();   // also: every warp of this warpgroup has retired GEMM1, so T is free for the next tile's attention half
+    if (leader && tile + (int)gridDim.x < ntiles) issue_att(tile + gridDim.x);
 
     // ---- GEMM2 + bias + GELU -> h (fp16 into H) -----------------------------------------------------------------------------------
 #pragma unroll 1
     for (int h = 0; h < 2; h++) {
-      wg_tile_mma<128, false, 8>(acc, sA + wg * 64 * 128, OPB, wait_chunk(), OPB, false);
+      wg_tile_mma<128, false, 8>(acc, sX, OPH, acquire(0), OPB, false);
       wgmma_wait<0>();
-      release_chunk();
+      release(1);
 #pragma unroll
       for (int j = 0; j < 16; j++) {
         const int c = 8 * j + cq;
         const float2 b = __ldg(reinterpret_cast<const float2*>(g.b1 + 128 * h + c));
-        st_op(pH, rl, 128 * h + c, pack_f16(gelu_fast(acc[4 * j] + b.x), gelu_fast(acc[4 * j + 1] + b.y)));
-        st_op(pH, rl + 8, 128 * h + c, pack_f16(gelu_fast(acc[4 * j + 2] + b.x), gelu_fast(acc[4 * j + 3] + b.y)));
+        st_op(sH, rl, 128 * h + c, pack_f16(gelu_fast(acc[4 * j] + b.x), gelu_fast(acc[4 * j + 1] + b.y)));
+        st_op(sH, rl + 8, 128 * h + c, pack_f16(gelu_fast(acc[4 * j + 2] + b.x), gelu_fast(acc[4 * j + 3] + b.y)));
       }
     }
-    fence_async_smem();
-    __syncthreads();
+    wg_sync();
 
-    // ---- GEMM3 + bias + x1 + Norm2 -> y (fp32 rows; fp16 y and y + pos into A / P for the tail) -----------------------------------
-#pragma unroll 1
-    for (int kc = 0; kc < 2; kc++) {
-      wg_tile_mma<128, false, 8>(acc, sH + kc * 2 * OPB + wg * 64 * 128, OPB, wait_chunk(), OPB, kc > 0);
+    // ---- GEMM3 (both K chunks back to back) + bias + x1 + Norm2 -> y (fp32 rows; fp16 y into X and y + pos into H for the tail) --
+    {
+      const uint32_t w0 = acquire(0), w1 = acquire(1);
+      wg_tile_mma<128, false, 8>(acc, sH, OPH, w0, OPB, false);
+      wg_tile_mma<128, false, 8>(acc, sH + 2 * OPH, OPH, w1, OPB, true);
       wgmma_wait<0>();
-      release_chunk();
+      release(2);
     }
 #pragma unroll
     for (int j = 0; j < 16; j++) {
@@ -229,41 +305,38 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
       acc[4 * j + 3] += b.y + x1[4 * j + 3];
     }
     row_norm(acc, g.g2, g.be2, g.eps, g.affine);
-    int codeA = 0, codeB = 0;
-    if (TAIL) {
-      codeA = okA ? g.pos_code[rowA] : 0;
-      codeB = okB ? g.pos_code[rowB] : 0;
-    }
 #pragma unroll
     for (int j = 0; j < 16; j++) {
       const int c = 8 * j + cq;
       if (okA) *reinterpret_cast<float2*>(g.y + (size_t)rowA * D + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
       if (okB) *reinterpret_cast<float2*>(g.y + (size_t)rowB * D + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       if (TAIL) {
-        st_op(pA, rl, c, pack_f16(acc[4 * j], acc[4 * j + 1]));
-        st_op(pA, rl + 8, c, pack_f16(acc[4 * j + 2], acc[4 * j + 3]));
+        st_op(sX, rl, c, pack_f16(acc[4 * j], acc[4 * j + 1]));
+        st_op(sX, rl + 8, c, pack_f16(acc[4 * j + 2], acc[4 * j + 3]));
         const float2 pa = pos_pair(g, codeA, c), pb = pos_pair(g, codeB, c);
-        st_op(pP, rl, c, pack_f16(acc[4 * j] + pa.x, acc[4 * j + 1] + pa.y));
-        st_op(pP, rl + 8, c, pack_f16(acc[4 * j + 2] + pb.x, acc[4 * j + 3] + pb.y));
+        st_op(sH, rl, c, pack_f16(acc[4 * j] + pa.x, acc[4 * j + 1] + pa.y));
+        st_op(sH, rl + 8, c, pack_f16(acc[4 * j + 2] + pb.x, acc[4 * j + 3] + pb.y));
       }
     }
     if (!TAIL) continue;
-    fence_async_smem();
-    __syncthreads();
+    wg_sync();
 
     // ---- GEMM4: next layer's q|k (from y + pos) and v (from y) + bias -> fp16 rows ------------------------------------------------
 #pragma unroll 1
     for (int q = 0; q < 3; q++) {
-      wg_tile_mma<128, false, 8>(acc, (q < 2 ? sP : sA) + wg * 64 * 128, OPB, wait_chunk(), OPB, false);
+      wg_tile_mma<128, false, 8>(acc, q < 2 ? sH : sX, OPH, acquire(0), OPB, false);
       wgmma_wait<0>();
-      release_chunk();
+      release(1);
+      uint32_t pa[16], pb[16];
 #pragma unroll
       for (int j = 0; j < 16; j++) {
         const int c = 8 * j + cq;
         const float2 b = __ldg(reinterpret_cast<const float2*>(g.bqkv + 128 * q + c));
-        if (okA) *reinterpret_cast<uint32_t*>(g.qkv + (size_t)rowA * 3 * D + 128 * q + c) = pack_f16(acc[4 * j] + b.x, acc[4 * j + 1] + b.y);
-        if (okB) *reinterpret_cast<uint32_t*>(g.qkv + (size_t)rowB * 3 * D + 128 * q + c) = pack_f16(acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y);
+        pa[j] = pack_f16(acc[4 * j] + b.x, acc[4 * j + 1] + b.y);
+        pb[j] = pack_f16(acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y);
       }
+      st_row_f16(g.qkv + (size_t)rowA * 3 * D + 128 * q, pa, okA);
+      st_row_f16(g.qkv + (size_t)rowB * 3 * D + 128 * q, pb, okB);
     }
   }
 }
@@ -316,7 +389,7 @@ int sstb_sra_chain2(sstb200_ctx* c, const sstb200_sra_layer* L, const __half* at
                next_plan->pos_ndim > 3))
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "fused QKV tail needs the next plan's positional table with a per-axis length that is a multiple of 32");
   int rc = 0;
-  rc |= tmap_2d_sw128(&maps.att, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, att, 128, (uint64_t)n_cap, 256, 64, 128);
+  rc |= tmap_2d_sw128(&maps.att, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, att, 128, (uint64_t)n_cap, 256, 64, HM);   // per-warpgroup halves
   rc |= tmap_2d_sw128(&maps.wo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L->out_proj_w_f16, 128, 128, 256, 64, 128);
   rc |= tmap_2d_sw128(&maps.w1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L->lin1_w_f16, 128, 256, 256, 64, 128);
   rc |= tmap_2d_sw128(&maps.w2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L->lin2_w_f16, 256, 128, 512, 64, 128);
