@@ -430,6 +430,34 @@ int sstb200_connected_components(sstb200_ctx* ctx, const float* centers, int str
                                  float dist, const float xy_min[2], const float xy_max[2], int32_t* labels,
                                  int32_t* num_components_dev, int32_t* num_components_host);
 
+/* ---- next-3 (SURVEY 8f): FSD RoI point pooling.  dynamic_point_pool / dynamic_point_pool_mixed (mmdet3d/ops/dynamic_point_pool_op.py:9-113,
+ * kernel in TorchEx's unvendored dynamic_point_pool_ext) as used by DynamicPointROIExtractor (models/roi_heads/roi_extractors/
+ * dynamic_point_roi_extractor.py:32-136).  rois [num_rois, 7] fp32 = (x, y, z_bottom, w, l, h, rz) mmdet3d-0.15 LiDAR boxes; pts [num_pts, 3].
+ * rois_batch / pts_batch: int32 batch ids (>= 0) or both NULL (one sample); a point pairs only with RoIs of its own batch id.
+ * In-box test: check_pt_in_box3d of mmdet3d/ops/roiaware_pool3d/src/points_in_boxes_cuda.cu:24-49 as the same float expressions (centre
+ * z = bottom + h/2, |z - cz| > h/2 rejects, angle rz + pi/2, strict |local x| < l/2, |local y| < w/2).
+ * Output rows (pair = point inside the ENLARGED box): out_pts_idx int64, out_roi_idx int64, out_feats fp32 [., 13] = point xyz,
+ * local xyz, boundary offsets [6], is_in_margin.  Pinned by the reference: the layout, off[0]+off[3] = l, off[1]+off[4] = w,
+ * off[2]+off[5] = h, xyz = pts[idx], and one fake row (-1, -1, zeros) when nothing pairs.
+ * Chosen here (TorchEx's source is not available; the offset order and the origin of local z feed FullySparseBboxHead's f_cluster and are
+ * UNVERIFIED against TorchEx, so a checkpoint trained with it may see different features):
+ *   - enlarged box: same centre and yaw, dims (w + e0, l + e1, h + e2), i.e. the box (x, y, z_bottom - e2/2, w + e0, l + e1, h + e2, rz);
+ *   - is_in_margin = 1 inside the enlarged box but outside the original one, else 0;
+ *   - local xyz = (local x, local y, z - centre z): local z from the box CENTRE;
+ *   - offsets = (l/2 + lx, w/2 + ly, h/2 + lz, l/2 - lx, w/2 - ly, h/2 - lz) against the ORIGINAL box (negative in the margin);
+ *   - rows sorted by RoI, then point index; every RoI keeps its first max_inbox_point (1..8192) points in input order.  Deterministic:
+ *     two calls give bit-identical results (the reference assigns slots with atomics, so its choice and order vary from run to run);
+ *   - capacity: pairs beyond max_all_pts (>= 1) are dropped in (RoI, point) order.  per_sample = 0: max_all_pts and the fake row apply
+ *     to the whole call (outputs hold max_all_pts rows; no RoI at all gives no row).  per_sample = 1 (batch ids required, RoIs grouped by
+ *     ascending batch id): they apply to every sample, i.e. every run of equal RoI batch ids, its fake row placed where its rows would
+ *     be - the per-sample loop of DynamicPointROIExtractor in one call; outputs hold max_all_pts x (number of samples) rows.
+ * num_out_dev: rows written.  num_pairs_host (int32[3]) != NULL: one stream sync, then [0] rows written, [1] pairs found (at most
+ * max_inbox_point per RoI), [2] pairs written; a negative batch id, or RoIs not grouped in per-sample mode, is then an error. */
+int sstb200_dynamic_point_pool(sstb200_ctx* ctx, const float* rois, const int32_t* rois_batch, int num_rois, const float* pts,
+                               const int32_t* pts_batch, int num_pts, const float extra_wlh[3], int max_inbox_point, int max_all_pts,
+                               int per_sample, int64_t* out_pts_idx, int64_t* out_roi_idx, float* out_feats, int32_t* num_out_dev,
+                               int32_t* num_pairs_host);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,5 +1,5 @@
-"""FSD instance grouping on libsstb200 (SURVEY 8f next-3): the connected-components step between the segmentation / voting head and the
-SIR backbone.  Mirrors mmdet3d/models/detectors/single_stage_fsd.py:28-81 (filter_almost_empty, find_connected_componets*),
+"""FSD on libsstb200 (SURVEY 8f next-3): the instance grouping between the segmentation / voting head and the SIR backbone, and the RoI
+point pooling of the second stage (DynamicPointROIExtractor, at the end of this file).  Mirrors mmdet3d/models/detectors/single_stage_fsd.py:28-81 (filter_almost_empty, find_connected_componets*),
 :144-151 (modify_cluster_by_class) and :922-999 (ClusterAssigner) by name, arguments and return values.
 
 The reference builds a dense n x n distance matrix per sample and labels it with scipy on the CPU (training and, by default, eval;
@@ -12,7 +12,9 @@ import torch
 from torch import nn
 
 from . import _lib as L
+from . import ops
 from .ops import scatter_v2, unique_rows
+from .registry import ROI_EXTRACTORS
 
 L.SIGNATURES["sstb200_connected_components"] = (C.c_int, [L.vp, L.vp, C.c_int, L.vp, C.c_int, C.c_int, C.c_float, L.P_f32, L.P_f32, L.vp, L.vp,
                                                          L.P_i32])
@@ -121,3 +123,70 @@ class ClusterAssigner(nn.Module):
         assert len(cluster_inds) == len(sampled_centers)
         cluster_inds_per_point = torch.stack([batch_idx, cluster_inds[inv_inds]], 1)
         return cluster_inds_per_point, valid_mask
+
+
+@ROI_EXTRACTORS.register_module()
+class DynamicPointROIExtractor(nn.Module):
+    """dynamic_point_roi_extractor.py:9-136: the points of every RoI of FSD's second stage (roi_head of configs/fsd), through
+    sstb200_dynamic_point_pool.  Returns (point index, RoI index, dict(local_xyz, boundary_offset, is_in_margin)).
+
+    The reference loops over the samples, one op call each, adding running point / RoI bases.  Here the samples go through ONE call
+    whose capacity (max_all_pts) and fake row (-1, -1, zeros for a sample without any pair) apply per sample, which gives the loop's
+    output row for row.  As in the reference, every sample needs a RoI and a point, and the points are sorted by batch; the RoIs
+    must be too (rois[:, 0] ascending), or the reference's bases would index the wrong rows."""
+
+    def __init__(self, init_cfg=None, debug=True, extra_wlh=[0, 0, 0], max_inbox_point=512, max_all_pts=50000):
+        super().__init__()
+        self.init_cfg = init_cfg
+        self.debug = debug
+        self.extra_wlh = extra_wlh
+        self.max_inbox_point = max_inbox_point
+        self.max_all_pts = max_all_pts
+
+    def forward(self, pts_xyz, batch_inds, rois, max_inbox_point=None, batch_size=None):
+        if batch_size == 1:
+            return self.fast_single_sample_forward(pts_xyz, rois, max_inbox_point)
+        if not (pts_xyz.is_cuda and batch_inds.is_cuda and rois.is_cuda):
+            raise L.SSTB200Error("sst_b200 DynamicPointROIExtractor needs CUDA tensors (no CPU fallback)")
+        assert len(pts_xyz) > 0 and len(batch_inds) > 0 and len(rois) > 0
+        if max_inbox_point is None:
+            max_inbox_point = self.max_inbox_point
+        pb, rb = batch_inds.int(), rois[:, 0].int()
+        num = int(pb.max()) + 1
+        stats = torch.cat([torch.stack([(pb[1:] >= pb[:-1]).all(), (rb[1:] >= rb[:-1]).all(), (rb >= 0).all(), (pb >= 0).all()]).int(),
+                           torch.bincount(rb.clamp(0, num), minlength=num + 1)[:num].int(), torch.bincount(pb.clamp(0), minlength=num).int()])
+        stats = stats.tolist()
+        if not (stats[0] and stats[3]):
+            raise ValueError("DynamicPointROIExtractor: batch_inds must be sorted and non-negative")
+        if not (stats[1] and stats[2]):
+            raise ValueError("DynamicPointROIExtractor: rois[:, 0] must be sorted (ascending, non-negative batch ids)")
+        nroi, npts = stats[4:4 + num], stats[4 + num:]
+        if min(nroi) == 0 or min(npts) == 0:
+            raise ValueError(f"DynamicPointROIExtractor: every sample needs RoIs and points (RoIs {nroi}, points {npts})")
+        used = sum(nroi)   # RoIs of batch ids past the points' are never visited by the reference loop
+        all_inds, all_roi_inds, all_pts_info = ops.point_pool(rois[:used, 1:], rb[:used], pts_xyz, pb, self.extra_wlh, max_inbox_point,
+                                                              self.max_all_pts, per_sample=True, num_samples=num)
+        all_out_xyz = all_pts_info[:, :3]
+        all_local_xyz = all_pts_info[:, 3:6]
+        all_offset = all_pts_info[:, 6:-1]
+        is_in_margin = all_pts_info[:, -1]
+        if self.debug:   # dynamic_point_roi_extractor.py:92-101
+            roi_per_pts = rois[..., 1:][all_roi_inds]
+            in_box_pts = pts_xyz[all_inds]
+            assert torch.isclose(in_box_pts, all_out_xyz).all()
+            assert torch.isclose(all_offset[:, 0] + all_offset[:, 3], roi_per_pts[:, 4]).all()
+            assert torch.isclose(all_offset[:, 1] + all_offset[:, 4], roi_per_pts[:, 3]).all()
+            assert torch.isclose(all_offset[:, 2] + all_offset[:, 5], roi_per_pts[:, 5]).all()
+            assert (all_local_xyz[:, 0].abs() < roi_per_pts[:, 4] + self.extra_wlh[0] + 1e-5).all()
+            assert (all_local_xyz[:, 1].abs() < roi_per_pts[:, 3] + self.extra_wlh[1] + 1e-5).all()
+            assert (all_local_xyz[:, 2].abs() < roi_per_pts[:, 5] + self.extra_wlh[2] + 1e-5).all()
+        return all_inds, all_roi_inds, dict(local_xyz=all_local_xyz, boundary_offset=all_offset, is_in_margin=is_in_margin)
+
+    def fast_single_sample_forward(self, pts_xyz, rois, max_inbox_point=None):
+        """:111-136 (the op's default max_all_pts, as there)"""
+        if max_inbox_point is None:
+            max_inbox_point = self.max_inbox_point
+        ext_pts_inds, roi_inds, ext_pts_info = ops.dynamic_point_pool(rois[..., 1:].contiguous(), pts_xyz.contiguous(), self.extra_wlh,
+                                                                      max_inbox_point)
+        return ext_pts_inds, roi_inds, dict(local_xyz=ext_pts_info[:, 3:6], boundary_offset=ext_pts_info[:, 6:-1],
+                                            is_in_margin=ext_pts_info[:, -1])

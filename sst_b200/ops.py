@@ -9,6 +9,7 @@ and error behaviour; no CPU path - CPU tensors raise.
     get_window_coors, make_continuous_inds, get_flat2win_inds(_v2), flat2window(_v2), window2flat(_v2)
                                       ops/sst/sst_ops.py:27-149,266-331      (B1, B4, B6)
     build_mlp, get_activation(_layer) ops/sst/sst_ops.py:334-392             (S3)
+    dynamic_point_pool(_mixed)        ops/dynamic_point_pool_op.py:9-113     (FSD RoI point pooling)
 """
 import ctypes as C
 import math
@@ -604,3 +605,77 @@ def linear(x, weight, bias=None, act=None):
     L.check(c, L.lib().sstb200_linear(c, x.data_ptr(), w.data_ptr(), L.ptr(b), out.data_ptr(), x.shape[0], w.shape[0],
                                       w.shape[1], {None: 0, "relu": 1, "gelu": 2}[act]))
     return out
+
+
+# ----------------------------------------------------------------------------------------------
+# FSD RoI point pooling (ops/dynamic_point_pool_op.py:9-113)
+# ----------------------------------------------------------------------------------------------
+L.SIGNATURES["sstb200_dynamic_point_pool"] = (C.c_int, [L.vp, L.vp, L.vp, C.c_int, L.vp, L.vp, C.c_int, L.P_f32, C.c_int, C.c_int,
+                                                        C.c_int, L.vp, L.vp, L.vp, L.vp, L.P_i32])
+
+
+def point_pool(rois, rois_batch, pts, pts_batch, extra_wlh, max_inbox_point, max_all_pts, per_sample=False, num_samples=1):
+    """sstb200_dynamic_point_pool -> (pts_idx int64 [K], roi_idx int64 [K], feats fp32 [K, 13]).  per_sample: max_all_pts and the fake
+    row apply to every sample (RoIs grouped by ascending batch id, num_samples distinct ids) instead of to the whole call."""
+    _need_cuda(rois, pts, rois_batch, pts_batch)
+    rois = rois.float().contiguous()
+    pts = pts[:, :3].float().contiguous()
+    rb = None if rois_batch is None else rois_batch.int().contiguous()
+    pb = None if pts_batch is None else pts_batch.int().contiguous()
+    cap = int(max_all_pts) * (int(num_samples) if per_sample else 1)
+    dev = pts.device
+    out_idx = torch.empty((cap,), dtype=torch.int64, device=dev)
+    out_roi = torch.empty((cap,), dtype=torch.int64, device=dev)
+    out_feats = torch.empty((cap, 13), dtype=torch.float32, device=dev)
+    num_dev = torch.empty((1,), dtype=torch.int32, device=dev)
+    num_host = (C.c_int32 * 3)()
+    c = L.ctx(dev)
+    L.check(c, L.lib().sstb200_dynamic_point_pool(c, rois.data_ptr(), L.ptr(rb), rois.shape[0], pts.data_ptr(), L.ptr(pb), pts.shape[0],
+                                                  L.arr(C.c_float, [float(v) for v in extra_wlh]), int(max_inbox_point), int(max_all_pts),
+                                                  int(bool(per_sample)), out_idx.data_ptr(), out_roi.data_ptr(), out_feats.data_ptr(),
+                                                  num_dev.data_ptr(), num_host))
+    k, found, written = num_host[0], num_host[1], num_host[2]
+    if found > written:
+        import warnings
+        warnings.warn(f"dynamic_point_pool: {found - written} of {found} RoI-point pairs exceed max_all_pts={max_all_pts} and were dropped")
+    return out_idx[:k], out_roi[:k], out_feats[:k]
+
+
+class DynamicPointPoolFunction(Function):
+    """dynamic_point_pool_op.py:9-58.  rois [R, 7] (x, y, z_bottom, w, l, h, rz), pts [N, 3] -> point index, RoI index, features
+    [K, 13] = point xyz, local xyz, 6 boundary offsets, is_in_margin; rows sorted by RoI then point index; one (-1, -1, 0) row when no
+    point lies in any enlarged box.  Deterministic."""
+
+    @staticmethod
+    def forward(ctx, rois, pts, extra_wlh, max_inbox_point, max_all_pts=50000):
+        assert len(rois) > 0
+        out = point_pool(rois, None, pts, None, extra_wlh, max_inbox_point, max_all_pts)
+        for t in out:
+            ctx.mark_non_differentiable(t)
+        return out
+
+    @staticmethod
+    def backward(ctx, g1, g2, g3):
+        return None, None, None, None, None
+
+
+dynamic_point_pool = DynamicPointPoolFunction.apply
+
+
+class DynamicPointPoolMixedFunction(Function):
+    """dynamic_point_pool_op.py:63-111: as above over several samples at once; a point pairs only with RoIs of its own batch id."""
+
+    @staticmethod
+    def forward(ctx, rois, rois_batch, pts, pts_batch, extra_wlh, max_inbox_point, max_all_pts=200000):
+        assert len(rois) > 0
+        out = point_pool(rois, rois_batch, pts, pts_batch, extra_wlh, max_inbox_point, max_all_pts)
+        for t in out:
+            ctx.mark_non_differentiable(t)
+        return out
+
+    @staticmethod
+    def backward(ctx, g1, g2, g3):
+        return None, None, None, None, None, None, None
+
+
+dynamic_point_pool_mixed = DynamicPointPoolMixedFunction.apply

@@ -44,7 +44,7 @@ class Registry:
 
 
 MODELS = Registry("models")
-VOXEL_ENCODERS = MIDDLE_ENCODERS = BACKBONES = FUSION_LAYERS = MODELS
+VOXEL_ENCODERS = MIDDLE_ENCODERS = BACKBONES = FUSION_LAYERS = ROI_EXTRACTORS = MODELS
 NORM_LAYERS = Registry("norm layer")
 
 
