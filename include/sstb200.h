@@ -458,6 +458,39 @@ int sstb200_dynamic_point_pool(sstb200_ctx* ctx, const float* rois, const int32_
                                int per_sample, int64_t* out_pts_idx, int64_t* out_roi_idx, float* out_feats, int32_t* num_out_dev,
                                int32_t* num_pairs_host);
 
+/* ---- Rotated BEV overlap, IoU and NMS: mmdet3d/ops/iou3d (iou3d_utils.py, src/iou3d.cpp, src/iou3d_kernel.cu), used by
+ * box3d_multiclass_nms (core/post_processing/box3d_nms.py:10-143), CenterHead / FullySparseBboxHead (nms_gpu) and
+ * BaseInstance3DBoxes.overlaps (boxes_overlap_bev_gpu).
+ * Boxes are fp32 [x1, y1, x2, y2, r] rows.  Corners (x1,y1), (x2,y1), (x2,y2), (x1,y2) are turned about the box centre by
+ * (dx cos r + dy sin r, -dx sin r + dy cos r), the reference's convention.  Overlap = exact area of the two rectangles' intersection,
+ * evaluated in fp32 relative to one box's centre (0 when the circumscribed circles are apart, 0 for a zero-area box, never NaN);
+ * iou = overlap / max(sa + sb - overlap, 1e-8), s = (x2 - x1)(y2 - y1).
+ *
+ * sstb200_boxes_overlap_bev / sstb200_boxes_iou_bev: out [num_a, num_b] row-major (out[i * num_b + j] for a_i, b_j); every entry is
+ * written.  num_a or num_b = 0 writes nothing; a negative size is SSTB_ERR_ARG; num_a > 65535 * 32 is SSTB_ERR_UNSUPPORTED.  No sync. */
+int sstb200_boxes_overlap_bev(sstb200_ctx* ctx, const float* boxes_a, int num_a, const float* boxes_b, int num_b, float* overlap);
+int sstb200_boxes_iou_bev(sstb200_ctx* ctx, const float* boxes_a, int num_a, const float* boxes_b, int num_b, float* iou);
+
+/* Segmented greedy NMS (nms_gpu / nms_normal_gpu of iou3d_utils.py:31-56,106-124 over every segment of one call).
+ * boxes [num, 5] are grouped into segments s = rows [seg_offsets[s], seg_offsets[s+1]), each sorted by descending score (the caller
+ * sorts).  seg_offsets is a HOST int32 array of num_segs + 1 entries: seg_offsets[0] = 0, non-decreasing, seg_offsets[num_segs] = num;
+ * thresh is a HOST float array of num_segs thresholds (INFINITY keeps every box of its segment).  Within a segment, box j is
+ * suppressed by an earlier kept box i iff IoU(i, j) > thresh[s] (strict); rotated = 1 uses the rotated IoU, rotated = 0 the
+ * axis-aligned IoU of nms_normal_gpu (r ignored).  The result equals the reference's 64-bit mask + greedy scan (iou3d.cpp:130-143)
+ * run on each segment alone, up to fp32 rounding of IoUs that lie at the threshold.
+ * keep_out (int64, capacity num): positions into `boxes` of the kept boxes, segment after segment, ascending within a segment;
+ * num_keep_dev (device int32): their number; num_keep_host != NULL: one stream sync, then the same number on the host.
+ * Workspace: caller-allocated device memory of at least sstb200_nms_bev_workspace_bytes(num, seg_offsets, num_segs) bytes (mask of
+ * sum_s n_s * ceil(n_s / 64) 64-bit words, plus num + num_segs int32 and the segment table); the call allocates nothing and uses no
+ * atomics, so results are deterministic.  Largest segment: 65536 boxes (SSTB_ERR_UNSUPPORTED beyond, from both functions).
+ * Errors (SSTB_ERR_ARG, nothing enqueued): num or num_segs negative, seg_offsets NULL with num_segs > 0, num_segs = 0 with num > 0,
+ * offsets not starting at 0, decreasing or not ending at num, boxes / keep_out / thresh NULL when needed, workspace NULL;
+ * workspace_bytes below the query's value is SSTB_ERR_WORKSPACE. */
+int sstb200_nms_bev_workspace_bytes(sstb200_ctx* ctx, int num, const int32_t* seg_offsets, int num_segs, int64_t* bytes);
+int sstb200_nms_bev(sstb200_ctx* ctx, const float* boxes, int num, const int32_t* seg_offsets, int num_segs, const float* thresh,
+                    int rotated, void* workspace, int64_t workspace_bytes, int64_t* keep_out, int32_t* num_keep_dev,
+                    int32_t* num_keep_host);
+
 #ifdef __cplusplus
 }
 #endif

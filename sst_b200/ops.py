@@ -10,6 +10,9 @@ and error behaviour; no CPU path - CPU tensors raise.
                                       ops/sst/sst_ops.py:27-149,266-331      (B1, B4, B6)
     build_mlp, get_activation(_layer) ops/sst/sst_ops.py:334-392             (S3)
     dynamic_point_pool(_mixed)        ops/dynamic_point_pool_op.py:9-113     (FSD RoI point pooling)
+    boxes_iou_bev, boxes_overlap_bev, nms_gpu, nms_normal_gpu
+                                      ops/iou3d/iou3d_utils.py               (rotated BEV IoU / NMS)
+    box3d_multiclass_nms              core/post_processing/box3d_nms.py:10-143
 """
 import ctypes as C
 import math
@@ -679,3 +682,142 @@ class DynamicPointPoolMixedFunction(Function):
 
 
 dynamic_point_pool_mixed = DynamicPointPoolMixedFunction.apply
+
+
+# ----------------------------------------------------------------------------------------------
+# Rotated BEV overlap / IoU / NMS (ops/iou3d/iou3d_utils.py, core/post_processing/box3d_nms.py:10-143)
+# ----------------------------------------------------------------------------------------------
+L.SIGNATURES["sstb200_boxes_overlap_bev"] = (C.c_int, [L.vp, L.vp, C.c_int, L.vp, C.c_int, L.vp])
+L.SIGNATURES["sstb200_boxes_iou_bev"] = (C.c_int, [L.vp, L.vp, C.c_int, L.vp, C.c_int, L.vp])
+L.SIGNATURES["sstb200_nms_bev_workspace_bytes"] = (C.c_int, [L.vp, C.c_int, L.P_i32, C.c_int, L.P_i64])
+L.SIGNATURES["sstb200_nms_bev"] = (C.c_int, [L.vp, L.vp, C.c_int, L.P_i32, C.c_int, L.P_f32, C.c_int, L.vp, C.c_int64, L.vp, L.vp,
+                                             L.P_i32])
+
+
+def _bev_boxes(boxes, name):
+    if boxes.dim() != 2 or boxes.shape[1] != 5:
+        raise L.SSTB200Error(f"{name}: boxes must be [N, 5] (x1, y1, x2, y2, r), got {tuple(boxes.shape)}")
+    return boxes.float().contiguous()
+
+
+def _bev_pairs(fn, boxes_a, boxes_b):
+    _need_cuda(boxes_a, boxes_b)
+    a, b = _bev_boxes(boxes_a, fn), _bev_boxes(boxes_b, fn)
+    out = torch.empty((a.shape[0], b.shape[0]), dtype=torch.float32, device=a.device)
+    c = L.ctx(a.device)
+    L.check(c, getattr(L.lib(), fn)(c, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], out.data_ptr()))
+    return out
+
+
+def boxes_iou_bev(boxes_a, boxes_b):
+    """iou3d_utils.py:12-28: rotated BEV IoU of boxes_a [M, 5] and boxes_b [N, 5] ([x1, y1, x2, y2, r]) -> fp32 [M, N]."""
+    return _bev_pairs("sstb200_boxes_iou_bev", boxes_a, boxes_b)
+
+
+def boxes_overlap_bev(boxes_a, boxes_b):
+    """iou3d_cuda.boxes_overlap_bev_gpu (BaseInstance3DBoxes.overlaps): rotated BEV overlap area, fp32 [M, N]."""
+    return _bev_pairs("sstb200_boxes_overlap_bev", boxes_a, boxes_b)
+
+
+def nms_bev(boxes, seg_offsets, thresh, rotated=True):
+    """Segmented greedy NMS (sstb200_nms_bev): boxes [num, 5] grouped into segments [seg_offsets[s], seg_offsets[s+1]), each sorted by
+    descending score; thresh[s] per segment (None keeps the whole segment).  Returns int64 positions into `boxes` of the kept boxes,
+    segment after segment, in score order; one host sync for their number."""
+    _need_cuda(boxes)
+    b = _bev_boxes(boxes, "nms_bev")
+    S = len(seg_offsets) - 1
+    off = L.arr(C.c_int32, [int(v) for v in seg_offsets])
+    th = L.arr(C.c_float, [math.inf if t is None else float(t) for t in thresh])
+    if len(th) != S:
+        raise L.SSTB200Error(f"nms_bev: {len(th)} thresholds for {S} segments")
+    c = L.ctx(b.device)
+    nbytes = C.c_int64()
+    L.check(c, L.lib().sstb200_nms_bev_workspace_bytes(c, b.shape[0], off, S, C.byref(nbytes)))
+    ws = torch.empty((nbytes.value,), dtype=torch.uint8, device=b.device)
+    keep = torch.empty((b.shape[0],), dtype=torch.int64, device=b.device)
+    num_dev = torch.empty((1,), dtype=torch.int32, device=b.device)
+    num = C.c_int32()
+    L.check(c, L.lib().sstb200_nms_bev(c, b.data_ptr(), b.shape[0], off, S, th, int(bool(rotated)), ws.data_ptr(), nbytes.value,
+                                       keep.data_ptr(), num_dev.data_ptr(), C.byref(num)))
+    return keep[:num.value]
+
+
+def nms_gpu(boxes, scores, thresh, pre_maxsize=None, post_max_size=None):
+    """iou3d_utils.py:31-56: rotated NMS.  boxes [N, 5], scores [N] -> int64 indices into the input of the kept boxes, by descending
+    score (the reference's `scores.sort(0, descending=True)`, so ties fall in torch's order as there)."""
+    _need_cuda(boxes, scores)
+    order = scores.sort(0, descending=True)[1]
+    if pre_maxsize is not None:
+        order = order[:pre_maxsize]
+    keep = order[nms_bev(boxes[order], [0, order.numel()], [thresh], rotated=True)].contiguous()
+    if post_max_size is not None:
+        keep = keep[:post_max_size]
+    return keep
+
+
+def nms_normal_gpu(boxes, scores, thresh):
+    """iou3d_utils.py:106-124: NMS with the axis-aligned IoU (r ignored)."""
+    _need_cuda(boxes, scores)
+    order = scores.sort(0, descending=True)[1]
+    return order[nms_bev(boxes[order], [0, order.numel()], [thresh], rotated=False)].contiguous()
+
+
+def box3d_multiclass_nms(mlvl_bboxes, mlvl_bboxes_for_nms, mlvl_scores, score_thr, max_num, cfg, mlvl_dir_scores=None,
+                         mlvl_attr_scores=None, mlvl_bboxes2d=None):
+    """box3d_nms.py:10-143 with every class in ONE segmented NMS call.  Same arguments, outputs and order: classes in turn, each
+    class's kept boxes by descending score (boxes in input order for a class whose nms_thr is None), then the reference's own
+    `scores.sort(descending=True)` when more than max_num remain.  Within a class, equal scores are taken in input order; the reference
+    takes them in torch's sort order, so the two agree whenever a class has no tied scores."""
+    _need_cuda(mlvl_bboxes, mlvl_bboxes_for_nms, mlvl_scores, mlvl_dir_scores, mlvl_attr_scores, mlvl_bboxes2d)
+    num_classes = mlvl_scores.shape[1] - 1
+    dev = mlvl_scores.device
+    if isinstance(score_thr, (list, tuple)):
+        assert len(score_thr) == num_classes
+        score_thrs = list(score_thr)
+    else:
+        score_thrs = [score_thr] * num_classes
+    nms_thr = cfg.nms_thr
+    if isinstance(nms_thr, (list, tuple)):
+        assert len(nms_thr) == num_classes
+        nms_thrs = list(nms_thr)
+    else:
+        nms_thrs = [nms_thr] * num_classes
+    cls_scores = mlvl_scores[:, :num_classes]
+    thr = torch.tensor([float(t) for t in score_thrs], dtype=mlvl_scores.dtype, device=dev)
+    cls, idx = (cls_scores > thr).t().nonzero(as_tuple=True)           # class-major, input order within a class
+    sc = cls_scores[idx, cls]
+    no_nms = torch.tensor([t is None for t in nms_thrs], dtype=torch.bool, device=dev)
+    key = torch.where(no_nms[cls], torch.zeros_like(sc), sc)           # a class without NMS keeps input order
+    o = torch.sort(key, descending=True, stable=True).indices
+    o = o[torch.sort(cls[o], stable=True).indices]
+    cls, idx, sc = cls[o], idx[o], sc[o]
+    counts = torch.bincount(cls, minlength=num_classes).tolist()
+    if sum(counts) == 0:
+        bboxes = mlvl_scores.new_zeros((0, mlvl_bboxes.size(-1)))
+        scores = mlvl_scores.new_zeros((0,))
+        labels = mlvl_scores.new_zeros((0,), dtype=torch.long)
+        dir_scores = mlvl_scores.new_zeros((0,)) if mlvl_dir_scores is not None else None
+        attr_scores = mlvl_scores.new_zeros((0,)) if mlvl_attr_scores is not None else None
+        bboxes2d = mlvl_scores.new_zeros((0, 4)) if mlvl_bboxes2d is not None else None
+    else:
+        offsets = [0]
+        for n in counts:
+            offsets.append(offsets[-1] + n)
+        keep = nms_bev(mlvl_bboxes_for_nms[idx], offsets, nms_thrs, rotated=cfg.use_rotate_nms)
+        sel = idx[keep]
+        bboxes, scores, labels = mlvl_bboxes[sel], sc[keep], cls[keep]
+        dir_scores = mlvl_dir_scores[sel] if mlvl_dir_scores is not None else None
+        attr_scores = mlvl_attr_scores[sel] if mlvl_attr_scores is not None else None
+        bboxes2d = mlvl_bboxes2d[sel] if mlvl_bboxes2d is not None else None
+        if bboxes.shape[0] > max_num:
+            _, inds = scores.sort(descending=True)
+            inds = inds[:max_num]
+            bboxes, labels, scores = bboxes[inds, :], labels[inds], scores[inds]
+            dir_scores = dir_scores[inds] if dir_scores is not None else None
+            attr_scores = attr_scores[inds] if attr_scores is not None else None
+            bboxes2d = bboxes2d[inds] if bboxes2d is not None else None
+    results = (bboxes, scores, labels)
+    for extra, given in ((dir_scores, mlvl_dir_scores), (attr_scores, mlvl_attr_scores), (bboxes2d, mlvl_bboxes2d)):
+        if given is not None:
+            results = results + (extra,)
+    return results
