@@ -491,6 +491,58 @@ int sstb200_nms_bev(sstb200_ctx* ctx, const float* boxes, int num, const int32_t
                     int rotated, void* workspace, int64_t workspace_bytes, int64_t* keep_out, int32_t* num_keep_dev,
                     int32_t* num_keep_host);
 
+/* ---- Points in boxes and RoI-aware pooling: mmdet3d/ops/roiaware_pool3d (points_in_boxes.py, roiaware_pool3d.py, src/).
+ * Boxes / RoIs are fp32 rows (x, y, z_bottom, w, l, h, rz).  A point is inside when check_pt_in_box3d
+ * (src/points_in_boxes_cuda.cu:24-49) says so, evaluated as the same float expressions: centre z = bottom + h/2, |z - cz| > h/2 rejects,
+ * angle rz + pi/2, strict |local x| < l/2, |local y| < w/2.  Results are bit-identical to the reference kernels'.
+ *
+ * sstb200_points_in_boxes: pts [batch, num_pts, 3], boxes [batch, num_boxes, 7] (sample b's points against sample b's boxes).
+ * mode SSTB200_PIB_FIRST (points_in_boxes_gpu): out int32 [batch, num_pts] = the LOWEST box index containing the point, else -1.
+ * mode SSTB200_PIB_ALL (points_in_boxes_batch): out int32 [batch, num_pts, num_boxes] = 1 inside, else 0.
+ * Every entry is written (no fill needed); zero-size boxes contain nothing.  No atomics, no sync.  Errors: negative sizes or an unknown
+ * mode (SSTB_ERR_ARG); more than 786432 boxes per sample in ALL mode (SSTB_ERR_UNSUPPORTED). */
+#define SSTB200_PIB_FIRST 0
+#define SSTB200_PIB_ALL 1
+int sstb200_points_in_boxes(sstb200_ctx* ctx, const float* pts, const float* boxes, int batch, int num_pts, int num_boxes, int mode,
+                            int32_t* out);
+
+/* RoIAwarePool3d (roiaware_pool3d.py:24-86, src/roiaware_pool3d_kernel.cu), in two calls on one context:
+ *
+ * sstb200_roiaware_pool3d_plan: rois [num_rois, 7], pts [num_pts, 3]; rois_batch / pts_batch int32 batch ids (>= 0) or both NULL (one
+ * sample): a point pairs only with the RoIs of its own batch id, so one call covers every sample.  out_size = (ox, oy, oz), each in
+ * [1, 255]; max_pts_per_voxel = m >= 1.  Finds the (RoI, point) pairs and syncs the stream once: *num_pairs_host = P, their number.
+ * What it computed stays in the context's scratch arena for sstb200_roiaware_pool3d_forward, which must be the next call on the context.
+ * Errors: negative sizes, out_size outside [1, 255], m < 1, a negative batch id (SSTB_ERR_ARG); RoI, voxel and point indices that do
+ * not fit one 64-bit key, or P >= 2^31 (SSTB_ERR_UNSUPPORTED).
+ *
+ * sstb200_roiaware_pool3d_forward: pts_feature [num_pts, channels] fp32, mode SSTB200_POOL3D_MAX or _AVG.  A point inside RoI r falls in
+ * voxel (x, y, z) = int((local x + l/2) / (l/ox)), int((local y + w/2) / (w/oy)), int((z - z_bottom) / (h/oz)) (fp32, each clamped to
+ * [0, o - 1]); every voxel keeps its first m - 1 points in ascending point index (the reference's buffer holds a counter in slot 0).
+ * max: from -inf, strict `>` in ascending point order (argmax = the first point reaching the maximum; NaN / -inf are never selected);
+ * avg: sequential fp32 sum in ascending point order / count.  pooled [num_rois, ox, oy, oz, channels] is dense and fully written; a voxel
+ * without a selected point writes 0.  The state the backward needs is compact, in caller buffers of capacity P (P + 1 offsets):
+ *   voxel_slot int64   occupied voxels, ascending r * ox*oy*oz + (x * oy + y) * oz + z;
+ *   voxel_offsets      int32 CSR over them into point_idx;
+ *   point_idx int32    kept point indices, ascending within a voxel;
+ *   argmax int32       [occupied, channels] (max mode only; NULL for avg), -1 where nothing was selected;
+ *   counts_dev int32[2] (device): occupied voxels, kept points.
+ * Deterministic; no sync.
+ *
+ * sstb200_roiaware_pool3d_backward: grad_out [num_rois, ox, oy, oz, channels] -> grad_in [num_pts, channels], fully written.  max: the
+ * grad_out of every (voxel, channel) whose argmax is the point; avg: grad_out * (1 / max(count, 1)) of every voxel that kept the point.
+ * Each point's terms are summed in (RoI, voxel) order without atomics, so two runs are bit-identical (the reference adds them with
+ * float atomics).  num_pairs = the plan's P, with the state written by the forward.  No sync. */
+#define SSTB200_POOL3D_MAX 0
+#define SSTB200_POOL3D_AVG 1
+int sstb200_roiaware_pool3d_plan(sstb200_ctx* ctx, const float* rois, const int32_t* rois_batch, int num_rois, const float* pts,
+                                 const int32_t* pts_batch, int num_pts, const int32_t out_size[3], int max_pts_per_voxel,
+                                 int64_t* num_pairs_host);
+int sstb200_roiaware_pool3d_forward(sstb200_ctx* ctx, const float* pts_feature, int channels, int mode, float* pooled, int64_t* voxel_slot,
+                                    int32_t* voxel_offsets, int32_t* point_idx, int32_t* argmax, int32_t* counts_dev);
+int sstb200_roiaware_pool3d_backward(sstb200_ctx* ctx, int num_pts, int channels, int mode, int64_t num_pairs, const int64_t* voxel_slot,
+                                     const int32_t* voxel_offsets, const int32_t* point_idx, const int32_t* argmax,
+                                     const int32_t* counts_dev, const float* grad_out, float* grad_in);
+
 #ifdef __cplusplus
 }
 #endif

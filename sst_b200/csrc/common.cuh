@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <memory>
 #include <string>
 #include <utility>
 #include <vector>
@@ -27,6 +28,9 @@ struct sstb200_ctx {
   size_t arena_cap = 0;
   size_t arena_off = 0;
   std::vector<void*> retired;  // old arenas kept alive until destroy (stream-ordered safety)
+  unsigned long long arena_epoch = 0;  // bumped by arena_reset: what a call left in the arena survives while this is unchanged
+  std::shared_ptr<void> handoff;       // host record of such arena contents, for the call that consumes them
+  unsigned long long handoff_epoch = 0;
   std::string err;
   int32_t* pinned_i32 = nullptr;  // small pinned scratch for D2H counters
   cudaEvent_t ev_coords = nullptr;  // recorded by the VFE entry points once voxel_coors / num_dev are produced (fork point of a side branch)
@@ -59,7 +63,10 @@ inline int sstb_fail(sstb200_ctx* c, int code, const char* fmt, ...) {
 #define LAUNCH_CHECK(ctx) CUDA_TRY(ctx, cudaGetLastError())
 
 // ---- arena ---------------------------------------------------------------
-inline void arena_reset(sstb200_ctx* c) { c->arena_off = 0; }
+inline void arena_reset(sstb200_ctx* c) {
+  c->arena_off = 0;
+  c->arena_epoch++;
+}
 
 // Reserve: make sure `bytes` are available from offset 0 (called once at the top of an op
 // with an upper bound, so that no growth happens mid-op).

@@ -13,6 +13,8 @@ and error behaviour; no CPU path - CPU tensors raise.
     boxes_iou_bev, boxes_overlap_bev, nms_gpu, nms_normal_gpu
                                       ops/iou3d/iou3d_utils.py               (rotated BEV IoU / NMS)
     box3d_multiclass_nms              core/post_processing/box3d_nms.py:10-143
+    points_in_boxes_gpu, points_in_boxes_batch, RoIAwarePool3d
+                                      ops/roiaware_pool3d                    (box membership, RoI-aware pooling)
 """
 import ctypes as C
 import math
@@ -821,3 +823,129 @@ def box3d_multiclass_nms(mlvl_bboxes, mlvl_bboxes_for_nms, mlvl_scores, score_th
         if given is not None:
             results = results + (extra,)
     return results
+
+
+# ----------------------------------------------------------------------------------------------
+# Points in boxes and RoI-aware pooling (ops/roiaware_pool3d: points_in_boxes.py, roiaware_pool3d.py)
+# ----------------------------------------------------------------------------------------------
+L.SIGNATURES["sstb200_points_in_boxes"] = (C.c_int, [L.vp, L.vp, L.vp, C.c_int, C.c_int, C.c_int, C.c_int, L.vp])
+L.SIGNATURES["sstb200_roiaware_pool3d_plan"] = (C.c_int, [L.vp, L.vp, L.vp, C.c_int, L.vp, L.vp, C.c_int, L.P_i32, C.c_int, L.P_i64])
+L.SIGNATURES["sstb200_roiaware_pool3d_forward"] = (C.c_int, [L.vp, L.vp, C.c_int, C.c_int, L.vp, L.vp, L.vp, L.vp, L.vp, L.vp])
+L.SIGNATURES["sstb200_roiaware_pool3d_backward"] = (C.c_int, [L.vp, C.c_int, C.c_int, C.c_int, C.c_int64, L.vp, L.vp, L.vp, L.vp, L.vp,
+                                                              L.vp, L.vp])
+
+
+def _points_in_boxes(points, boxes, mode):
+    assert boxes.shape[0] == points.shape[0], \
+        f'Points and boxes should have the same batch size, got {boxes.shape[0]} and {points.shape[0]}'
+    assert boxes.shape[2] == 7, f'boxes dimension should be 7, got unexpected shape {boxes.shape[2]}'
+    assert points.shape[2] == 3, f'points dimension should be 3, got unexpected shape {points.shape[2]}'
+    _need_cuda(points, boxes)
+    assert points.device == boxes.device, 'Points and boxes should be put on the same device'
+    B, M, _ = points.shape
+    T = boxes.shape[1]
+    out = torch.empty((B, M) if mode == 0 else (B, M, T), dtype=torch.int32, device=points.device)
+    p, b = points.float().contiguous(), boxes.float().contiguous()
+    c = L.ctx(points.device)
+    L.check(c, L.lib().sstb200_points_in_boxes(c, p.data_ptr(), b.data_ptr(), B, M, T, mode, out.data_ptr()))
+    return out
+
+
+def points_in_boxes_gpu(points, boxes):
+    """points_in_boxes.py:6-47: points [B, M, 3], boxes [B, T, 7] (x, y, z_bottom, w, l, h, rz) -> int32 [B, M], the lowest index of a
+    box holding the point, -1 for none (overlapping boxes: the first one wins, as in the reference's loop)."""
+    return _points_in_boxes(points, boxes, 0)
+
+
+def points_in_boxes_batch(points, boxes):
+    """points_in_boxes.py:85-123: points [B, M, 3], boxes [B, T, 7] -> int32 [B, M, T], 1 where the point is inside the box, else 0."""
+    return _points_in_boxes(points, boxes, 1)
+
+
+_POOL3D_MODES = {"max": 0, "avg": 1}
+
+
+def _out_size3(out_size):
+    if isinstance(out_size, int):
+        return (out_size,) * 3
+    assert len(out_size) == 3 and all(isinstance(v, int) for v in out_size), f"out_size must be an int or 3 ints, got {out_size!r}"
+    return tuple(out_size)
+
+
+def roiaware_pool3d_forward(rois, pts, pts_feature, out_size, max_pts_per_voxel, mode, rois_batch=None, pts_batch=None):
+    """sstb200_roiaware_pool3d_plan + _forward.  rois [R, 7], pts [N, 3], pts_feature [N, C]; mode 0 (max) or 1 (avg); optional int32
+    batch ids of RoIs and points (a point pairs only with RoIs of its own batch id).  Returns pooled [R, ox, oy, oz, C] and the compact
+    state of the backward: (voxel_slot, voxel_offsets, point_idx, argmax or None, counts, num_pairs).  One stream sync."""
+    if mode not in (0, 1):
+        raise L.SSTB200Error(f"roiaware_pool3d: mode must be 0 (max) or 1 (avg), got {mode!r}")
+    ox, oy, oz = _out_size3(out_size)
+    if not all(1 <= v <= 255 for v in (ox, oy, oz)):      # the reference asserts < 256 (voxel indices are packed into 8 bits each)
+        raise L.SSTB200Error(f"roiaware_pool3d: out_size {(ox, oy, oz)} outside [1, 255]")
+    if int(max_pts_per_voxel) < 1:
+        raise L.SSTB200Error(f"roiaware_pool3d: max_pts_per_voxel must be >= 1, got {max_pts_per_voxel}")
+    _need_cuda(rois, pts, pts_feature, rois_batch, pts_batch)
+    rois, pts, feats = rois.float().contiguous(), pts.float().contiguous(), pts_feature.float().contiguous()
+    assert rois.dim() == 2 and rois.shape[1] == 7 and pts.dim() == 2 and pts.shape[1] == 3
+    assert feats.dim() == 2 and feats.shape[0] == pts.shape[0]
+    rb = None if rois_batch is None else rois_batch.int().contiguous()
+    pb = None if pts_batch is None else pts_batch.int().contiguous()
+    R, N, Ch = rois.shape[0], pts.shape[0], feats.shape[1]
+    dev = pts.device
+    c = L.ctx(dev)
+    P = C.c_int64()
+    L.check(c, L.lib().sstb200_roiaware_pool3d_plan(c, rois.data_ptr(), L.ptr(rb), R, pts.data_ptr(), L.ptr(pb), N,
+                                                    L.arr(C.c_int32, [ox, oy, oz]), int(max_pts_per_voxel), C.byref(P)))
+    P = P.value
+    pooled = torch.empty((R, ox, oy, oz, Ch), dtype=torch.float32, device=dev)
+    slot = torch.empty((max(P, 1),), dtype=torch.int64, device=dev)
+    voff = torch.empty((P + 1,), dtype=torch.int32, device=dev)
+    pidx = torch.empty((max(P, 1),), dtype=torch.int32, device=dev)
+    argmax = torch.empty((max(P, 1), Ch), dtype=torch.int32, device=dev) if mode == 0 else None
+    counts = torch.empty((2,), dtype=torch.int32, device=dev)
+    L.check(c, L.lib().sstb200_roiaware_pool3d_forward(c, feats.data_ptr(), Ch, mode, pooled.data_ptr(), slot.data_ptr(), voff.data_ptr(),
+                                                       pidx.data_ptr(), L.ptr(argmax), counts.data_ptr()))
+    return pooled, (slot, voff, pidx, argmax, counts, P)
+
+
+def roiaware_pool3d_backward(grad_out, state, num_pts, mode):
+    """sstb200_roiaware_pool3d_backward: grad_out [R, ox, oy, oz, C] -> grad_in [num_pts, C] (bit-identical from run to run)."""
+    slot, voff, pidx, argmax, counts, P = state
+    g = grad_out.float().contiguous()
+    Ch = g.shape[-1]
+    grad_in = torch.empty((num_pts, Ch), dtype=torch.float32, device=g.device)
+    c = L.ctx(g.device)
+    L.check(c, L.lib().sstb200_roiaware_pool3d_backward(c, num_pts, Ch, mode, P, slot.data_ptr(), voff.data_ptr(), pidx.data_ptr(),
+                                                        L.ptr(argmax), counts.data_ptr(), g.data_ptr(), grad_in.data_ptr()))
+    return grad_in
+
+
+class RoIAwarePool3dFunction(Function):
+    """roiaware_pool3d.py:45-86: rois [R, 7] (x, y, z_bottom, w, l, h, rz), pts [N, 3], pts_feature [N, C], out_size (int or 3 ints),
+    max_pts_per_voxel m, mode 0 (max) / 1 (avg) -> pooled [R, ox, oy, oz, C]; gradient for pts_feature only.  The saved state is compact
+    (occupied voxels, their kept points, [occupied, C] argmax) instead of the reference's dense [R, ox, oy, oz, m] index buffer.
+    Optional rois_batch / pts_batch pool every sample of a batch in one call."""
+
+    @staticmethod
+    def forward(ctx, rois, pts, pts_feature, out_size, max_pts_per_voxel, mode, rois_batch=None, pts_batch=None):
+        pooled, state = roiaware_pool3d_forward(rois, pts, pts_feature, out_size, max_pts_per_voxel, mode, rois_batch, pts_batch)
+        ctx.roiaware_pool3d_for_backward = (state, mode, pts.shape[0])
+        return pooled
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        state, mode, num_pts = ctx.roiaware_pool3d_for_backward
+        return None, None, roiaware_pool3d_backward(grad_out, state, num_pts, mode), None, None, None, None, None
+
+
+class RoIAwarePool3d(nn.Module):
+    """roiaware_pool3d.py:8-42: RoIAwarePool3d(out_size, max_pts_per_voxel=128, mode='max'); forward(rois, pts, pts_feature)."""
+
+    def __init__(self, out_size, max_pts_per_voxel=128, mode='max'):
+        super().__init__()
+        self.out_size = out_size
+        self.max_pts_per_voxel = max_pts_per_voxel
+        assert mode in ['max', 'avg']
+        self.mode = _POOL3D_MODES[mode]
+
+    def forward(self, rois, pts, pts_feature):
+        return RoIAwarePool3dFunction.apply(rois, pts, pts_feature, self.out_size, self.max_pts_per_voxel, self.mode)
