@@ -325,6 +325,13 @@ int sstb200_group_csr(sstb200_ctx* ctx, const int64_t* inv, int num_points, int 
 int sstb200_recover_bev(sstb200_ctx* ctx, const float* voxel_feat, const int64_t* coors, int num_voxels, int channels,
                         int batch_size, int ny, int nx, float* canvas);
 
+/* A4' backward: grad_feat[m, :] = grad_canvas[b_m, :, y_m, x_m] for every row m (rows that share a cell each receive that cell's
+ * gradient, as torch's index_put backward gives them), a pure copy.  grad_canvas [B,C,ny,nx] fp32 contiguous, grad_feat [M,C] fp32.
+ * Precondition: the coordinates passed sstb200_recover_bev (no check here, so no stream synchronisation); a row outside the
+ * canvas gets zeros and nothing is read for it. */
+int sstb200_recover_bev_backward(sstb200_ctx* ctx, const float* grad_canvas, const int64_t* coors, int num_voxels, int channels,
+                                 int batch_size, int ny, int nx, float* grad_feat);
+
 /* N1  Voxel2PointScatterNeck.forward (mmdet3d/models/necks/voxel2point_neck.py:28-62; SURVEY 8f next-2): points [N,Cp] fp32,
  * pts_coors [N,4] int64 (b,z,y,x), voxel_feats [M,C] fp32 (rows of dropped voxels hold `padding`), voxel2point_inds [N] int64.
  * out [<=N, C(+3)] receives, for every point whose voxel row is not all-padding and in input order, the voxel row followed (with_xyz)
@@ -334,6 +341,14 @@ int sstb200_voxel2point(sstb200_ctx* ctx, const float* points, int point_dims, c
                         int num_voxels, int channels, const int64_t* voxel2point_inds, int num_points, float padding,
                         const float voxel_size[3], const float pc_min[3], int with_xyz, int normalize_local_xyz, float* out,
                         uint8_t* mask_out, int32_t* num_out_dev, int32_t* num_out_host);
+
+/* N1 backward (gradient w.r.t. voxel_feats only): grad_out [num_kept, C(+3 if with_xyz)] fp32 is the gradient of the forward's
+ * `out`, mask [N] its mask_out and num_kept its row count.  grad_voxel [M,C] fp32 receives, for each voxel v, the sum of
+ * grad_out[pos(p), 0:C] over the kept points p with voxel2point_inds[p] == v (pos = rank among the kept points); voxels no kept
+ * point references (padded rows among them) get 0.  Summed in fp64 without float atomics, so two calls give the same bits.
+ * No stream synchronisation; indices outside [0, M) are skipped. */
+int sstb200_voxel2point_backward(sstb200_ctx* ctx, const float* grad_out, const uint8_t* mask, const int64_t* voxel2point_inds,
+                                 int num_points, int num_kept, int num_voxels, int channels, int with_xyz, float* grad_voxel);
 
 /* A4  the whole encoder stack (SSTv2.forward's block loop, mmdet3d/models/backbones/sst_v2.py:129-133 with
  * BasicShiftBlockV2.forward, models/sst/sst_basic_block_v2.py:144-169): layer l uses the windows of shift l % 2.

@@ -1,5 +1,5 @@
 // Bitmap-rank index ("unique rows, sorted" without a sort), CSR grouping and segmented reduce.
-// Shared by voxel.cu / window.cu / vfe.cu / sir.cu.
+// Shared by voxel.cu / window.cu / vfe.cu / sir.cu / neck.cu.
 #pragma once
 #include "common.cuh"
 
@@ -283,7 +283,7 @@ __global__ void __launch_bounds__(256) segment_reduce_kernel(const float* __rest
                                                              const int32_t* __restrict__ order, int nseg_host,
                                                              const int32_t* __restrict__ nseg_dev, int mode,
                                                              float empty_value, float* __restrict__ out,
-                                                             long long* __restrict__ argmax, int n_rows) {
+                                                             long long* __restrict__ argmax, int n_rows, int ld) {
   pdl_wait();
   pdl_launch();
   int nseg = nseg_dev ? *nseg_dev : nseg_host;
@@ -297,7 +297,7 @@ __global__ void __launch_bounds__(256) segment_reduce_kernel(const float* __rest
         long long am = n_rows;
         for (uint32_t k = b; k < e; k++) {
           int p = order[k];
-          float v = src[(size_t)p * C + c];
+          float v = src[(size_t)p * ld + c];
           if (v > m || (v == m && p < am)) {
             m = v;
             am = p;
@@ -309,7 +309,7 @@ __global__ void __launch_bounds__(256) segment_reduce_kernel(const float* __rest
       } else {
         // fp64 accumulation: exact for these magnitudes, so the result does not depend on CSR order
         double acc = 0.0;
-        for (uint32_t k = b; k < e; k++) acc += (double)src[(size_t)order[k] * C + c];
+        for (uint32_t k = b; k < e; k++) acc += (double)src[(size_t)order[k] * ld + c];
         float r = (float)acc;
         if (mode == SSTB200_REDUCE_MEAN && e > b) r = (float)acc / (float)(e - b);
         out[(size_t)s * C + c] = r;
@@ -328,14 +328,14 @@ __global__ void __launch_bounds__(256) segment_reduce_v4_kernel(const float* __r
                                                                 const int32_t* __restrict__ order, int nseg_host,
                                                                 const int32_t* __restrict__ nseg_dev, int mode,
                                                                 float empty_value, float* __restrict__ out,
-                                                                long long* __restrict__ argmax, int n_rows) {
+                                                                long long* __restrict__ argmax, int n_rows, int ld) {
   pdl_wait();
   pdl_launch();
   constexpr int RIF = NV4 == 1 ? 8 : 4;  // rows in flight per lane (independent 16-byte loads)
   const int nseg = nseg_dev ? *nseg_dev : nseg_host;
   const int groups_per_block = blockDim.x / GROUP;
   const int g = threadIdx.x / GROUP, l = threadIdx.x % GROUP;
-  const int C4 = C >> 2;
+  const int C4 = C >> 2, ld4 = ld >> 2;
   const float4* __restrict__ src4 = reinterpret_cast<const float4*>(src);
   // lanes of a group always run the same trip counts, but different groups of a warp do not: shuffles are group-masked
   const unsigned gmask = GROUP == 32 ? 0xffffffffu : (((1u << GROUP) - 1u) << ((threadIdx.x & 31) / GROUP * GROUP));
@@ -368,7 +368,7 @@ __global__ void __launch_bounds__(256) segment_reduce_v4_kernel(const float* __r
         for (int u = 0; u < RIF; u++)
 #pragma unroll
           for (int j = 0; j < NV4; j++)
-            v[u][j] = (p[u] >= 0 && l + j * GROUP < C4) ? __ldg(&src4[(size_t)p[u] * C4 + l + j * GROUP]) : make_float4(fill, fill, fill, fill);
+            v[u][j] = (p[u] >= 0 && l + j * GROUP < C4) ? __ldg(&src4[(size_t)p[u] * ld4 + l + j * GROUP]) : make_float4(fill, fill, fill, fill);
         if (mode == SSTB200_REDUCE_MAX && !ARG) {
           // plain max: absent rows were loaded as -inf, one FMNMX per element
 #pragma unroll
@@ -437,17 +437,18 @@ __global__ void __launch_bounds__(256) segment_reduce_v4_kernel(const float* __r
 
 static void launch_segment_reduce(sstb200_ctx* c, const float* src, int C, const uint32_t* offsets,
                                   const int32_t* order, int nseg_cap, const int32_t* nseg_dev, int mode,
-                                  float empty_value, float* out, long long* argmax, int n_rows) {
+                                  float empty_value, float* out, long long* argmax, int n_rows, int ld = 0) {
   int grid = c->num_sms * 8;
-  const bool vec = (C % 4 == 0) && C <= 256 && (((uintptr_t)src | (uintptr_t)out | (uintptr_t)argmax) & 15) == 0;
+  if (ld <= 0) ld = C;  // source row pitch in floats (>= C): e.g. the C leading columns of [rows, C + 3] neck gradients
+  const bool vec = (C % 4 == 0) && (ld % 4 == 0) && C <= 256 && (((uintptr_t)src | (uintptr_t)out | (uintptr_t)argmax) & 15) == 0;
 #define SEGV4(G, NV)                                                                                                                     \
   do {                                                                                                                                  \
     if (argmax)                                                                                                                         \
       launch_pdl(segment_reduce_v4_kernel<G, NV, true>, dim3(grid), dim3(256), (size_t)(0), c->stream, src, C, offsets, order, nseg_cap, \
-                 nseg_dev, mode, empty_value, out, argmax, n_rows);                                                                     \
+                 nseg_dev, mode, empty_value, out, argmax, n_rows, ld);                                                                 \
     else                                                                                                                                \
       launch_pdl(segment_reduce_v4_kernel<G, NV, false>, dim3(grid), dim3(256), (size_t)(0), c->stream, src, C, offsets, order, nseg_cap, \
-                 nseg_dev, mode, empty_value, out, argmax, n_rows);                                                                     \
+                 nseg_dev, mode, empty_value, out, argmax, n_rows, ld);                                                                 \
   } while (0)
   if (vec) {
     int c4 = C / 4;
@@ -462,11 +463,11 @@ static void launch_segment_reduce(sstb200_ctx* c, const float* src, int C, const
   }
 #undef SEGV4
   if (C >= 32)
-    launch_pdl(segment_reduce_kernel<32>, dim3(grid), dim3(256), (size_t)(0), c->stream, src, C, offsets, order, nseg_cap, nseg_dev, mode, empty_value, out, argmax, n_rows);
+    launch_pdl(segment_reduce_kernel<32>, dim3(grid), dim3(256), (size_t)(0), c->stream, src, C, offsets, order, nseg_cap, nseg_dev, mode, empty_value, out, argmax, n_rows, ld);
   else if (C > 4)
-    launch_pdl(segment_reduce_kernel<8>, dim3(grid), dim3(256), (size_t)(0), c->stream, src, C, offsets, order, nseg_cap, nseg_dev, mode, empty_value, out, argmax, n_rows);
+    launch_pdl(segment_reduce_kernel<8>, dim3(grid), dim3(256), (size_t)(0), c->stream, src, C, offsets, order, nseg_cap, nseg_dev, mode, empty_value, out, argmax, n_rows, ld);
   else
-    launch_pdl(segment_reduce_kernel<4>, dim3(grid), dim3(256), (size_t)(0), c->stream, src, C, offsets, order, nseg_cap, nseg_dev, mode, empty_value, out, argmax, n_rows);
+    launch_pdl(segment_reduce_kernel<4>, dim3(grid), dim3(256), (size_t)(0), c->stream, src, C, offsets, order, nseg_cap, nseg_dev, mode, empty_value, out, argmax, n_rows, ld);
 }
 
 // CSR over a map -> (offsets[nseg+1], order[n]) ; count must already hold per-segment counts.

@@ -6,6 +6,7 @@
 // pass, a look-back scan over the keep flags (order-preserving compaction) and one warp-per-point write pass.
 #include <stdarg.h>
 #include "common.cuh"
+#include "index.cuh"
 
 __global__ void __launch_bounds__(256) v2p_mask_kernel(const float* __restrict__ voxel_feats, int C, const long long* __restrict__ inds, int N,
                                                        int M, float padding, uint32_t* __restrict__ keep, uint8_t* __restrict__ mask_out,
@@ -95,5 +96,68 @@ extern "C" int sstb200_voxel2point(sstb200_ctx* c, const float* points, int Cp, 
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   if (c->pinned_i32[1]) return sstb_fail(c, SSTB_ERR_ARG, "voxel2point: voxel2point_inds out of range [0, %d)", M);
   if (num_out_host) *num_out_host = c->pinned_i32[0];
+  return SSTB_OK;
+}
+
+// ---- backward: grad_voxel[v] = sum of grad_out[pos(p), 0:C] over the kept points p with inds[p] == v ------------------------------
+// The kept points' voxel ids are compacted to their output rows (the forward's scan over the mask), grouped into a CSR and summed
+// by the shared segmented reduce, reading grad_out with its row pitch C(+3).  Its fp64 accumulation makes the sum independent of
+// the CSR order, so the result is deterministic without float atomics; voxels no kept point references get 0.
+struct LoadMaskU8 {
+  const uint8_t* p;
+  __device__ __forceinline__ uint32_t operator()(size_t i) const { return p[i] ? 1u : 0u; }
+  __device__ __forceinline__ void load8(size_t base, size_t n, uint32_t* v) const {
+#pragma unroll
+    for (int i = 0; i < 8; i++) v[i] = (base + i < n && p[base + i]) ? 1u : 0u;
+  }
+};
+
+__global__ void __launch_bounds__(256) v2p_compact_kernel(const uint8_t* __restrict__ mask, const uint32_t* __restrict__ pos,
+                                                          const long long* __restrict__ inds, int N, int K, int M,
+                                                          long long* __restrict__ row_voxel) {
+  pdl_wait();
+  pdl_launch();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N || !mask[i]) return;
+  const uint32_t r = pos[i];
+  if (r >= (uint32_t)K) return;  // a mask with more kept points than grad_out has rows: never write past K
+  const long long v = inds[i];
+  row_voxel[r] = (v >= 0 && v < M) ? v : -1;  // -1: not counted, not grouped (csr_fill skips it)
+}
+
+extern "C" int sstb200_voxel2point_backward(sstb200_ctx* c, const float* grad_out, const uint8_t* mask, const int64_t* voxel2point_inds,
+                                            int N, int K, int M, int C, int with_xyz, float* grad_voxel) {
+  CHECK_ARG(c, c && N >= 0 && K >= 0 && K <= N && M >= 0 && C >= 1);
+  if (M == 0) return SSTB_OK;
+  CHECK_ARG(c, grad_voxel);
+  if (K == 0) {
+    CUDA_TRY(c, cudaMemsetAsync(grad_voxel, 0, (size_t)M * C * 4, c->stream));
+    return SSTB_OK;
+  }
+  CHECK_ARG(c, grad_out && mask && voxel2point_inds);
+  const int ld = C + (with_xyz ? 3 : 0);
+  arena_reset(c);
+  int rc = arena_reserve(c, al256((size_t)N * 4 + 64) + scan_temps_bytes(N) + al256((size_t)K * 8) + al256((size_t)M * 4 + 4) +
+                                csr_bytes(K, M) + 4096);
+  if (rc) return rc;
+  uint32_t* pos = arena_alloc<uint32_t>(c, (size_t)N + 2);
+  uint8_t* z = arena_alloc<uint8_t>(c, scan_temps_bytes(N));
+  long long* row_voxel = arena_alloc<long long>(c, (size_t)K);
+  int32_t* count = arena_alloc<int32_t>(c, (size_t)M + 1);
+  if (!pos || !z || !row_voxel || !count) return sstb_fail(c, SSTB_ERR_WORKSPACE, "voxel2point_backward: arena");
+  ScanTemps st{(uint32_t*)z, (unsigned long long*)z + 32};
+  int32_t* err = (int32_t*)(st.ticket + 2);  // count_index_kernel's flag for -1 rows; nothing reads it
+  CUDA_TRY(c, cudaMemsetAsync(z, 0, scan_temps_bytes(N), c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(row_voxel, 0xFF, (size_t)K * 8, c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(count, 0, (size_t)M * 4, c->stream));
+  launch_exclusive_scan(c->stream, LoadMaskU8{mask}, (size_t)N, nullptr, st, pos, st.ticket + 1, true);
+  launch_pdl(v2p_compact_kernel, dim3((N + 255) / 256), dim3(256), (size_t)0, c->stream, mask, (const uint32_t*)pos,
+             (const long long*)voxel2point_inds, N, K, M, row_voxel);
+  launch_pdl(count_index_kernel, dim3((K + 255) / 256), dim3(256), (size_t)0, c->stream, (const long long*)row_voxel, K, M, count, err);
+  Csr r;
+  rc = csr_build(c, r, (const long long*)row_voxel, K, count, (size_t)M, nullptr);
+  if (rc) return rc;
+  launch_segment_reduce(c, grad_out, C, r.offsets, r.order, M, nullptr, SSTB200_REDUCE_SUM, 0.f, grad_voxel, nullptr, K, ld);
+  LAUNCH_CHECK(c);
   return SSTB_OK;
 }

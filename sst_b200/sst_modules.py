@@ -233,6 +233,7 @@ class SSTInputLayerV2(nn.Module):
 # SRA encoder
 # ------------------------------------------------------------------------------------------------
 L.SIGNATURES["sstb200_recover_bev"] = (C.c_int, [L.vp, L.vp, L.vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, L.vp])
+L.SIGNATURES["sstb200_recover_bev_backward"] = (C.c_int, [L.vp, L.vp, L.vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, L.vp])
 
 
 class _SraLayer(C.Structure):
@@ -498,17 +499,44 @@ class SSTv2(nn.Module):
 
     def recover_bev(self, voxel_feat, coors, batch_size):
         """models/backbones/sst_v2.py:161-196: sparse rows -> dense [B, C, ny, nx] canvas in one HBM-write-bound pass
-        (csrc/bev.cu; the canvas is written exactly once, zeros included)."""
+        (csrc/bev.cu; the canvas is written exactly once, zeros included).  With a gradient to propagate, the canvas gradient
+        is gathered back to the rows by sstb200_recover_bev_backward."""
         ny, nx = self.output_shape
         ops._need_cuda(voxel_feat, coors)
-        voxel_feat = voxel_feat.float().contiguous()
         coors = coors.long().contiguous()
-        M, C_ = voxel_feat.shape
-        canvas = torch.empty((batch_size, C_, ny, nx), dtype=torch.float32, device=voxel_feat.device)
-        c = L.ctx(voxel_feat.device)
-        L.check(c, L.lib().sstb200_recover_bev(c, voxel_feat.data_ptr(), coors.data_ptr(), M, C_, batch_size, ny, nx,
-                                               canvas.data_ptr()))
-        return canvas
+        if torch.is_grad_enabled() and voxel_feat.requires_grad:
+            return _RecoverBevFunction.apply(voxel_feat.float(), coors, batch_size, ny, nx)
+        return _recover_bev(voxel_feat.float().contiguous(), coors, batch_size, ny, nx)
+
+
+def _recover_bev(voxel_feat, coors, batch_size, ny, nx):
+    M, C_ = voxel_feat.shape
+    canvas = torch.empty((batch_size, C_, ny, nx), dtype=torch.float32, device=voxel_feat.device)
+    c = L.ctx(voxel_feat.device)
+    L.check(c, L.lib().sstb200_recover_bev(c, voxel_feat.data_ptr(), coors.data_ptr(), M, C_, batch_size, ny, nx,
+                                           canvas.data_ptr()))
+    return canvas
+
+
+class _RecoverBevFunction(torch.autograd.Function):
+    """recover_bev with its backward: d voxel_feat[m] = d canvas[b_m, :, y_m, x_m] for every row (rows sharing a cell each
+    receive that cell's gradient, like the reference's index_put).  Saves only the coordinates and the canvas shape."""
+
+    @staticmethod
+    def forward(ctx, voxel_feat, coors, batch_size, ny, nx):
+        ctx.save_for_backward(coors)
+        ctx.shape = (voxel_feat.shape[0], voxel_feat.shape[1], batch_size, ny, nx)
+        return _recover_bev(voxel_feat.contiguous(), coors, batch_size, ny, nx)
+
+    @staticmethod
+    def backward(ctx, grad_canvas):
+        (coors,) = ctx.saved_tensors
+        M, C_, B, ny, nx = ctx.shape
+        g = grad_canvas.float().contiguous()
+        grad = torch.empty((M, C_), dtype=torch.float32, device=g.device)
+        c = L.ctx(g.device)
+        L.check(c, L.lib().sstb200_recover_bev_backward(c, g.data_ptr(), coors.data_ptr(), M, C_, B, ny, nx, grad.data_ptr()))
+        return grad, None, None, None, None
 
 
 # ------------------------------------------------------------------------------------------------
