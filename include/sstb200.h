@@ -315,6 +315,33 @@ int sstb200_sir_layer_forward_ex(sstb200_ctx* ctx, const sstb200_sir_layer* laye
                                  const int32_t* csr_offsets, const int32_t* csr_order, int precision, float* out_point,
                                  int out_point_ld, float* out_group);
 
+/* S1 training (fp32, as the reference trains SIRLayer under @force_fp32).  Range: mode_max, rel-MLP present with rel_in <= 32 and
+ * widths <= 256, 1-2 VFE layers with feat_channels multiples of 32 and <= 256, in_channels in [3, 256]; anything else is
+ * SSTB_ERR_UNSUPPORTED.  num_points = 0 or num_groups = 0 launches nothing (and writes nothing).
+ * forward_train: the inputs of sstb200_sir_layer_forward_ex on dense fp32 rows, the same outputs as the fp32 eval forward, and a
+ * caller-owned `state` of sstb200_sir_layer_train_state_bytes() bytes (the pre-LayerNorm values of the VFE layers and the row of
+ * each group max, the lowest point index attaining it) that the backward reads.  The state must outlive the backward call. */
+size_t sstb200_sir_layer_train_state_bytes(const sstb200_sir_layer* layer, int num_points, int num_groups);
+int sstb200_sir_layer_forward_train(sstb200_ctx* ctx, const sstb200_sir_layer* layer, const float* in_feats, const float* f_cluster,
+                                    const int64_t* inv, int num_points, int num_groups, const int32_t* csr_offsets,
+                                    const int32_t* csr_order, float* out_point, float* out_group, void* state, size_t state_bytes);
+/* Parameter gradients in the layout of the parameters (rel_w[i] [dims[i], in_i], vfe_w[i] [C_i, in_i], ...); written, not added. */
+typedef struct {
+  float* rel_w[4];
+  float* rel_ln_w[4];
+  float* rel_ln_b[4];
+  float* vfe_w[2];
+  float* vfe_ln_w[2];
+  float* vfe_ln_b[2];
+} sstb200_sir_layer_grads;
+/* backward of forward_train with the same layer, inputs, CSR and state: grad_point [N, C_last] (d loss / d out_point) and
+ * grad_group [G, C0+C1] (d loss / d out_group), either NULL = zero.  Writes grad_in_feats [N, in_channels] and grad_f_cluster
+ * [N, rel_in] (each NULL = skipped) and every gradient of `grads`.  No float atomics: two calls give the same bits. */
+int sstb200_sir_layer_backward(sstb200_ctx* ctx, const sstb200_sir_layer* layer, const float* in_feats, const float* f_cluster,
+                               const int64_t* inv, int num_points, int num_groups, const int32_t* csr_offsets, const int32_t* csr_order,
+                               const void* state, size_t state_bytes, const float* grad_point, const float* grad_group,
+                               float* grad_in_feats, float* grad_f_cluster, const sstb200_sir_layer_grads* grads);
+
 /* Points grouped by `inv` (values in [0, num_groups)): offsets [num_groups+1] int32, order [num_points] int32 (order inside a
  * group unspecified).  What SIR.forward (models/backbones/sir.py:67-87, `unique_once`) shares between its blocks. */
 int sstb200_group_csr(sstb200_ctx* ctx, const int64_t* inv, int num_points, int num_groups, int32_t* offsets, int32_t* order);

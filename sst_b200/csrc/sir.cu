@@ -10,21 +10,15 @@
 // The reference runs this as ~25 ATen/torch_scatter launches per block with [N,256] concat tensors and float
 // atomics.  Here: one warp-per-point kernel for the relation MLP + gating, FFMA row GEMMs with fused LN/act,
 // and a sorted segmented max (CSR order, in-tile reduce, order-preserving atomicMax only at tile edges).
+//
+// Training (sstb200_sir_layer_forward_train) runs this same fp32 forward; it writes the pre-LN values to the caller's state and
+// takes each group max with its arg-max row (launch_segment_reduce) - the backward is in sir_train.cu.
 #include <stdarg.h>
 #include "index.cuh"
+#include "sir.cuh"
 #include "sra.cuh"
 
 // ---- relation MLP + gating: one warp per point -----------------------------------------------------
-struct RelDev {
-  int cin, n_rel, dims[4], rel_in, act;
-  float eps, inv_norm[3], rel_dist_scaler;
-  const float *w[4], *g[4], *b[4];
-};
-
-__device__ __forceinline__ float act_fn(float x, int act) { return act == 2 ? gelu_erf(x) : fmaxf(x, 0.f); }
-
-#define REL_MAXC 8  // channels per lane (Cin <= 256)
-
 __global__ void __launch_bounds__(256) sir_rel_gate_kernel(RelDev r, const float* __restrict__ feats /*[N,cin]*/,
                                                            const float* __restrict__ f_cluster /*[N,3]*/, int N,
                                                            float* __restrict__ x0 /*[N,cin]*/) {
@@ -192,6 +186,10 @@ static int group_csr(sstb200_ctx* c, const long long* inv, int N, int G, int32_t
   return SSTB_OK;
 }
 
+int sstb_sir_group_csr(sstb200_ctx* c, const long long* inv, int N, int G, int32_t* offsets, int32_t* order) {
+  return group_csr(c, inv, N, G, offsets, order);
+}
+
 extern "C" int sstb200_group_csr(sstb200_ctx* c, const int64_t* inv, int N, int G, int32_t* offsets, int32_t* order) {
   CHECK_ARG(c, c && N >= 0 && G >= 0);
   if (N == 0 || G == 0) return SSTB_OK;
@@ -200,6 +198,168 @@ extern "C" int sstb200_group_csr(sstb200_ctx* c, const int64_t* inv, int N, int 
   int rc = arena_reserve(c, csr_bytes(N, G) + al256((size_t)G * 4 + 8) + 65536);
   if (rc) return rc;
   return group_csr(c, (const long long*)inv, N, G, offsets, order);
+}
+
+int sstb_sir_rel_dev(sstb200_ctx* c, const sstb200_sir_layer* L, RelDev* rd, size_t* smem_out) {
+  if (L->num_rel <= 0) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "SIRLayer without rel-MLP is not built");
+  rd->cin = L->in_channels;
+  rd->n_rel = L->num_rel;
+  rd->rel_in = L->rel_in;
+  rd->act = L->act;
+  rd->eps = L->norm_eps;
+  rd->rel_dist_scaler = L->rel_dist_scaler;
+  size_t smem = 0;
+  int in = L->rel_in;
+  for (int l = 0; l < 4; l++) {
+    rd->dims[l] = l < L->num_rel ? L->rel_dims[l] : 0;
+    rd->w[l] = L->rel_w[l];
+    rd->g[l] = L->rel_ln_w[l];
+    rd->b[l] = L->rel_ln_b[l];
+    if (l < L->num_rel) {
+      CHECK_ARG(c, rd->w[l] && rd->g[l] && rd->b[l]);
+      smem += (size_t)in * rd->dims[l] * 4;
+      in = rd->dims[l];
+    }
+  }
+  for (int i = 0; i < 3; i++) rd->inv_norm[i] = L->xyz_normalizer[i];
+  if (smem > 200 * 1024) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "rel-MLP weights do not fit shared memory");
+  *smem_out = smem;
+  return SSTB_OK;
+}
+
+int sstb_sir_rel_gate(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster, int N, float* x0) {
+  RelDev rd;
+  size_t smem = 0;
+  int rc = sstb_sir_rel_dev(c, L, &rd, &smem);
+  if (rc) return rc;
+  static SmemAttr sa;
+  CUDA_TRY(c, ensure_smem(c, sa, sir_rel_gate_kernel, (size_t)200 * 1024));
+  launch_pdl(sir_rel_gate_kernel, dim3(c->num_sms * 4), dim3(256), (size_t)(smem), c->stream, rd, in_feats, f_cluster, N, x0);
+  return SSTB_OK;
+}
+
+// [G, C] dense -> columns col0.. of out [G, ldo]
+__global__ void copy_cols_kernel(const float* __restrict__ src, int G, int C, float* __restrict__ out, int ldo, int col0) {
+  pdl_wait();
+  pdl_launch();
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)G * C) return;
+  out[(i / C) * ldo + col0 + i % C] = src[i];
+}
+
+// Group max of src [N, C] into columns col0.. of out_group.  Eval: sorted max kernels (no arg-max).  Training (am != NULL): the
+// segmented reduce with its arg-max (lowest point index attaining the max) through the dense [G, C] scratch gtmp.
+static void sir_group_max(sstb200_ctx* c, const float* src, int C, const int32_t* off, const int32_t* order, const long long* inv, int N, int G,
+                          uint32_t* gord, float* gtmp, long long* am, float* out_group, int Cg, int col0) {
+  cudaStream_t st = c->stream;
+  size_t gn = (size_t)G * C;
+  if (am) {
+    launch_segment_reduce(c, src, C, (const uint32_t*)off, order, G, nullptr, SSTB200_REDUCE_MAX, 0.f, gtmp, am, N);
+    launch_pdl(copy_cols_kernel, dim3((unsigned)((gn + 255) / 256)), dim3(256), (size_t)(0), st, (const float*)gtmp, G, C, out_group, Cg, col0);
+    return;
+  }
+  launch_pdl(fill_u32_kernel, dim3((unsigned)((gn + 255) / 256)), dim3(256), (size_t)(0), st, gord, gn, 0u);
+  launch_pdl(segmax_sorted_kernel, dim3((N + SEG_ROWS - 1) / SEG_ROWS), dim3(128), (size_t)(0), st, src, C, order, inv, N, gord);
+  launch_pdl(segmax_finalize_kernel, dim3((unsigned)((gn + 255) / 256)), dim3(256), (size_t)(0), st, (const uint32_t*)gord, G, C, out_group, Cg, col0);
+}
+
+// The fp32 forward.  s == NULL: eval.  s != NULL: training - t0 / t1 land in the state, the group maxima record their arg-max
+// rows there (off = the group CSR offsets), everything else is the same launch sequence.
+static int sir_forward_fp32(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster, const long long* inv,
+                            int N, int G, const int32_t* off, const int32_t* order, uint32_t* gord, float* gterm, float* out_point,
+                            float* out_group, const SirState* s) {
+  cudaStream_t st = c->stream;
+  const int cin = L->in_channels, C0 = L->feat_channels[0], C1 = L->num_vfe > 1 ? L->feat_channels[1] : 0;
+  const int Cmax = C0 > C1 ? C0 : C1;
+  float* x0 = arena_alloc<float>(c, (size_t)N * cin);
+  float* t = s ? nullptr : arena_alloc<float>(c, (size_t)N * Cmax);
+  float* p0 = arena_alloc<float>(c, (size_t)N * Cmax);
+  if (!x0 || (!s && !t) || !p0) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
+  float* t0 = s ? s->t0 : t;
+  float* t1 = s ? s->t1 : t;
+
+  // 1. relation MLP + gating
+  int rc = sstb_sir_rel_gate(c, L, in_feats, f_cluster, N, x0);
+  if (rc) return rc;
+  // 2. layer 0: p0 = act(LN(W0 x0)); g0 = segmax(p0)
+  CHECK_ARG(c, L->vfe_w[0] && L->vfe_ln_w[0] && L->vfe_ln_b[0]);
+  sstb_gemm_rows_ex(st, x0, cin, L->vfe_w[0], cin, nullptr, nullptr, 0, nullptr, t0, C0, N, nullptr, C0, cin, 0, nullptr, nullptr, 0, 0, 0, 0);
+  float* p0out = (C1 == 0) ? out_point : p0;
+  sstb_add_norm_act(st, t0, nullptr, L->vfe_ln_w[0], L->vfe_ln_b[0], nullptr, nullptr, L->norm_eps, p0out, N, nullptr, C0, L->act);
+  const int Cg = C0 + C1;
+  sir_group_max(c, p0out, C0, off, order, inv, N, G, gord, gterm, s ? s->am0 : nullptr, out_group, Cg, 0);
+  if (C1) {
+    CHECK_ARG(c, L->vfe_w[1] && L->vfe_ln_w[1] && L->vfe_ln_b[1]);
+    // 3. layer 1 on [p0 || g0[group]]:  W1a p0 + (W1b g0)[group]
+    sstb_gemm_rows_ex(st, out_group, Cg, L->vfe_w[1] + C0, 2 * C0, nullptr, nullptr, 0, nullptr, gterm, C1, G, nullptr, C1, C0, 0, nullptr,
+                      nullptr, 0, 0, 0, 0);
+    sstb_gemm_rows_ex(st, p0, C0, L->vfe_w[1], 2 * C0, nullptr, gterm, C1, inv, t1, C1, N, nullptr, C1, C0, 0, nullptr,
+                      nullptr, 0, 0, 0, 0);
+    sstb_add_norm_act(st, t1, nullptr, L->vfe_ln_w[1], L->vfe_ln_b[1], nullptr, nullptr, L->norm_eps, out_point, N, nullptr, C1, L->act);
+    sir_group_max(c, out_point, C1, off, order, inv, N, G, gord, gterm, s ? s->am1 : nullptr, out_group, Cg, C0);
+  }
+  {
+    int Cl = C1 ? C1 : C0;
+    if (L->with_shortcut && cin - 3 == Cl)
+      launch_pdl(shortcut_kernel, dim3((unsigned)(((size_t)N * Cl + 255) / 256)), dim3(256), (size_t)(0), st, out_point, in_feats, N, Cl, cin);
+  }
+  LAUNCH_CHECK(c);
+  return SSTB_OK;
+}
+
+int sstb_sir_train_check(sstb200_ctx* c, const sstb200_sir_layer* L) {
+  CHECK_ARG(c, L->num_vfe >= 1 && L->num_vfe <= 2 && L->num_rel >= 0 && L->num_rel <= 4 && (L->act == 1 || L->act == 2));
+  if (!L->mode_max) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "SIRLayer training: only mode='max' is built");
+  if (L->num_rel == 0) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "SIRLayer training: a layer without rel-MLP is not built");
+  const int cin = L->in_channels, C0 = L->feat_channels[0], C1 = L->num_vfe > 1 ? L->feat_channels[1] : 0;
+  if (cin < 3 || cin > 32 * REL_MAXC || C0 <= 0 || C0 > 256 || C1 > 256 || C0 % 32 || C1 % 32)
+    return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "SIRLayer training: dims (cin=%d, C0=%d, C1=%d) not supported", cin, C0, C1);
+  if (L->rel_in < 1 || L->rel_in > 32) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "SIRLayer training: rel_mlp_in_channel %d (1..32)", L->rel_in);
+  for (int l = 0; l < L->num_rel; l++)
+    if (L->rel_dims[l] < 1 || L->rel_dims[l] > 32 * REL_MAXC)
+      return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "SIRLayer training: rel-MLP width %d", L->rel_dims[l]);
+  if (L->rel_dims[L->num_rel - 1] != cin) return sstb_fail(c, SSTB_ERR_ARG, "last rel-MLP layer must produce in_channels");
+  return SSTB_OK;
+}
+
+extern "C" size_t sstb200_sir_layer_train_state_bytes(const sstb200_sir_layer* L, int N, int G) {
+  if (!L || N < 0 || G < 0 || L->num_vfe < 1 || L->num_vfe > 2) return 0;
+  return sir_state_layout(N, G, L->feat_channels[0], L->num_vfe > 1 ? L->feat_channels[1] : 0, nullptr, nullptr);
+}
+
+extern "C" int sstb200_sir_layer_forward_train(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster,
+                                               const int64_t* inv, int N, int G, const int32_t* csr_offsets, const int32_t* csr_order,
+                                               float* out_point, float* out_group, void* state, size_t state_bytes) {
+  CHECK_ARG(c, c && L && N >= 0 && G >= 0);
+  int rc = sstb_sir_train_check(c, L);
+  if (rc) return rc;
+  if (N == 0 || G == 0) return SSTB_OK;
+  CHECK_ARG(c, in_feats && f_cluster && inv && out_point && out_group && state);
+  CHECK_ARG(c, (csr_offsets == nullptr) == (csr_order == nullptr));
+  const int cin = L->in_channels, C0 = L->feat_channels[0], C1 = L->num_vfe > 1 ? L->feat_channels[1] : 0;
+  const int Cmax = C0 > C1 ? C0 : C1;
+  SirState s;
+  if (state_bytes < sir_state_layout(N, G, C0, C1, state, &s))
+    return sstb_fail(c, SSTB_ERR_WORKSPACE, "SIRLayer training state: %zu bytes given, %zu needed", state_bytes,
+                     sir_state_layout(N, G, C0, C1, nullptr, nullptr));
+  arena_reset(c);
+  rc = arena_reserve(c, csr_bytes(N, G) + al256((size_t)G * 4 + 8) + al256((size_t)N * cin * 4) + al256((size_t)N * Cmax * 4) +
+                            2 * al256((size_t)G * Cmax * 4) + 2 * al256(((size_t)N + 4) * 4) + 65536);
+  if (rc) return rc;
+  const int32_t *off = csr_offsets, *order = csr_order;
+  if (!order) {
+    int32_t* o = arena_alloc<int32_t>(c, (size_t)G + 2);
+    int32_t* ord = arena_alloc<int32_t>(c, (size_t)N + 1);
+    if (!o || !ord) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
+    rc = group_csr(c, (const long long*)inv, N, G, o, ord);
+    if (rc) return rc;
+    off = o;
+    order = ord;
+  }
+  uint32_t* gord = arena_alloc<uint32_t>(c, (size_t)G * Cmax);
+  float* gterm = arena_alloc<float>(c, (size_t)G * Cmax);
+  if (!gord || !gterm) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
+  return sir_forward_fp32(c, L, in_feats, f_cluster, (const long long*)inv, N, G, off, order, gord, gterm, out_point, out_group, &s);
 }
 
 int sstb_sir_layer_bf16(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster, const long long* inv,
@@ -262,73 +422,7 @@ extern "C" int sstb200_sir_layer_forward_ex(sstb200_ctx* c, const sstb200_sir_la
     LAUNCH_CHECK(c);
     return SSTB_OK;
   }
-  float* x0 = arena_alloc<float>(c, (size_t)N * cin);
-  float* t = arena_alloc<float>(c, (size_t)N * Cmax);
-  float* p0 = arena_alloc<float>(c, (size_t)N * Cmax);
-  if (!x0 || !t || !p0) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
-
-  // 1. relation MLP + gating
-  const float* xin = in_feats;
-  if (L->num_rel > 0) {
-    RelDev rd;
-    rd.cin = cin;
-    rd.n_rel = L->num_rel;
-    rd.rel_in = L->rel_in;
-    rd.act = L->act;
-    rd.eps = L->norm_eps;
-    rd.rel_dist_scaler = L->rel_dist_scaler;
-    size_t smem = 0;
-    int in = L->rel_in;
-    for (int l = 0; l < 4; l++) {
-      rd.dims[l] = l < L->num_rel ? L->rel_dims[l] : 0;
-      rd.w[l] = L->rel_w[l];
-      rd.g[l] = L->rel_ln_w[l];
-      rd.b[l] = L->rel_ln_b[l];
-      if (l < L->num_rel) {
-        CHECK_ARG(c, rd.w[l] && rd.g[l] && rd.b[l]);
-        smem += (size_t)in * rd.dims[l] * 4;
-        in = rd.dims[l];
-      }
-    }
-    for (int i = 0; i < 3; i++) rd.inv_norm[i] = L->xyz_normalizer[i];
-    if (smem > 200 * 1024) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "rel-MLP weights do not fit shared memory");
-    static SmemAttr sa;
-    CUDA_TRY(c, ensure_smem(c, sa, sir_rel_gate_kernel, (size_t)200 * 1024));
-    launch_pdl(sir_rel_gate_kernel, dim3(c->num_sms * 4), dim3(256), (size_t)(smem), st, rd, in_feats, f_cluster, N, x0);
-    xin = x0;
-  } else {
-    return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "SIRLayer without rel-MLP is not built");
-  }
-  // 2. layer 0: p0 = act(LN(W0 x0)); g0 = segmax(p0)
-  CHECK_ARG(c, L->vfe_w[0] && L->vfe_ln_w[0] && L->vfe_ln_b[0]);
-  sstb_gemm_rows_ex(st, xin, cin, L->vfe_w[0], cin, nullptr, nullptr, 0, nullptr, t, C0, N, nullptr, C0, cin, 0, nullptr, nullptr, 0, 0, 0, 0);
-  float* p0out = (C1 == 0) ? out_point : p0;
-  sstb_add_norm_act(st, t, nullptr, L->vfe_ln_w[0], L->vfe_ln_b[0], nullptr, nullptr, L->norm_eps, p0out, N, nullptr, C0, L->act);
-  const int Cg = C0 + C1;
-  size_t gn = (size_t)G * C0;
-  launch_pdl(fill_u32_kernel, dim3((unsigned)((gn + 255) / 256)), dim3(256), (size_t)(0), st, gord, gn, 0u);
-  launch_pdl(segmax_sorted_kernel, dim3((N + SEG_ROWS - 1) / SEG_ROWS), dim3(128), (size_t)(0), st, p0out, C0, order, (const long long*)inv, N, gord);
-  launch_pdl(segmax_finalize_kernel, dim3((unsigned)((gn + 255) / 256)), dim3(256), (size_t)(0), st, gord, G, C0, out_group, Cg, 0);
-  if (C1) {
-    CHECK_ARG(c, L->vfe_w[1] && L->vfe_ln_w[1] && L->vfe_ln_b[1]);
-    // 3. layer 1 on [p0 || g0[group]]:  W1a p0 + (W1b g0)[group]
-    sstb_gemm_rows_ex(st, out_group, Cg, L->vfe_w[1] + C0, 2 * C0, nullptr, nullptr, 0, nullptr, gterm, C1, G, nullptr, C1, C0, 0, nullptr,
-                      nullptr, 0, 0, 0, 0);
-    sstb_gemm_rows_ex(st, p0, C0, L->vfe_w[1], 2 * C0, nullptr, gterm, C1, (const long long*)inv, t, C1, N, nullptr, C1, C0, 0, nullptr,
-                      nullptr, 0, 0, 0, 0);
-    sstb_add_norm_act(st, t, nullptr, L->vfe_ln_w[1], L->vfe_ln_b[1], nullptr, nullptr, L->norm_eps, out_point, N, nullptr, C1, L->act);
-    gn = (size_t)G * C1;
-    launch_pdl(fill_u32_kernel, dim3((unsigned)((gn + 255) / 256)), dim3(256), (size_t)(0), st, gord, gn, 0u);
-    launch_pdl(segmax_sorted_kernel, dim3((N + SEG_ROWS - 1) / SEG_ROWS), dim3(128), (size_t)(0), st, out_point, C1, order, (const long long*)inv, N, gord);
-    launch_pdl(segmax_finalize_kernel, dim3((unsigned)((gn + 255) / 256)), dim3(256), (size_t)(0), st, gord, G, C1, out_group, Cg, C0);
-  }
-  {
-    int Cl = C1 ? C1 : C0;
-    if (L->with_shortcut && cin - 3 == Cl)
-      launch_pdl(shortcut_kernel, dim3((unsigned)(((size_t)N * Cl + 255) / 256)), dim3(256), (size_t)(0), st, out_point, in_feats, N, Cl, cin);
-  }
-  LAUNCH_CHECK(c);
-  return SSTB_OK;
+  return sir_forward_fp32(c, L, in_feats, f_cluster, (const long long*)inv, N, G, nullptr, order, gord, gterm, out_point, out_group, nullptr);
 }
 
 extern "C" int sstb200_sir_layer_forward(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster,

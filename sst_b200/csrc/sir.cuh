@@ -1,0 +1,45 @@
+// SIRLayer pieces shared by the forward (sir.cu) and the training backward (sir_train.cu).
+#pragma once
+#include "common.cuh"
+
+// relation-MLP parameters as the warp-per-point kernels read them
+struct RelDev {
+  int cin, n_rel, dims[4], rel_in, act;
+  float eps, inv_norm[3], rel_dist_scaler;
+  const float *w[4], *g[4], *b[4];
+};
+
+#define REL_MAXC 8  // channels per lane (Cin <= 256)
+
+__device__ __forceinline__ float act_fn(float x, int act) { return act == 2 ? gelu_erf(x) : fmaxf(x, 0.f); }
+
+// What sstb200_sir_layer_forward_train keeps for the backward, carved out of the caller's state buffer: the pre-LayerNorm
+// values of both VFE layers and the row that attains each group max (lowest point index on ties).  x0, the rel-MLP and p0 are
+// recomputed by the backward.
+struct SirState {
+  float* t0;       // [N, C0]
+  float* t1;       // [N, C1] (C1 > 0)
+  long long* am0;  // [G, C0]
+  long long* am1;  // [G, C1] (C1 > 0)
+};
+static inline size_t sir_state_layout(int N, int G, int C0, int C1, void* base, SirState* s) {
+  size_t o0 = 0, o1 = o0 + al256((size_t)N * C0 * 4), o2 = o1 + al256((size_t)N * C1 * 4), o3 = o2 + al256((size_t)G * C0 * 8);
+  size_t end = o3 + al256((size_t)G * C1 * 8);
+  if (s) {
+    char* b = (char*)base;
+    s->t0 = (float*)(b + o0);
+    s->t1 = C1 ? (float*)(b + o1) : nullptr;
+    s->am0 = (long long*)(b + o2);
+    s->am1 = C1 ? (long long*)(b + o3) : nullptr;
+  }
+  return end;
+}
+
+// fills `rd` from the layer and checks the rel-MLP (SSTB_OK or an error code with the message set); *smem = its weight bytes
+int sstb_sir_rel_dev(sstb200_ctx* c, const sstb200_sir_layer* L, RelDev* rd, size_t* smem);
+// x0 = [xyz / xyz_normalizer || rest] * rel_mlp(f_cluster / rel_dist_scaler)   [N, cin]
+int sstb_sir_rel_gate(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster, int N, float* x0);
+// group CSR into caller buffers (offsets [G+2], order [N+1]) from the arena-reserved context, as sstb200_group_csr builds it
+int sstb_sir_group_csr(sstb200_ctx* c, const long long* inv, int N, int G, int32_t* offsets, int32_t* order);
+// the range the fp32 training path covers (SSTB_ERR_UNSUPPORTED / SSTB_ERR_ARG with a message otherwise)
+int sstb_sir_train_check(sstb200_ctx* c, const sstb200_sir_layer* L);

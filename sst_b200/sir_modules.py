@@ -4,12 +4,14 @@
     SIR        mmdet3d/models/backbones/sir.py:15-87
 
 Same constructor kwargs / forward signatures / state-dict keys (`rel_mlp.{k}.{0,1}.*`,
-`vfe_layers.{j}.{linear,norm}.*`).  Eval forward = one sstb200_sir_layer_forward call per block.
+`vfe_layers.{j}.{linear,norm}.*`).  Eval forward = one sstb200_sir_layer_forward call per block; with gradients, one
+SirLayerFunction (sstb200_sir_layer_forward_train / _backward, fp32) per block.
 """
 import ctypes as C
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import _lib as L
 from . import ops
@@ -32,6 +34,79 @@ L.SIGNATURES["sstb200_sir_layer_forward_ex"] = (C.c_int, [L.vp, C.POINTER(_SirLa
                                                           C.c_int, C.c_int, L.vp, L.vp, C.c_int, L.vp, C.c_int, L.vp])
 L.SIGNATURES["sstb200_group_csr"] = (C.c_int, [L.vp, L.vp, C.c_int, C.c_int, L.vp, L.vp])
 _PREC = {"fp32": 0, "bf16": 1}
+
+
+class _SirGrads(C.Structure):
+    _fields_ = [("rel_w", C.c_void_p * 4), ("rel_ln_w", C.c_void_p * 4), ("rel_ln_b", C.c_void_p * 4), ("vfe_w", C.c_void_p * 2),
+                ("vfe_ln_w", C.c_void_p * 2), ("vfe_ln_b", C.c_void_p * 2)]
+
+
+L.SIGNATURES["sstb200_sir_layer_train_state_bytes"] = (C.c_size_t, [C.POINTER(_SirLayer), C.c_int, C.c_int])
+L.SIGNATURES["sstb200_sir_layer_forward_train"] = (C.c_int, [L.vp, C.POINTER(_SirLayer), L.vp, L.vp, L.vp, C.c_int, C.c_int, L.vp, L.vp,
+                                                             L.vp, L.vp, L.vp, C.c_size_t])
+L.SIGNATURES["sstb200_sir_layer_backward"] = (C.c_int, [L.vp, C.POINTER(_SirLayer), L.vp, L.vp, L.vp, C.c_int, C.c_int, L.vp, L.vp, L.vp,
+                                                        C.c_size_t, L.vp, L.vp, L.vp, L.vp, C.POINTER(_SirGrads)])
+
+
+class SirLayerFunction(torch.autograd.Function):
+    """(point_feats [N, C_last], group_feats [G, C0+C1]) = one SIRLayer in fp32 through sstb200_sir_layer_forward_train /
+    _backward.  The parameters are explicit inputs (SIRLayer._train_params order) so that autograd routes their gradients;
+    the layer's state (pre-LN values and arg-max rows) lives on ctx until the backward."""
+
+    @staticmethod
+    def forward(ctx, layer, with_shortcut, in_feats, f_cluster, unq_inv, num_groups, csr, *params):
+        ops._need_cuda(in_feats, f_cluster, unq_inv)
+        in_feats = in_feats.float().contiguous()
+        f_cluster = f_cluster.float().contiguous()
+        unq_inv = unq_inv.long().contiguous()
+        params = [p.contiguous() for p in params]
+        N, G, dev = in_feats.shape[0], num_groups, in_feats.device
+        assert in_feats.shape[1] == layer.in_channels and f_cluster.shape == (N, layer.rel_in), (in_feats.shape, f_cluster.shape)
+        point = torch.empty((N, layer.feat_channels[-1]), dtype=torch.float32, device=dev)
+        group = torch.empty((G, sum(layer.feat_channels)), dtype=torch.float32, device=dev)
+        s = layer._struct(params)
+        s.with_shortcut = int(with_shortcut)
+        if csr is None and N and G:
+            csr = group_csr(unq_inv, G)
+        off, order = csr if csr is not None else (None, None)
+        nbytes = L.lib().sstb200_sir_layer_train_state_bytes(C.byref(s), N, G)
+        state = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+        c = L.ctx(dev)
+        L.check(c, L.lib().sstb200_sir_layer_forward_train(
+            c, C.byref(s), in_feats.data_ptr(), f_cluster.data_ptr(), unq_inv.data_ptr(), N, G, L.ptr(off), L.ptr(order),
+            point.data_ptr(), group.data_ptr(), state.data_ptr(), nbytes))
+        ctx.save_for_backward(in_feats, f_cluster, unq_inv, *params)
+        ctx.layer, ctx.with_shortcut, ctx.G, ctx.csr, ctx.state = layer, with_shortcut, G, (off, order), state
+        ctx.set_materialize_grads(False)  # an unused output arrives as None and is passed as NULL
+        return point, group
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_point, d_group):
+        in_feats, f_cluster, unq_inv, *params = ctx.saved_tensors
+        N, G = in_feats.shape[0], ctx.G
+        d_point = None if d_point is None else d_point.float().contiguous()
+        d_group = None if d_group is None else d_group.float().contiguous()
+        want_in, want_fc = ctx.needs_input_grad[2], ctx.needs_input_grad[3]
+        pg = [torch.zeros_like(p) for p in params]
+        if not (N and G and (d_point is not None or d_group is not None)):
+            return (None, None, torch.zeros_like(in_feats) if want_in else None, torch.zeros_like(f_cluster) if want_fc else None,
+                    None, None, None, *pg)
+        g_in = torch.empty_like(in_feats) if want_in else None
+        g_fc = torch.empty_like(f_cluster) if want_fc else None
+        s = ctx.layer._struct(params)
+        s.with_shortcut = int(ctx.with_shortcut)
+        gs = _SirGrads()
+        for i in range(s.num_rel):
+            gs.rel_w[i], gs.rel_ln_w[i], gs.rel_ln_b[i] = (t.data_ptr() for t in pg[3 * i:3 * i + 3])
+        for i in range(s.num_vfe):
+            gs.vfe_w[i], gs.vfe_ln_w[i], gs.vfe_ln_b[i] = (t.data_ptr() for t in pg[3 * (s.num_rel + i):3 * (s.num_rel + i) + 3])
+        off, order = ctx.csr
+        c = L.ctx(in_feats.device)
+        L.check(c, L.lib().sstb200_sir_layer_backward(
+            c, C.byref(s), in_feats.data_ptr(), f_cluster.data_ptr(), unq_inv.data_ptr(), N, G, L.ptr(off), L.ptr(order),
+            ctx.state.data_ptr(), ctx.state.numel(), L.ptr(d_point), L.ptr(d_group), L.ptr(g_in), L.ptr(g_fc), C.byref(gs)))
+        return (None, None, g_in, g_fc, None, None, None, *pg)
 
 
 def group_csr(unq_inv, num_groups):
@@ -69,6 +144,7 @@ class SIRLayer(nn.Module):
         self.act = act
         self.norm_eps = norm_cfg.get("eps", 1e-5)
         self.norm_type = norm_cfg["type"]
+        self.dropout_p = dropout
         self.fp16_enabled = False
         if with_rel_mlp:
             # the reference appends in place (voxel_encoder.py:665); a fresh list keeps shared config lists intact
@@ -89,23 +165,37 @@ class SIRLayer(nn.Module):
         self.num_vfe = len(layers)
         self.feat_channels = list(feat_channels)
 
-    def _struct(self):
+    def _train_params(self):
+        """The parameters the fused layer reads, in _struct's order: per rel-MLP layer (weight, LN weight, LN bias), then per VFE
+        layer (linear weight, LN weight, LN bias)."""
+        ps = []
+        for i in range(len(self.rel_dims)):
+            ps += [self.rel_mlp[i][0].weight, self.rel_mlp[i][1].weight, self.rel_mlp[i][1].bias]
+        for l in self.vfe_layers:
+            ps += [l.linear.weight, l.norm.weight, l.norm.bias]
+        return ps
+
+    def _native_train(self):
+        """The variants the fused training path covers (SirLayerFunction); the others train through _forward_composed."""
+        return (self.norm_type == "LN" and self._with_rel_mlp and 1 <= self.num_vfe <= 2 and len(self.rel_dims) <= 4
+                and self.mode == "max" and self.dropout_p == 0 and self.act in ("relu", "gelu"))
+
+    def _struct(self, params=None):
         if self.norm_type != "LN":
             raise NotImplementedError("fused SIRLayer expects norm_cfg type 'LN' (as in configs/fsd)")
         if not self._with_rel_mlp or self.num_vfe > 2 or len(self.rel_dims) > 4:
             raise NotImplementedError("SIRLayer variant not built")
+        ptrs = [p.data_ptr() for p in (self._train_params() if params is None else params)]
         s = _SirLayer()
         s.in_channels, s.rel_in, s.num_rel = self.in_channels, self.rel_in, len(self.rel_dims)
         for i, d in enumerate(self.rel_dims):
             s.rel_dims[i] = d
-            s.rel_w[i] = self.rel_mlp[i][0].weight.data_ptr()
-            s.rel_ln_w[i] = self.rel_mlp[i][1].weight.data_ptr()
-            s.rel_ln_b[i] = self.rel_mlp[i][1].bias.data_ptr()
+            s.rel_w[i], s.rel_ln_w[i], s.rel_ln_b[i] = ptrs[3 * i:3 * i + 3]
         s.num_vfe = self.num_vfe
-        for i, l in enumerate(self.vfe_layers):
+        k = 3 * len(self.rel_dims)
+        for i in range(self.num_vfe):
             s.feat_channels[i] = self.feat_channels[i]
-            s.vfe_w[i] = l.linear.weight.data_ptr()
-            s.vfe_ln_w[i], s.vfe_ln_b[i] = l.norm.weight.data_ptr(), l.norm.bias.data_ptr()
+            s.vfe_w[i], s.vfe_ln_w[i], s.vfe_ln_b[i] = ptrs[k + 3 * i:k + 3 * i + 3]
         s.act = {"relu": 1, "gelu": 2}[self.act]
         s.mode_max = int(self.mode == "max")
         s.with_shortcut = int(bool(self.with_shortcut))
@@ -159,6 +249,30 @@ class SIRLayer(nn.Module):
             return voxel_feats, new_coors, unq_inv
         return voxel_feats, new_coors
 
+    def _forward_train(self, features, coors, f_cluster, return_inv, return_both, unq_inv_once, new_coors_once, csr_once):
+        """The training forward in fp32 (the reference runs SIRLayer under @force_fp32, whatever `precision` says): one
+        SirLayerFunction call; f_cluster=None is built from the group mean here, so autograd carries its gradient to `features`."""
+        ops._need_cuda(features, coors)
+        features = features.float()
+        if unq_inv_once is None:
+            new_coors, unq_inv = ops.unique_rows(coors.long())
+        else:
+            new_coors, unq_inv = new_coors_once, unq_inv_once
+        G = new_coors.shape[0]
+        if f_cluster is None:  # voxel_encoder.py:717-723 (the division by rel_dist_scaler happens inside the kernels)
+            mean, _ = ops.segment_reduce(features[:, :3].contiguous(), unq_inv, "mean", G, want_argmax=False)
+            f_cluster = features[:, :3] - mean[unq_inv]
+        wants_shortcut = return_both or self.return_point_feats
+        point_feats, voxel_feats = SirLayerFunction.apply(self, bool(self.with_shortcut) and wants_shortcut, features, f_cluster.float(),
+                                                          unq_inv, G, csr_once, *self._train_params())
+        if return_both:
+            return point_feats, voxel_feats, new_coors
+        if self.return_point_feats:
+            return point_feats, voxel_feats
+        if return_inv:
+            return voxel_feats, new_coors, unq_inv
+        return voxel_feats, new_coors
+
     def forward(self, features, coors, f_cluster=None, points=None, img_feats=None, img_metas=None, return_inv=False,
                 return_both=False, unq_inv_once=None, new_coors_once=None, csr_once=None, point_feats_out=None, feat_gap=None):
         """`csr_once` = group_csr(unq_inv, G) shared between blocks; `point_feats_out` = a [N, >=C] fp32 view (last dim
@@ -166,6 +280,8 @@ class SIRLayer(nn.Module):
         block i's output straight into block i+1's [points || feats] input).  `feat_gap` = (at, width): `features` is that
         hand-over buffer, whose columns >= at sit `width` floats further right (bf16 path)."""
         if torch.is_grad_enabled() and (self.training or features.requires_grad or (f_cluster is not None and f_cluster.requires_grad)):
+            if features.is_cuda and self._native_train():
+                return self._forward_train(features, coors, f_cluster, return_inv, return_both, unq_inv_once, new_coors_once, csr_once)
             return self._forward_composed(features, coors, f_cluster, return_inv, return_both, unq_inv_once, new_coors_once)
         ops._need_cuda(features, coors)
         features = features.float().contiguous()
