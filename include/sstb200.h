@@ -406,7 +406,9 @@ size_t sstb200_sra_train_workspace_bytes(int n, int num_layers);
 int sstb200_sra_stack_forward_train(sstb200_ctx* ctx, const sstb200_sra_layer* layers, int num_layers,
                                     const sstb200_sra_plan* plan_shift0, const sstb200_sra_plan* plan_shift1, const float* x,
                                     float* y_out, void* workspace, int n);
-/* dy [n,128] = d loss / d y_out  ->  dx [n,128] = d loss / d x, parameter gradients accumulated into `grads` */
+/* dy [n,128] = d loss / d y_out  ->  dx [n,128] = d loss / d x, parameter gradients accumulated into `grads`.  Every reduction
+ * runs in a fixed order without float atomics, so two calls give the same bits, and the result equals G0 + g bit for bit, where
+ * G0 is what `grads` held and g what the call adds to zeroed buffers.  n == 0 touches neither dx nor `grads`. */
 int sstb200_sra_stack_backward(sstb200_ctx* ctx, const sstb200_sra_layer* layers, const sstb200_sra_layer_wt* wt,
                                const sstb200_sra_layer_grads* grads, int num_layers, const sstb200_sra_plan* plan_shift0,
                                const sstb200_sra_plan* plan_shift1, const float* x, void* workspace, const float* dy, float* dx,

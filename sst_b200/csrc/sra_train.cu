@@ -68,13 +68,16 @@ static TrainWs train_ws(int n, int L) {
 
 // ------------------------------------------------------------------------------------------------
 // LayerNorm backward over 128-wide rows: dt = rstd * (dy g - mean(dy g) - xhat mean(dy g xhat)), xhat from the saved pre-LN
-// sum t.  One warp per row (4 columns per lane); per-column sums of dy xhat (-> d gamma), dy (-> d beta) and dt (-> d of the
-// bias that was added before the LayerNorm) are kept in registers across the warp's rows and flushed with one atomic per
-// column and block.
+// sum t, with the variance taken as the forward epilogue takes it: E[t^2] - mean^2 while mean^2 <= E[t^2] / 2 (then the
+// subtraction loses at most one bit), else from the centred values in a second pass, so that a large common offset in t does
+// not cancel it.  One warp per row (4 columns per lane);
+// per-column sums of dy xhat (-> d gamma), dy (-> d beta) and dt (-> d of the bias that was added before the LayerNorm) are
+// kept in registers across the warp's rows, summed over the block's warps in a fixed order and written to part[block][3][128];
+// ln_reduce_kernel adds the blocks' partials in a fixed order, so two calls give the same bits.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ t, const float* __restrict__ gamma,
                                                      float eps, int n, float* __restrict__ dt, __nv_bfloat16* __restrict__ dtb,
-                                                     float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias) {
+                                                     float* __restrict__ part) {
   pdl_wait();
   pdl_launch();
   __shared__ float red[3][8][DM];
@@ -88,7 +91,14 @@ __global__ void __launch_bounds__(256) ln_bwd_kernel(const float* __restrict__ d
     s = warp_sum(s);
     q = warp_sum(q);
     const float mean = s * (1.0f / DM);
-    const float rstd = rsqrtf(fmaxf(q * (1.0f / DM) - mean * mean, 0.f) + eps);
+    float var;
+    if (mean * mean > 0.5f * (q * (1.0f / DM))) {   // E[t^2] - mean^2 would cancel: second pass over the centred values (warp-uniform)
+      const float4 d = make_float4(tv.x - mean, tv.y - mean, tv.z - mean, tv.w - mean);
+      var = warp_sum((d.x * d.x + d.y * d.y) + (d.z * d.z + d.w * d.w)) * (1.0f / DM);
+    } else {
+      var = fmaxf(q * (1.0f / DM) - mean * mean, 0.f);
+    }
+    const float rstd = rsqrtf(var + eps);
     const float4 xh = make_float4((tv.x - mean) * rstd, (tv.y - mean) * rstd, (tv.z - mean) * rstd, (tv.w - mean) * rstd);
     const float4 dg = make_float4(dv.x * g4.x, dv.y * g4.y, dv.z * g4.z, dv.w * g4.w);
     float c1 = (dg.x + dg.y) + (dg.z + dg.w), c2 = (dg.x * xh.x + dg.y * xh.y) + (dg.z * xh.z + dg.w * xh.w);
@@ -112,9 +122,47 @@ __global__ void __launch_bounds__(256) ln_bwd_kernel(const float* __restrict__ d
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; w++) v += red[which][w][col];
-    float* dst = which == 0 ? dgamma : (which == 1 ? dbeta : dbias);
-    if (dst) atomicAdd(dst + col, v);
+    part[(size_t)blockIdx.x * 3 * DM + i] = v;
   }
+}
+
+// d gamma / d beta / d bias [col] += sum over the ln_bwd_kernel blocks' partials, in a fixed order.  Block = (sum, 32-column
+// group), 12 blocks; warp w adds the partials of blocks w, w + 8, ... for its lane's column, then warp 0 adds the 8 warp sums
+// in warp order.
+__global__ void __launch_bounds__(256) ln_reduce_kernel(const float* __restrict__ part, int nblk, float* __restrict__ dgamma,
+                                                        float* __restrict__ dbeta, float* __restrict__ dbias) {
+  pdl_wait();
+  pdl_launch();
+  __shared__ float red[8][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int i = blockIdx.x * 32 + lane, which = blockIdx.x / (DM / 32);   // i indexes [3][128]
+  float* dst = which == 0 ? dgamma : (which == 1 ? dbeta : dbias);
+  if (!dst) return;   // uniform per block
+  float s = 0.f;
+#pragma unroll 4
+  for (int b = warp; b < nblk; b += 8) s += part[(size_t)b * 3 * DM + i];
+  red[warp][lane] = s;
+  __syncthreads();
+  if (warp == 0) {
+    float t = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; w++) t += red[w][lane];
+    dst[i % DM] += t;
+  }
+}
+
+static int launch_ln_bwd(sstb200_ctx* c, const float* dy, const float* t, const float* gamma, float eps, int n, float* dt, __nv_bfloat16* dtb,
+                         float* dgamma, float* dbeta, float* dbias) {
+  const int grid = c->num_sms * 2;
+  // per-block partials in the arena; the reduce is enqueued before any later arena_reset can hand the memory out again
+  arena_reset(c);
+  int rc = arena_reserve(c, (size_t)grid * 3 * DM * 4);
+  if (rc) return rc;
+  float* part = arena_alloc<float>(c, (size_t)grid * 3 * DM);
+  if (!part) return sstb_fail(c, SSTB_ERR_WORKSPACE, "LayerNorm partials: arena");
+  CUDA_TRY(c, launch_pdl(ln_bwd_kernel, dim3(grid), dim3(256), (size_t)0, c->stream, dy, t, gamma, eps, n, dt, dtb, part));
+  CUDA_TRY(c, launch_pdl(ln_reduce_kernel, dim3(3 * DM / 32), dim3(256), (size_t)0, c->stream, (const float*)part, grid, dgamma, dbeta, dbias));
+  return SSTB_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -122,7 +170,8 @@ __global__ void __launch_bounds__(256) ln_bwd_kernel(const float* __restrict__ d
 // Work item = (output block, row split).  A CTA walks its rows in slabs of 64 (cp.async double buffer); 8 warps, warp w owns
 // output rows 16w..16w+15 of the block (64 fp32 accumulators per thread); fragments come from the row-major slabs with
 // ldmatrix.trans (both operands are "transposed" for mma.sync: the reduction index is the row).  X is either a bf16 matrix or
-// the fp32 residual stream (+ positional table) converted while staging.  Partial blocks are added with fp32 atomics.
+// the fp32 residual stream (+ positional table) converted while staging.  Each item writes its split's partial block (and the
+// bias partials); dw_reduce_kernel adds them to dW in split order, so two calls give the same bits.
 // ------------------------------------------------------------------------------------------------
 struct DwArgs {
   const __nv_bfloat16* dY;
@@ -637,7 +686,7 @@ __global__ void tau_grad_kernel(const float* __restrict__ part, int nparts, cons
   const float t = tau[h];
   if (t >= tau_min) {
     const float cinv = 1.0f / t;
-    dtau[h] += -cinv * cinv * s;
+    dtau[h] = __fadd_rn(dtau[h], -cinv * cinv * s);   // not contracted into an FMA: the call adds exactly its own d tau
   }
 }
 
@@ -767,7 +816,6 @@ extern "C" int sstb200_sra_stack_backward(sstb200_ctx* c, const sstb200_sra_laye
   float* dx1 = reinterpret_cast<float*>(tmp + w.dx1);
   float* dxbuf[2] = {reinterpret_cast<float*>(tmp + w.dxa), reinterpret_cast<float*>(tmp + w.dxb)};
   const float* dcur = dy;
-  const int ln_grid = c->num_sms * 2;
   for (int l = num_layers - 1; l >= 0; l--) {
     const sstb200_sra_layer* L = &layers[l];
     const sstb200_sra_plan* P = &plans[l & 1];
@@ -779,8 +827,9 @@ extern "C" int sstb200_sra_stack_backward(sstb200_ctx* c, const sstb200_sra_laye
     GemmArgs g;
     int rc;
     // LN2': dt2 (fp32 + bf16), d gamma2, d beta2, d b2
-    CUDA_TRY(c, launch_pdl(ln_bwd_kernel, dim3(ln_grid), dim3(256), (size_t)0, c->stream, dcur, reinterpret_cast<const float*>(lw + w.t2), L->norm2_w,
-                           L->norm_eps, n, dt, dtb, G->norm2_w, G->norm2_b, G->lin2_b));
+    if ((rc = launch_ln_bwd(c, dcur, reinterpret_cast<const float*>(lw + w.t2), L->norm2_w, L->norm_eps, n, dt, dtb, G->norm2_w, G->norm2_b,
+                            G->lin2_b)))
+      return rc;
     // dW2 += dt2^T h
     if ((rc = launch_dw(c, dtb, DM, DM, reinterpret_cast<const __nv_bfloat16*>(lw + w.h), nullptr, DFF, DFF, nullptr, G->lin2_w, n))) return rc;
     // dz = (dt2 W2) * gelu'(z)
@@ -794,8 +843,9 @@ extern "C" int sstb200_sra_stack_backward(sstb200_ctx* c, const sstb200_sra_laye
     g.M_cap = n, g.A = dzb, g.lda = DFF, g.W = T->lin1_wt, g.res = dt, g.out_f32 = dx1;
     if ((rc = launch_umma<256, 128, PRO_H16, EPI_ADD_F32, FMT_BF16>(c, g, 1))) return rc;
     // LN1': dt1, d gamma1, d beta1, d bo
-    CUDA_TRY(c, launch_pdl(ln_bwd_kernel, dim3(ln_grid), dim3(256), (size_t)0, c->stream, (const float*)dx1, reinterpret_cast<const float*>(lw + w.t1),
-                           L->norm1_w, L->norm_eps, n, dt, dtb, G->norm1_w, G->norm1_b, G->out_proj_b));
+    if ((rc = launch_ln_bwd(c, dx1, reinterpret_cast<const float*>(lw + w.t1), L->norm1_w, L->norm_eps, n, dt, dtb, G->norm1_w, G->norm1_b,
+                            G->out_proj_b)))
+      return rc;
     // dWo += dt1^T att ;  datt = dt1 Wo
     if ((rc = launch_dw(c, dtb, DM, DM, reinterpret_cast<const __nv_bfloat16*>(lw + w.att), nullptr, DM, DM, nullptr, G->out_proj_w, n))) return rc;
     memset(&g, 0, sizeof(g));

@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
   uint8_t* sE = base;                           // epilogue staging (aliases the operands)
   constexpr int STAGE = (EPI == EPI_RES_LN || EPI == EPI_ADD_F32) ? TILE_M * NT * 4 : TILE_M * NT * 2;
   float* sAcc = reinterpret_cast<float*>(base + STAGE);   // [128][NT] fp32 accumulators (aliases the operands, not the staging)
-  __shared__ float red[2][TILE_M][2];
+  __shared__ float red[2][TILE_M][EPI == EPI_RES_LN ? 3 : 2];   // per half-row: sum, sum of squares (, centred squares)
   __shared__ int sRow[TILE_M];
 
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -338,12 +338,27 @@ __global__ void __launch_bounds__(256) umma_gemm_kernel(GemmArgs g) {
             *reinterpret_cast<float4*>(g.out_pre + (size_t)gr * NT + ch * 4) =
                 *reinterpret_cast<const float4*>(sE + (size_t)r * NT * 4 + ((ch ^ (r & 31)) << 4));
         }
-        __syncthreads();
       }
       sum = red[0][lrow][0] + red[1][lrow][0];
       sq = red[0][lrow][1] + red[1][lrow][1];
       const float mean = sum * (1.0f / NT);
-      const float var = fmaxf(sq * (1.0f / NT) - mean * mean, 0.f);
+      // E[t^2] - mean^2 loses at most one bit while mean^2 <= E[t^2] / 2; past that (a large common offset in the row) it
+      // cancels, and the row's variance comes from its centred values in a second pass over the staged tile.  Both threads of
+      // a row see the same sums, so they agree on the branch.
+      const bool centred = EPI == EPI_RES_LN && mean * mean > 0.5f * (sq * (1.0f / NT));
+      float csq = 0.f;
+#pragma unroll 1
+      for (int c0 = cbeg; c0 < cbeg + CB && centred; c0 += 4) {
+        const int ch = c0 >> 2;
+        const float4 t = *reinterpret_cast<const float4*>(sE + (size_t)lrow * NT * 4 + ((ch ^ (lrow & 31)) << 4));
+        const float dx = t.x - mean, dy = t.y - mean, dz = t.z - mean, dw = t.w - mean;
+        csq += (dx * dx + dy * dy) + (dz * dz + dw * dw);
+      }
+      if (EPI == EPI_RES_LN) {   // also orders the pre-LayerNorm stores above before the normalisation overwrites the tile
+        red[half][lrow][2] = csq;
+        __syncthreads();
+      }
+      const float var = centred ? (red[0][lrow][2] + red[1][lrow][2]) * (1.0f / NT) : fmaxf(sq * (1.0f / NT) - mean * mean, 0.f);
       const float rstd = rsqrtf(var + g.eps);
 #pragma unroll 1
       for (int c0 = cbeg; c0 < cbeg + CB && EPI == EPI_RES_LN; c0 += 4) {
