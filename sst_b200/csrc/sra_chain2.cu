@@ -62,6 +62,7 @@ struct Chain2Args {
   const float* pos_tab;          // next layer's per-axis positional table, added to y for the q|k chunks
   const int32_t* pos_code;
   int posL, pos_maxw, pos_ndim;
+  int pos_axes;                  // byte grp: the axis of columns [32 grp, 32 grp + 32)
 };
 
 // chunk j of a tile: 0 Wo | 1, 2 W1 rows 0-127, 128-255 | 3, 4 W2 K 0-127, 128-255 | 5, 6, 7 Wqkv rows 0-127, 128-255, 256-383
@@ -82,38 +83,56 @@ __device__ __forceinline__ void st_op(uint32_t buf, int row, int k, uint32_t v) 
   asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(buf + (k >> 6) * OPH + row * 128 + ((((k & 63) >> 3) ^ (row & 7)) << 4) + (k & 7) * 2), "r"(v) : "memory");
 }
 
-// t = fragment of [64 rows x 128] (rows ra: t[4j], t[4j+1]; rb: t[4j+2], t[4j+3]; columns 8j + 2 (lane & 3)): per-row normalisation
+// t = fragment of [64 rows x 128] (rows ra: t[4j], t[4j+1]; rb: t[4j+2], t[4j+3]; columns 8j + 2 (lane & 3)): per-row normalisation.
+// LayerNorm statistics take two passes over the register-resident rows, the mean and then the sum of centred squares, so a large
+// common offset in a row does not cancel the variance away as E[t^2] - mean^2 would.
 __device__ __forceinline__ void row_norm(float (&t)[64], const float* __restrict__ gam, const float* __restrict__ bet, float eps, bool affine) {
   const int cq = 2 * (threadIdx.x & 3);
-  float mean0 = 0.f, mean1 = 0.f, rstd0 = 1.f, rstd1 = 1.f;
-  if (!affine) {
-    float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
+  if (affine) {   // eval BatchNorm folded to one scale and shift per channel
 #pragma unroll
     for (int j = 0; j < 16; j++) {
-      s0 += t[4 * j] + t[4 * j + 1];
-      q0 += t[4 * j] * t[4 * j] + t[4 * j + 1] * t[4 * j + 1];
-      s1 += t[4 * j + 2] + t[4 * j + 3];
-      q1 += t[4 * j + 2] * t[4 * j + 2] + t[4 * j + 3] * t[4 * j + 3];
+      const int c = 8 * j + cq;
+      const float2 g2 = __ldg(reinterpret_cast<const float2*>(gam + c)), b2 = __ldg(reinterpret_cast<const float2*>(bet + c));
+      t[4 * j] = fmaf(t[4 * j], g2.x, b2.x);
+      t[4 * j + 1] = fmaf(t[4 * j + 1], g2.y, b2.y);
+      t[4 * j + 2] = fmaf(t[4 * j + 2], g2.x, b2.x);
+      t[4 * j + 3] = fmaf(t[4 * j + 3], g2.y, b2.y);
     }
-#pragma unroll
-    for (int o = 1; o < 4; o <<= 1) {
-      s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-      q0 += __shfl_xor_sync(0xffffffffu, q0, o);
-      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-      q1 += __shfl_xor_sync(0xffffffffu, q1, o);
-    }
-    mean0 = s0 * (1.f / D), mean1 = s1 * (1.f / D);
-    rstd0 = rsqrtf(fmaxf(q0 * (1.f / D) - mean0 * mean0, 0.f) + eps);
-    rstd1 = rsqrtf(fmaxf(q1 * (1.f / D) - mean1 * mean1, 0.f) + eps);
+    return;
   }
+  float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+  for (int j = 0; j < 16; j++) {
+    s0 += t[4 * j] + t[4 * j + 1];
+    s1 += t[4 * j + 2] + t[4 * j + 3];
+  }
+#pragma unroll
+  for (int o = 1; o < 4; o <<= 1) {
+    s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+  }
+  const float mean0 = s0 * (1.f / D), mean1 = s1 * (1.f / D);
+  float q0 = 0.f, q1 = 0.f;
+#pragma unroll
+  for (int j = 0; j < 16; j++) {
+    t[4 * j] -= mean0, t[4 * j + 1] -= mean0, t[4 * j + 2] -= mean1, t[4 * j + 3] -= mean1;
+    q0 = fmaf(t[4 * j], t[4 * j], fmaf(t[4 * j + 1], t[4 * j + 1], q0));
+    q1 = fmaf(t[4 * j + 2], t[4 * j + 2], fmaf(t[4 * j + 3], t[4 * j + 3], q1));
+  }
+#pragma unroll
+  for (int o = 1; o < 4; o <<= 1) {
+    q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+    q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+  }
+  const float rstd0 = rsqrtf(q0 * (1.f / D) + eps), rstd1 = rsqrtf(q1 * (1.f / D) + eps);
 #pragma unroll
   for (int j = 0; j < 16; j++) {
     const int c = 8 * j + cq;
     const float2 g2 = __ldg(reinterpret_cast<const float2*>(gam + c)), b2 = __ldg(reinterpret_cast<const float2*>(bet + c));
-    t[4 * j] = (t[4 * j] - mean0) * rstd0 * g2.x + b2.x;
-    t[4 * j + 1] = (t[4 * j + 1] - mean0) * rstd0 * g2.y + b2.y;
-    t[4 * j + 2] = (t[4 * j + 2] - mean1) * rstd1 * g2.x + b2.x;
-    t[4 * j + 3] = (t[4 * j + 3] - mean1) * rstd1 * g2.y + b2.y;
+    t[4 * j] = fmaf(t[4 * j] * rstd0, g2.x, b2.x);
+    t[4 * j + 1] = fmaf(t[4 * j + 1] * rstd0, g2.y, b2.y);
+    t[4 * j + 2] = fmaf(t[4 * j + 2] * rstd1, g2.x, b2.x);
+    t[4 * j + 3] = fmaf(t[4 * j + 3] * rstd1, g2.y, b2.y);
   }
 }
 
@@ -139,17 +158,17 @@ __device__ __forceinline__ void st_row_f16(__half* row, const uint32_t (&p)[16],
   }
 }
 
-__device__ __forceinline__ float2 pos_pair(const Chain2Args& g, int code, int c) {
-  const int axis = c / g.posL;   // posL % 32 == 0: the pair lies inside one axis
-  if (axis >= g.pos_ndim) return make_float2(0.f, 0.f);
+// Positional codes of one row for the 32 columns [32 grp, 32 grp + 32), which lie inside one axis (posL % 32 == 0): column c
+// adds pos_row(g, code, grp)[c], or nothing when the pointer is null (the columns lie past the last axis).
+__device__ __forceinline__ const float* pos_row(const Chain2Args& g, int code, int grp) {
+  const int axis = (g.pos_axes >> (8 * grp)) & 255;
+  if (axis >= g.pos_ndim) return nullptr;
   const int cv = (code >> (8 * axis)) & 255;
-  return __ldg(reinterpret_cast<const float2*>(g.pos_tab + ((size_t)axis * g.pos_maxw + cv) * g.posL + (c - axis * g.posL)));
+  return g.pos_tab + ((size_t)axis * (g.pos_maxw - 1) + cv) * g.posL;   // table row (axis, cv), shifted back by the axis's first column
 }
 
 template <bool TAIL>
 __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_constant__ Chain2Maps m, const Chain2Args g) {
-  pdl_wait();
-  pdl_launch();
   extern __shared__ uint8_t chain_raw[];
   uint8_t* base = (uint8_t*)(((uintptr_t)chain_raw + 1023) & ~(uintptr_t)1023);
   const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
@@ -157,10 +176,34 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
   const uint32_t sH = smem_u32(base + wg * WG_BYTES + OFF_H), sR = smem_u32(base + OFF_RING);
   __shared__ __align__(8) uint64_t bar_full[NSLOT], bar_wg0[NSLOT], bar_att[2];
   constexpr int NCH = TAIL ? 8 : 5;
+  static_assert(NCH >= NSLOT, "the chunks loaded before the dependency wait all belong to the CTA's first tile");
+
+  // Before the wait on the preceding kernel: barrier set-up and the first NSLOT weight chunks, all of the CTA's first tile, so the
+  // weight fetch overlaps the tail of the attention kernel.  This is safe because the 16-bit weights are written only by the cast
+  // when a layer's weights are (re)made, which completes before the first kernel of a forward pass starts, and no kernel of the
+  // pass writes them.  Everything the preceding kernels produce (attention output, residual rows, row count, folded BatchNorm)
+  // is read after the wait.  The grid has at most one CTA per tile of the capacity, so every CTA has a first tile unless the
+  // device-side row count is smaller.
+  if (tid == 0) {
+    for (int s = 0; s < NSLOT; s++) {
+      mbar_init(smem_u32(&bar_full[s]), 1);
+      mbar_init(smem_u32(&bar_wg0[s]), 1);
+    }
+    mbar_init(smem_u32(&bar_att[0]), 1);
+    mbar_init(smem_u32(&bar_att[1]), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    for (int n = 0; n < NSLOT; n++) issue_chunk(m, n, sR + n * SLOT, smem_u32(&bar_full[n]));
+  }
+  pdl_wait();
+  pdl_launch();
 
   const int M = g.M_dev ? *g.M_dev : g.M_cap;
   const int ntiles = (M + TM - 1) / TM;
-  if ((int)blockIdx.x >= ntiles) return;   // uniform per CTA, nothing issued yet
+  if ((int)blockIdx.x >= ntiles) {   // uniform per CTA: no tile, but the weight loads above must land before the CTA exits
+    if (tid == 0)
+      for (int s = 0; s < NSLOT; s++) mbar_wait(smem_u32(&bar_full[s]), 0);
+    return;
+  }
   // chunk `n` (counted over the CTA's whole tile sequence) belongs to a tile this CTA will process
   auto chunk_live = [&](int n) { return (int)blockIdx.x + (n / NCH) * (int)gridDim.x < ntiles; };
   const bool leader = (tid & 127) == 0;   // one elected thread per warpgroup
@@ -176,17 +219,6 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
       mbar_arrive(bar);
     }
   };
-  if (tid == 0) {
-    for (int s = 0; s < NSLOT; s++) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_wg0[s]), 1);
-    }
-    mbar_init(smem_u32(&bar_att[0]), 1);
-    mbar_init(smem_u32(&bar_att[1]), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    for (int n = 0; n < NSLOT; n++)
-      if (chunk_live(n)) issue_chunk(m, n % NCH, sR + n * SLOT, smem_u32(&bar_full[n]));
-  }
   __syncthreads();
   if (leader) issue_att(blockIdx.x);
 
@@ -281,41 +313,48 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
       for (int j = 0; j < 16; j++) {
         const int c = 8 * j + cq;
         const float2 b = __ldg(reinterpret_cast<const float2*>(g.b1 + 128 * h + c));
-        st_op(sH, rl, 128 * h + c, pack_f16(gelu_fast(acc[4 * j] + b.x), gelu_fast(acc[4 * j + 1] + b.y)));
-        st_op(sH, rl + 8, 128 * h + c, pack_f16(gelu_fast(acc[4 * j + 2] + b.x), gelu_fast(acc[4 * j + 3] + b.y)));
+        st_op(sH, rl, 128 * h + c, pack_f16(gelu_ex2(acc[4 * j] + b.x), gelu_ex2(acc[4 * j + 1] + b.y)));
+        st_op(sH, rl + 8, 128 * h + c, pack_f16(gelu_ex2(acc[4 * j + 2] + b.x), gelu_ex2(acc[4 * j + 3] + b.y)));
       }
     }
     wg_sync();
 
     // ---- GEMM3 (both K chunks back to back) + bias + x1 + Norm2 -> y (fp32 rows; fp16 y into X and y + pos into H for the tail) --
-    {
-      const uint32_t w0 = acquire(0), w1 = acquire(1);
-      wg_tile_mma<128, false, 8>(acc, sH, OPH, w0, OPB, false);
-      wg_tile_mma<128, false, 8>(acc, sH + 2 * OPH, OPH, w1, OPB, true);
-      wgmma_wait<0>();
-      release(2);
-    }
+    // the accumulators start at x1 + b2, so the MMA adds the residual and the bias and x1 is dead once it is issued
 #pragma unroll
     for (int j = 0; j < 16; j++) {
       const int c = 8 * j + cq;
       const float2 b = __ldg(reinterpret_cast<const float2*>(g.b2 + c));
-      acc[4 * j] += b.x + x1[4 * j];
-      acc[4 * j + 1] += b.y + x1[4 * j + 1];
-      acc[4 * j + 2] += b.x + x1[4 * j + 2];
-      acc[4 * j + 3] += b.y + x1[4 * j + 3];
+      acc[4 * j] = x1[4 * j] + b.x;
+      acc[4 * j + 1] = x1[4 * j + 1] + b.y;
+      acc[4 * j + 2] = x1[4 * j + 2] + b.x;
+      acc[4 * j + 3] = x1[4 * j + 3] + b.y;
+    }
+    {
+      const uint32_t w0 = acquire(0), w1 = acquire(1);
+      wg_tile_mma<128, false, 8>(acc, sH, OPH, w0, OPB, true);
+      wg_tile_mma<128, false, 8>(acc, sH + 2 * OPH, OPH, w1, OPB, true);
+      wgmma_wait<0>();
+      release(2);
     }
     row_norm(acc, g.g2, g.be2, g.eps, g.affine);
 #pragma unroll
-    for (int j = 0; j < 16; j++) {
-      const int c = 8 * j + cq;
-      if (okA) *reinterpret_cast<float2*>(g.y + (size_t)rowA * D + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
-      if (okB) *reinterpret_cast<float2*>(g.y + (size_t)rowB * D + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-      if (TAIL) {
-        st_op(sX, rl, c, pack_f16(acc[4 * j], acc[4 * j + 1]));
-        st_op(sX, rl + 8, c, pack_f16(acc[4 * j + 2], acc[4 * j + 3]));
-        const float2 pa = pos_pair(g, codeA, c), pb = pos_pair(g, codeB, c);
-        st_op(sH, rl, c, pack_f16(acc[4 * j] + pa.x, acc[4 * j + 1] + pa.y));
-        st_op(sH, rl + 8, c, pack_f16(acc[4 * j + 2] + pb.x, acc[4 * j + 3] + pb.y));
+    for (int grp = 0; grp < 4; grp++) {
+      const float* posA = TAIL ? pos_row(g, codeA, grp) : nullptr;
+      const float* posB = TAIL ? pos_row(g, codeB, grp) : nullptr;
+#pragma unroll
+      for (int j = 4 * grp; j < 4 * grp + 4; j++) {
+        const int c = 8 * j + cq;
+        if (okA) *reinterpret_cast<float2*>(g.y + (size_t)rowA * D + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        if (okB) *reinterpret_cast<float2*>(g.y + (size_t)rowB * D + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        if (TAIL) {
+          st_op(sX, rl, c, pack_f16(acc[4 * j], acc[4 * j + 1]));
+          st_op(sX, rl + 8, c, pack_f16(acc[4 * j + 2], acc[4 * j + 3]));
+          const float2 pa = posA ? __ldg(reinterpret_cast<const float2*>(posA + c)) : make_float2(0.f, 0.f);
+          const float2 pb = posB ? __ldg(reinterpret_cast<const float2*>(posB + c)) : make_float2(0.f, 0.f);
+          st_op(sH, rl, c, pack_f16(acc[4 * j] + pa.x, acc[4 * j + 1] + pa.y));
+          st_op(sH, rl + 8, c, pack_f16(acc[4 * j + 2] + pb.x, acc[4 * j + 3] + pb.y));
+        }
       }
     }
     if (!TAIL) continue;
@@ -385,7 +424,7 @@ int sstb_sra_chain2(sstb200_ctx* c, const sstb200_sra_layer* L, const __half* at
   memset(&g, 0, sizeof(g));
   memset(&maps, 0, sizeof(maps));
   const bool tail = next && next_plan && next_qkv;
-  if (tail && (!next_plan->pos_table || !next_plan->pos_code || next_plan->pos_L % 32 != 0 || next_plan->pos_ndim < 1 ||
+  if (tail && (!next_plan->pos_table || !next_plan->pos_code || next_plan->pos_L <= 0 || next_plan->pos_L % 32 != 0 || next_plan->pos_ndim < 1 ||
                next_plan->pos_ndim > 3))
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "fused QKV tail needs the next plan's positional table with a per-axis length that is a multiple of 32");
   int rc = 0;
@@ -402,6 +441,7 @@ int sstb_sra_chain2(sstb200_ctx* c, const sstb200_sra_layer* L, const __half* at
     g.posL = next_plan->pos_L;
     g.pos_maxw = next_plan->pos_maxw;
     g.pos_ndim = next_plan->pos_ndim;
+    for (int grp = 0; grp < 4; grp++) g.pos_axes |= (32 * grp / g.posL) << (8 * grp);
   }
   if (rc) return sstb_fail(c, SSTB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d): operands must be 16-byte aligned", rc);
   g.x = x;
