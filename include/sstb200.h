@@ -40,7 +40,8 @@ typedef struct sstb200_ctx sstb200_ctx;
                              * VFE / SIR tensor paths bf16; the API name of the mode stays 'bf16'. */
 #define SSTB200_PREC_F16 1
 #define SSTB200_PREC_FP32_TC 2 /* sstb200_spconv_forward only: fp32 tolerance on the tensor core - every operand carried as two fp16 numbers
-                                * (hi + residue, 22 significant bits), three wgmma products per stage, fp32 accumulation */
+                                * (hi + residue), three wgmma products per stage, fp32 accumulation.  22 significant bits for
+                                * every element within 2^-16 of the largest one its output row gathers (see sstb200_spconv_forward) */
 
 int sstb200_version(void);
 sstb200_ctx* sstb200_create(int device);
@@ -447,17 +448,28 @@ int sstb200_spconv_table(sstb200_ctx* ctx, const int32_t* in_coors, int n_in, co
 /* out[o, :] = act( (sum_k feats[nbr[o][k], :] . W[k]) * scale + shift + residual[o, :] )   - one launch for conv + folded
  * BatchNorm1d (+ residual add) (+ ReLU).  feats [*, c_in] fp32, weight [KV, c_in, c_out] fp32 = the reference's parameter layout
  * (D,H,W,in,out; mmdet3d/ops/spconv/conv.py:97-98), scale / shift [c_out] or NULL (1 / 0), residual [n_out, c_out] or NULL.
- * precision FP32: FFMA implicit GEMM (c_in, c_out multiples of 4).  precision BF16 (16-bit operands, fp32 accumulation):
- * wgmma implicit GEMM over weight_h16 = IEEE fp16 copy laid out [KV, c_out, c_in]; needs c_in, c_out multiples of 64, KV <= 27.
- * precision FP32_TC: the same kernel in split mode; weight_h16 = [2][KV, c_out, c_in]: the fp16 copy followed by the fp16 residue
- * (w - float(half(w))). */
-int sstb200_spconv_forward(sstb200_ctx* ctx, const float* feats, int c_in, const int32_t* nbr, int n_out, int kernel_volume,
-                           const float* weight, const void* weight_h16, int c_out, const float* scale, const float* shift,
-                           const float* residual, int relu, int precision, float* out);
+ * n_in = rows of feats (every nbr entry is < n_in).
+ * precision FP32: FFMA implicit GEMM (c_in, c_out multiples of 4).  precision BF16 (the name of the mode; the operands are IEEE
+ * fp16, fp32 accumulation): wgmma implicit GEMM over weight_h16 = fp16 copy laid out [KV, c_out, c_in]; needs c_in, c_out multiples
+ * of 64, KV <= 27.  precision FP32_TC: the same kernel in split mode; weight_h16 = [2][KV, c_out, c_in]: the fp16 copy followed by
+ * the fp16 residue (w - float(half(w))).
+ * Operand range of the two tensor-core modes.  fp16 keeps 11 bits only between 2^-14 and 65504, so neither operand is rounded as it
+ * is.  feats: the call first gives every row of feats a power-of-two exponent (one extra small launch, n_in ints of the context's
+ * arena); an output row's operand rows are scaled by the smallest exponent among the rows it gathers, which puts the largest
+ * gathered |element| in [2^13, 2^14), and the accumulator row is scaled back.  weight_h16: the copy may carry one power of two per
+ * output channel, w16[k][co][ci] = half(w[k][ci][co] * 2^e[co]); weight_h16_unscale [c_out] fp32 then holds 2^-e[co] (NULL: the copy
+ * is unscaled, which is accurate only for |w| in about [2^-14, 65504]).  All of this is exact in fp32, so the result is homogeneous:
+ * feats * 2^s or weight * 2^s gives out * 2^s with the same relative error, for any s that keeps out a normal fp32 number.  What
+ * remains is relative to the largest element an output row gathers: elements below 2^-27 of it (BF16; 2^-16 for the
+ * 22 bits of FP32_TC) are rounded with an absolute error of 2^-38 of it instead of a relative one. */
+int sstb200_spconv_forward(sstb200_ctx* ctx, const float* feats, int n_in, int c_in, const int32_t* nbr, int n_out, int kernel_volume,
+                           const float* weight, const void* weight_h16, const float* weight_h16_unscale, int c_out,
+                           const float* scale, const float* shift, const float* residual, int relu, int precision, float* out);
 
 /* Backward of sstb200_spconv_forward without epilogue (indice_conv_backward_fp32, mmdet3d/ops/spconv/src/all.cc:34-35 ->
  * spconv_ops.h:262-420).  The input gradient needs no entry point of its own: dX = sstb200_spconv_forward(dY, nbr_T, W^T) on the
- * TRANSPOSED table (nbr_inv of sstb200_spconv_table; the table SparseInverseConv3d runs on).  This call computes the weight gradient
+ * TRANSPOSED table (nbr_inv of sstb200_spconv_table; the table SparseInverseConv3d runs on); the operand exponents described there
+ * are what keeps it accurate for the 1e-5 ... 1e-8 rows of a mean-reduced loss's gradient.  This call computes the weight gradient
  * grad_weight [KV, c_in, c_out] fp32 (fully written) = sum over pairs of feats[nbr[o][k]]^T . grad_out[o]; fp32 atomics across row
  * chunks, so the last bits depend on the launch like the reference's backward. */
 int sstb200_spconv_backward_weight(sstb200_ctx* ctx, const float* feats, int c_in, const int32_t* nbr, int n_out, int kernel_volume,

@@ -314,6 +314,15 @@ __global__ void __launch_bounds__(256) spconv_dw_kernel(const float* __restrict_
 // walking 100-200 stages each: pure load latency), and a buffer is rewritten only after every warpgroup's group that read it has
 // completed (wgmma.wait_group before the stage barrier).  Offsets no row of the tile uses are skipped.  Epilogue straight from the
 // accumulator fragments: y = acc * scale + shift (+ residual) (ReLU), fp32 rows.
+//
+// Operand range.  fp16 has 5 exponent bits: unscaled, anything below 2^-14 loses bits and anything below 2^-24 is zero - which is
+// where the gradients of a mean-reduced loss live (dX runs this kernel with A = grad_out).  So both operands are brought to the
+// top of the fp16 range by exact powers of two before they are rounded, and the powers are taken out of the fp32 accumulators:
+//   * A: sp_row_exp_kernel gives every input row the exponent that puts its largest |element| in [2^13, 2^14); an OUTPUT row uses
+//     the smallest exponent among the rows it gathers (every offset of an output row meets in one accumulator row, so the exponent
+//     must be one per output row; nothing forces it to be one per tensor), applied while converting, removed per accumulator row.
+//   * W: one exponent per output channel, applied where the 16-bit copy is made (split_h16), removed per accumulator column.
+// The result is homogeneous in the scale of either operand: x * 2^s gives out * 2^s to the last bit while fp32 can hold it.
 // ------------------------------------------------------------------------------------------------------------------------------
 constexpr int SPU_TM = 128;
 constexpr int SPU_A_BYTES = SPU_TM * 128;
@@ -326,8 +335,36 @@ __device__ __forceinline__ uint32_t sp_pack_f16(float a, float b) {
   return r;
 }
 
+constexpr int SPU_EXP_TOP = 14;    // a scaled row's largest |element| lies in [2^13, 2^14): below fp16's 65504 with room for rounding
+constexpr int SPU_EXP_LIM = 100;   // |exponent| bound: 2^+-100 and every product with an fp16-range value are exact fp32
+
+// rexp[i] = the power of two that lifts row i's largest |element| into [2^(SPU_EXP_TOP - 1), 2^SPU_EXP_TOP); one warp per row
+__global__ void __launch_bounds__(256) sp_row_exp_kernel(const float* __restrict__ feats, int lda, int C, int n, const int32_t* __restrict__ n_dev,
+                                                        int32_t* __restrict__ rexp) {
+  pdl_wait();
+  pdl_launch();
+  if (n_dev) n = min(n, *n_dev);
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= n) return;
+  const float4* p = reinterpret_cast<const float4*>(feats + (size_t)row * lda);
+  uint32_t m = 0u;   // |x| as bits: ordered like the magnitudes
+  for (int q = lane; q < (C >> 2); q += 32) {
+    const float4 v = p[q];
+    m = max(max(m, __float_as_uint(v.x) & 0x7fffffffu), max(__float_as_uint(v.y) & 0x7fffffffu, __float_as_uint(v.z) & 0x7fffffffu));
+    m = max(m, __float_as_uint(v.w) & 0x7fffffffu);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  // amax = f * 2^(field - 126), f in [0.5, 1); an all-zero (or subnormal) row takes the largest exponent and never decides a minimum
+  if (lane == 0) rexp[row] = max(-SPU_EXP_LIM, min(SPU_EXP_LIM, SPU_EXP_TOP - ((int)(m >> 23) - 126)));
+}
+
+__device__ __forceinline__ float sp_exp2i(int e) { return __int_as_float((e + 127) << 23); }   // 2^e, |e| <= SPU_EXP_LIM
+
 struct SpArgs {
   const float* feats;      // [*, lda] fp32 rows (gathered through nbr, or row o itself when nbr == nullptr)
+  const int32_t* rexp;     // per-row power-of-two exponents of feats (sp_row_exp_kernel), or nullptr: operands converted as they are
+  const float* wun;        // [Cout] 2^-e of the exponent the 16-bit weight copy carries per output channel, or nullptr (1)
   int lda, Cin;
   const int32_t* nbr;      // [n_out, KV] or nullptr (KV must be 1: a plain row GEMM)
   int n_out;
@@ -350,9 +387,12 @@ struct SpStageRegs {
   uint32_t valid;                 // bit u: piece u has a source row (absent neighbours are neither loaded nor converted)
 };
 
-// SPLIT = the fp32-tolerance mode on the tensor core: every fp32 operand is carried as two fp16 numbers (hi = rn(x), lo = rn(x - hi):
-// 22 significant bits), and a stage issues the three products hi.hi + lo.hi + hi.lo into the same fp32 accumulators (the
-// dropped lo.lo term is 2^-22 relative).  Same staging, same epilogue; 3x the MMAs, 2x the operand bytes.
+// SPLIT = the fp32-tolerance mode on the tensor core: every fp32 operand is carried as two fp16 numbers (hi = rn(x), lo = rn(x - hi)),
+// and a stage issues the three products hi.hi + lo.hi + hi.lo into the same fp32 accumulators (the dropped lo.lo term is 2^-22
+// relative).  Same staging, same epilogue; 3x the MMAs, 2x the operand bytes.  hi + lo carries 22 significant bits of an element
+// while lo is a normal fp16 number, i.e. for scaled |x| >= 2^-3: elements within 2^-16 of their row group's largest.  Smaller
+// ones keep an absolute error of 2^-25 scaled = 2^-38 of that largest element, which is below the fp32 rounding of the sum they
+// are added to.
 template <int NT, int NS, bool SPLIT>
 __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma_kernel(SpArgs g) {
   pdl_wait();
@@ -366,6 +406,7 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
   static_assert(NS >= 2, "the stage barrier retires the group of the stage NS - 1 back");
   __shared__ uint32_t used_mask;
   __shared__ int sNbr[SPU_TM][SPU_MAX_KV];   // odd row pitch: conflict-free column reads
+  __shared__ int sExp[SPU_TM];               // exponent of output row r's gathered operand rows
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int row0 = blockIdx.x * SPU_TM, n0 = blockIdx.y * NT;
@@ -387,6 +428,16 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m |= __shfl_xor_sync(0xffffffffu, m, o);
     if (lane == 0 && m) atomicOr(&used_mask, m);
+  }
+  __syncthreads();
+  if (tid < SPU_TM) {
+    int e = g.rexp ? SPU_EXP_LIM : 0;
+    if (g.rexp)
+      for (int k = 0; k < KV; k++) {
+        const int v = sNbr[tid][k];
+        if (v >= 0) e = min(e, __ldg(g.rexp + v));
+      }
+    sExp[tid] = e;
   }
   __syncthreads();
   const int nch = Cin >> 6;
@@ -436,7 +487,9 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
       const int off = r * 128 + ((my_jj ^ (r & 7)) << 4);
       int4 v = make_int4(0, 0, 0, 0), vl = make_int4(0, 0, 0, 0);
       if ((R.valid >> u) & 1u) {
-        const float f[8] = {R.a0[u].x, R.a0[u].y, R.a0[u].z, R.a0[u].w, R.a1[u].x, R.a1[u].y, R.a1[u].z, R.a1[u].w};
+        const float as = sp_exp2i(sExp[r]);
+        const float f[8] = {R.a0[u].x * as, R.a0[u].y * as, R.a0[u].z * as, R.a0[u].w * as,
+                            R.a1[u].x * as, R.a1[u].y * as, R.a1[u].z * as, R.a1[u].w * as};
         uint32_t hi[4], lo[4];
 #pragma unroll
         for (int e = 0; e < 4; e++) {
@@ -494,6 +547,13 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
     const int o = row0 + wg * 64 + r;
     if (o >= n_out) return;
     const int col = n0 + cc;
+    // the operands' powers of two leave the accumulator first (exact), one factor at a time so that neither can leave fp32's range alone
+    const float ua = sp_exp2i(-sExp[wg * 64 + r]);
+    v0 *= ua, v1 *= ua;
+    if (g.wun) {
+      const float2 uw = __ldg(reinterpret_cast<const float2*>(g.wun + col));
+      v0 *= uw.x, v1 *= uw.y;
+    }
     float2 sc = make_float2(1.f, 1.f), sh = make_float2(0.f, 0.f);
     if (g.scale) sc = __ldg(reinterpret_cast<const float2*>(g.scale + col));
     if (g.shift) sh = __ldg(reinterpret_cast<const float2*>(g.shift + col));
@@ -669,10 +729,10 @@ extern "C" int sstb200_spconv_table(sstb200_ctx* c, const int32_t* in_coors, int
   return SSTB_OK;
 }
 
-extern "C" int sstb200_spconv_forward(sstb200_ctx* c, const float* feats, int c_in, const int32_t* nbr, int n_out, int kernel_volume,
-                                      const float* weight, const void* weight_h16, int c_out, const float* scale, const float* shift,
-                                      const float* residual, int relu, int precision, float* out) {
-  CHECK_ARG(c, c && n_out >= 0 && c_in >= 1 && c_out >= 1 && kernel_volume >= 1);
+extern "C" int sstb200_spconv_forward(sstb200_ctx* c, const float* feats, int n_in, int c_in, const int32_t* nbr, int n_out, int kernel_volume,
+                                      const float* weight, const void* weight_h16, const float* weight_h16_unscale, int c_out,
+                                      const float* scale, const float* shift, const float* residual, int relu, int precision, float* out) {
+  CHECK_ARG(c, c && n_in >= 0 && n_out >= 0 && c_in >= 1 && c_out >= 1 && kernel_volume >= 1);
   if (n_out == 0) return SSTB_OK;
   CHECK_ARG(c, feats && nbr && out);
   CHECK_ARG(c, ((uintptr_t)feats & 15) == 0 && ((uintptr_t)out & 15) == 0 && ((uintptr_t)residual & 15) == 0);
@@ -692,8 +752,16 @@ extern "C" int sstb200_spconv_forward(sstb200_ctx* c, const float* feats, int c_
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED,
                      "spconv_forward: the tensor-core path needs c_in, c_out multiples of 64 and kernel volume <= %d (got %d -> %d, %d); "
                      "use precision fp32", SPU_MAX_KV, c_in, c_out, kernel_volume);
+  // per-row exponents of feats: one small launch (reads feats once; the convolution gathers it kernel_volume times)
+  arena_reset(c);
+  int rc = arena_reserve(c, al256((size_t)n_in * 4) + 4096);
+  if (rc) return rc;
+  int32_t* rexp = arena_alloc<int32_t>(c, (size_t)n_in + 1);
+  if (!rexp) return sstb_fail(c, SSTB_ERR_WORKSPACE, "spconv_forward: arena too small");
+  if (n_in) launch_pdl(sp_row_exp_kernel, dim3((n_in + 7) / 8), dim3(256), (size_t)0, c->stream, feats, c_in, c_in, n_in, (const int32_t*)nullptr, rexp);
   SpArgs g;
-  g.feats = feats, g.lda = c_in, g.Cin = c_in, g.nbr = nbr, g.n_out = n_out, g.n_dev = nullptr, g.KV = kernel_volume;
+  g.feats = feats, g.rexp = rexp, g.wun = weight_h16_unscale;
+  g.lda = c_in, g.Cin = c_in, g.nbr = nbr, g.n_out = n_out, g.n_dev = nullptr, g.KV = kernel_volume;
   g.Whi = (const __half*)weight_h16;
   g.Wlo = g.Whi + (size_t)kernel_volume * c_out * c_in;   // FP32_TC: the residue copy follows the hi copy
   g.Cout = c_out, g.scale = scale, g.shift = shift, g.residual = residual, g.ldr = c_out, g.act = relu ? 1 : 0, g.out = out, g.ldo = c_out;
@@ -712,6 +780,7 @@ int sstb_gemm_rows_x3(sstb200_ctx* c, const float* A, int lda, const float* W, c
   const size_t n = (size_t)N * K;
   launch_pdl(split_f16_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), (size_t)0, c->stream, W, n, hi, lo);
   SpArgs g;
+  g.rexp = nullptr, g.wun = nullptr;   // operands converted as they are: see sra.cuh for the range this leaves the caller
   g.feats = A, g.lda = lda, g.Cin = K, g.nbr = nullptr, g.n_out = M_cap, g.n_dev = M_dev, g.KV = 1, g.Whi = hi, g.Wlo = lo, g.Cout = N;
   g.scale = nullptr, g.shift = bias, g.residual = res, g.ldr = ldr, g.act = act, g.out = out, g.ldo = ldo;
   return dispatch_spconv_umma(c, g, true);

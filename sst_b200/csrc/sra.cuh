@@ -11,6 +11,9 @@ void sstb_gemm_rows_ex(cudaStream_t st, const float* A, int lda, const float* W,
                        int act, const float* pos_tab, const int32_t* pos_code, int posL, int pos_maxw, int pos_ndim, int pos_ncols);
 // fp32-tolerance row GEMM on the tensor core (csrc/spconv.cu, split-fp16 operands): out = act(A . W^T + bias) + res.  Returns
 // SSTB_ERR_UNSUPPORTED (nothing launched) when the shape does not fit (K, N multiples of 64) - callers then use sstb_gemm_rows.
+// Operands are rounded to fp16 pairs as they are (no per-row / per-channel exponents, unlike sstb200_spconv_forward): the 2^-22
+// tolerance holds for |A|, |W| in about [2^-3, 65504] and degrades to an absolute 2^-25 per element below.  Its callers feed it
+// LayerNorm outputs, attention outputs and trained Linear weights, which sit in that range.
 int sstb_gemm_rows_x3(sstb200_ctx* c, const float* A, int lda, const float* W, const float* bias, const float* res, int ldr, float* out,
                       int ldo, int M_cap, const int32_t* M_dev, int N, int K, int act);
 void sstb_add_norm_act(cudaStream_t st, const float* a, const float* b, const float* gamma, const float* beta,

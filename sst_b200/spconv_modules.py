@@ -33,25 +33,49 @@ L.SIGNATURES["sstb200_spconv_out_coors"] = (C.c_int, [L.vp, L.vp, C.c_int, C.c_i
 L.SIGNATURES["sstb200_spconv_table"] = (C.c_int, [L.vp, L.vp, C.c_int, L.vp, C.c_int, C.c_int, L.P_i32, L.P_i32, L.P_i32, L.P_i32,
                                                  L.P_i32, L.vp, L.vp, L.P_i32])
 L.SIGNATURES["sstb200_spconv_backward_weight"] = (C.c_int, [L.vp, L.vp, C.c_int, L.vp, C.c_int, C.c_int, L.vp, C.c_int, L.vp])
-L.SIGNATURES["sstb200_spconv_forward"] = (C.c_int, [L.vp, L.vp, C.c_int, L.vp, C.c_int, C.c_int, L.vp, L.vp, C.c_int, L.vp, L.vp, L.vp,
-                                                   C.c_int, C.c_int, L.vp])
+L.SIGNATURES["sstb200_spconv_forward"] = (C.c_int, [L.vp, L.vp, C.c_int, C.c_int, L.vp, C.c_int, C.c_int, L.vp, L.vp, L.vp, C.c_int, L.vp, L.vp,
+                                                   L.vp, C.c_int, C.c_int, L.vp])
 
-PREC = {"fp32": 0, "bf16": 1, "fp32_tc": 2}   # fp32_tc: fp32 tolerance on the tensor core (split-fp16 operands, 3 products per stage)
+# "bf16" is the name of the 16-bit mode across the package; its sparse-convolution operands are IEEE fp16 (11 significant bits).
+# fp32_tc: fp32 tolerance on the tensor core (split-fp16 operands, 3 products per stage)
+PREC = {"fp32": 0, "bf16": 1, "fp32_tc": 2}
+H16_TOP = 14   # a scaled weight channel's largest |element| lies in [2^13, 2^14): the top of fp16's range, with room for rounding
 
 
 def split_h16(weight):
-    """[KV, Cin, Cout] fp32 -> the 16-bit operand copy of the tensor-core paths, laid out [KV, Cout, Cin]; with residue=True the fp16
-    residue  w - float(half(w))  follows the hi copy ([2 KV, Cout, Cin]) as SSTB200_PREC_FP32_TC expects."""
+    """[KV, Cin, Cout] fp32 -> (hi, lo, unscale): the fp16 operand copy of the tensor-core paths laid out [KV, Cout, Cin], its fp16
+    residue  w - float(half(w))  (SSTB200_PREC_FP32_TC takes cat([hi, lo])), and unscale [Cout] fp32.  Every output channel is
+    multiplied by the power of two that lifts its largest |w| to the top of fp16's range before it is rounded (exact), so that
+    weights of any magnitude keep their bits; unscale holds the inverse powers, which the kernel applies to its accumulators.  No
+    host synchronisation."""
     w = weight.detach().permute(0, 2, 1).contiguous().float()
+    _, e = torch.frexp(w.abs().amax(dim=(0, 2)))                 # amax = f * 2^e, f in [0.5, 1); 0 -> e = 0
+    e = (H16_TOP - e).clamp(-100, 100)
+    w = torch.ldexp(w, e.view(1, -1, 1))
     hi = w.half()
-    return hi, (w - hi.float()).half()
+    return hi, (w - hi.float()).half(), torch.ldexp(torch.ones_like(e, dtype=torch.float32), -e)
+
+
+def _pack_h16(weight, precision):
+    """(weight_h16, unscale) as sstb200_spconv_forward takes them at `precision`"""
+    hi, lo, un = split_h16(weight)
+    return (hi if PREC[precision] == 1 else torch.cat([hi, lo], 0)), un
+
+
+def _cache_key(t):
+    """What a cache derived from tensor t is valid for.  t._version sees torch's in-place writes to t; a parameter that FlatAdamW
+    turned into a view of its flat buffer is also written through that buffer (the fused optimizer step, an all-reduce or a
+    broadcast into it), which only the buffer's own version counter sees."""
+    flat = getattr(t, "_flat_base", None)
+    return (t._version, t.data_ptr(), -1 if flat is None else flat._version)
 FUSE_EPILOGUE = True   # eval mode: fold BatchNorm1d / residual / ReLU into the convolution launch (False = conv launch + torch modules)
 
 
-def _triple(v, ndim):
+def _triple(v, ndim, fill=1):
+    """per-dimension layer argument -> (z, y, x); a 2-D layer is a 3-D one with a z axis of `fill`"""
     v = list(v) if isinstance(v, (list, tuple)) else [v] * ndim
     assert len(v) == ndim
-    return [1] * (3 - ndim) + [int(x) for x in v] if ndim < 3 else [int(x) for x in v]
+    return [fill] * (3 - ndim) + [int(x) for x in v]
 
 
 def _i3(v):
@@ -123,13 +147,21 @@ def _indice_conv_launch(features, nbr, weight, weight_h16, scale, shift, residua
     if residual is not None:
         residual = residual.float().contiguous()
         assert residual.shape == out.shape
+    if precision not in PREC:
+        raise ValueError(f"precision {precision!r}: one of 'fp32' (FFMA), 'bf16' (tensor core, IEEE fp16 operands) or 'fp32_tc' "
+                         "(tensor core, split-fp16 operands)")
     prec = PREC[precision]
-    if prec != 0 and weight_h16 is None:
-        hi, lo = split_h16(weight)
-        weight_h16 = hi if prec == 1 else torch.cat([hi, lo], 0)
+    unscale = None
+    if prec != 0:
+        # weight_h16: (copy, unscale) of _pack_h16, or a plain unscaled fp16 copy (accurate for |w| in about [2^-14, 65504] only)
+        weight_h16, unscale = weight_h16 if isinstance(weight_h16, tuple) else \
+            (_pack_h16(weight, precision) if weight_h16 is None else (weight_h16, None))
+    else:
+        weight_h16 = None
     c = L.ctx(feats.device)
-    L.check(c, L.lib().sstb200_spconv_forward(c, feats.data_ptr(), cin, nbr.data_ptr(), n_out, kv, weight.data_ptr(), L.ptr(weight_h16), cout,
-                                              L.ptr(scale), L.ptr(shift), L.ptr(residual), int(bool(relu)), prec, out.data_ptr()))
+    L.check(c, L.lib().sstb200_spconv_forward(c, feats.data_ptr(), feats.shape[0], cin, nbr.data_ptr(), n_out, kv, weight.data_ptr(),
+                                              L.ptr(weight_h16), L.ptr(unscale), cout, L.ptr(scale), L.ptr(shift), L.ptr(residual),
+                                              int(bool(relu)), prec, out.data_ptr()))
     return out
 
 
@@ -170,7 +202,10 @@ class _IndiceConvFunction(torch.autograd.Function):
 def indice_conv(features, nbr, weight, weight_h16=None, scale=None, shift=None, residual=None, relu=False, precision="fp32",
                 transposed_table=None):
     """out[o] = act((sum_k features[nbr[o,k]] @ weight[k]) * scale + shift + residual[o]); weight [KV, Cin, Cout] fp32.
-    With gradients enabled the call must be epilogue-free and name its transposed table (a callable returning nbr_T [n_in, KV])."""
+    precision: 'fp32' (FFMA), 'bf16' (tensor core, IEEE fp16 operands - the name is the package-wide one of the 16-bit mode) or
+    'fp32_tc' (tensor core, split-fp16 operands).  Both tensor-core modes scale their operands by exact powers of two (per gathered
+    row group, per output channel), so their tolerance does not depend on the magnitude of features or weights.
+    weight_h16: what _pack_h16 returns, to save the conversion.  With gradients enabled the call must be epilogue-free and name its transposed table (a callable returning nbr_T [n_in, KV])."""
     if not features.is_cuda:
         raise L.SSTB200Error("sst_b200 spconv needs CUDA tensors (no CPU fallback)")
     if torch.is_grad_enabled() and (features.requires_grad or weight.requires_grad):
@@ -185,7 +220,7 @@ def fold_bn(bn, conv_bias=None):
     """eval-mode BatchNorm1d (+ the bias of the convolution in front of it) -> (scale, shift) fp32 [C]; cached on the module until a
     parameter / buffer changes (34 convolutions x 6 tiny torch kernels per U-Net forward otherwise)"""
     ts = (bn.running_mean, bn.running_var, bn.weight, bn.bias, conv_bias)
-    key = tuple((t._version, t.data_ptr()) for t in ts if t is not None)
+    key = tuple(_cache_key(t) for t in ts if t is not None)
     hit = getattr(bn, "_sstb200_fold", None)
     if hit is not None and hit[0] == key:
         return hit[1], hit[2]
@@ -342,9 +377,11 @@ class ToDense(SparseModule):
 # convolution layers
 # ------------------------------------------------------------------------------------------------------------------------
 class SparseConvolution(SparseModule):
-    """conv.py:45-206.  precision: 'fp32' (FFMA, exact path), 'bf16' (wgmma, 16-bit operands) or 'fp32_tc' (wgmma with split-fp16
-    operands: fp32 tolerance at tensor-core speed; channels % 64) - module attribute, also settable for a whole model with
-    set_spconv_precision()."""
+    """conv.py:45-206.  precision: 'fp32' (FFMA, exact path), 'bf16' (wgmma; the operands are IEEE fp16, 11 significant bits - 'bf16'
+    is the package-wide name of the 16-bit mode) or 'fp32_tc' (wgmma with split-fp16 operands: fp32 tolerance at tensor-core speed;
+    channels % 64) - module attribute, also settable for a whole model with set_spconv_precision().  The tensor-core modes carry
+    power-of-two exponents beside their fp16 operands, forward and backward, so features, weights and gradients of any magnitude
+    (1e-8 rows of a mean-reduced loss's gradient included) meet the same per-row tolerance as unit-scale ones."""
 
     def __init__(self, ndim, in_channels, out_channels, kernel_size=3, stride=1, padding=0, dilation=1, groups=1, bias=True, subm=False,
                  output_padding=0, transposed=False, inverse=False, indice_key=None, fused_bn=False):
@@ -382,16 +419,17 @@ class SparseConvolution(SparseModule):
                 self.bias.uniform_(-b, b)
 
     def _weight_h16(self):
-        key = (self.weight._version, self.weight.data_ptr(), self.precision)
+        key = _cache_key(self.weight) + (self.precision,)
         if self._h16 is None or self._h16[0] != key:
             kv = int(np.prod(self.kernel_size))
-            hi, lo = split_h16(self.weight.reshape(kv, self.in_channels, self.out_channels))
-            self._h16 = (key, hi if self.precision == "bf16" else torch.cat([hi, lo], 0))
+            self._h16 = (key, _pack_h16(self.weight.reshape(kv, self.in_channels, self.out_channels), self.precision))
         return self._h16[1]
 
     def _geometry(self, spatial_shape):
         nd = self.ndim
-        ks, st, pd = _triple(self.kernel_size, nd), _triple(self.stride, nd), _triple(self.padding, nd)
+        # a 2-D layer's z axis: kernel 1, stride 1, padding 0, so that outputs stay in the plane z = 0 - where the (b, y, x) rows a 2-D
+        # tensor carries are put back when the inverse layer builds its table
+        ks, st, pd = _triple(self.kernel_size, nd), _triple(self.stride, nd), _triple(self.padding, nd, 0)
         in_shape = _triple(spatial_shape, nd)
         if self.subm:   # spconv_ops.h:74-78: stride 1, padding k//2, whatever the layer says
             return in_shape, in_shape, ks, [1, 1, 1], [k // 2 for k in ks]
@@ -482,7 +520,7 @@ def build_conv_layer(cfg, *args, **kwargs):
 
 
 def set_spconv_precision(module, precision):
-    assert precision in PREC
+    assert precision in PREC, f"precision {precision!r}: 'fp32', 'bf16' (IEEE fp16 operands) or 'fp32_tc'"
     for m in module.modules():
         if isinstance(m, SparseConvolution):
             m.precision = precision

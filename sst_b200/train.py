@@ -145,6 +145,9 @@ class FlatAdamW:
                 self.flat[o:o + k].copy_(p.detach().reshape(-1))
                 p.data = self.flat[o:o + k].view_as(p)
                 p.grad = self.flat_grad[o:o + k].view_as(p)
+                # p keeps its own version counter, which no write through the buffer moves: caches derived from p (the 16-bit
+                # weight copies and folded BatchNorms of spconv_modules) also key on the buffer's
+                p._flat_base = self.flat
         self.lr, self.betas, self.eps, self.wd, self.t = lr, betas, eps, weight_decay, 0
 
     def zero_grad(self):
@@ -156,6 +159,8 @@ class FlatAdamW:
         L.check(c, L.lib().sstb200_adamw_step(c, self.flat.data_ptr(), self.flat_grad.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),
                                               self.flat.numel(), self.lr, self.betas[0], self.betas[1], self.eps, self.wd, self.t,
                                               float(grad_scale)))
+        # the kernel wrote through a raw pointer: tell torch, as an in-place torch op on the buffer would have
+        torch.autograd.graph.increment_version(self.flat)
 
 
 class TrainStep:

@@ -89,11 +89,9 @@ def main():
         # the input-resolution SubM convolution alone (64 -> 64), both paths
         nbr, _ = SP.conv_table(coors, coors, 1, shape, shape, [3, 3, 3], [1, 1, 1], [1, 1, 1])
         w = torch.randn((27, 64, 64), device=dev) * 0.02
-        w16 = w.permute(0, 2, 1).contiguous().half()
         pairs = int((nbr >= 0).sum())
-        hi, lo = SP.split_h16(w)
         for prec in ("fp32", "bf16", "fp32_tc"):
-            w16 = hi if prec != "fp32_tc" else torch.cat([hi, lo], 0)
+            w16 = SP._pack_h16(w, prec) if prec != "fp32" else None
             ms = timed(lambda: SP.indice_conv(feats, nbr, w, w16, precision=prec), a.reps * 3)
             res[f"subm64_{prec}"] = dict(us=ms * 1e3, pairs=pairs, tflops_pairs=2 * pairs * 64 * 64 / ms / 1e9,
                                          tflops_dense_tile=2 * coors.shape[0] * 27 * 64 * 64 / ms / 1e9,
