@@ -599,6 +599,28 @@ int sstb200_roiaware_pool3d_backward(sstb200_ctx* ctx, int num_pts, int channels
                                      const int32_t* voxel_offsets, const int32_t* point_idx, const int32_t* argmax,
                                      const int32_t* counts_dev, const float* grad_out, float* grad_in);
 
+/* ---- Deformable convolution: mmcv 1.3.8-1.4.0 deform_conv2d (DeformConv2d / DeformConv2dPack = 'DCN'), as CenterHead's DCNSeparateHead
+ * (mmdet3d/models/dense_heads/centerpoint_head.py:124-238) runs it.  fp32 only, FFMA.
+ * geom (15 int32) = N, Cin, H, W, Cout, kh, kw, stride h, stride w, pad h, pad w, dilation h, dilation w, groups, deform_groups.
+ * x [N, Cin, H, W], offset [N, 2 dg kh kw, Ho, Wo], weight [Cout, Cin / groups, kh, kw], y / grad_y [N, Cout, Ho, Wo], all contiguous fp32,
+ * Ho = (H + 2 ph - (dh (kh - 1) + 1)) / sh + 1 and the same for Wo.
+ * y[n, o, ho, wo] = sum over c in o's group and taps (i, j) of W[o, c mod Cin/groups, i, j] * S(n, c, p), with
+ *   p_h = (float)(ho sh - ph + i dh) + offset[n, 2K g + 2 (i kw + j), ho, wo],  p_w = (float)(wo sw - pw + j dw) + offset[.., + 1, ..],
+ *   g = c / (Cin / dg), K = kh kw; S = 0 unless -1 < p_h < H and -1 < p_w < W, else the bilinear blend of the corners floor(p) and
+ *   floor(p) + 1, a corner outside the image counting 0.  Zero offsets give a grouped conv2d.
+ * sstb200_dcn_forward: y fully written; temporaries (x transposed to NHWC) from the context arena.  No sync.
+ * sstb200_dcn_backward: grad_x = the transpose of the sampling, grad_offset = sum_c grad_col dS/dp with the corners held at floor(p) (the
+ *   forward difference at an integer p; 0 outside the open domain), grad_weight = sum over (n, ho, wo) of grad_y S.  Any of the three may be
+ *   NULL (not computed); the others are fully written.  Caller-owned workspace of sstb200_dcn_backward_workspace_bytes(geom) bytes; no
+ *   float atomics, so two calls give bit-identical results.  No sync.
+ * Errors: a size < 1, negative padding, Cin or Cout not divisible by groups, Cin not by dg, a kernel larger than the padded input
+ * (SSTB_ERR_ARG); 4 N dg K Ho Wo or N dg H W reaching 2^32, N > 65535 (SSTB_ERR_UNSUPPORTED); a short workspace (SSTB_ERR_WORKSPACE). */
+int sstb200_dcn_forward(sstb200_ctx* ctx, const int32_t geom[15], const float* x, const float* offset, const float* weight, float* y);
+int sstb200_dcn_backward_workspace_bytes(sstb200_ctx* ctx, const int32_t geom[15], int64_t* bytes);
+int sstb200_dcn_backward(sstb200_ctx* ctx, const int32_t geom[15], const float* x, const float* offset, const float* weight,
+                         const float* grad_y, void* workspace, int64_t workspace_bytes, float* grad_x, float* grad_offset,
+                         float* grad_weight);
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,6 +15,8 @@ and error behaviour; no CPU path - CPU tensors raise.
     box3d_multiclass_nms              core/post_processing/box3d_nms.py:10-143
     points_in_boxes_gpu, points_in_boxes_batch, RoIAwarePool3d
                                       ops/roiaware_pool3d                    (box membership, RoI-aware pooling)
+    deform_conv2d, DeformConv2dFunction
+                                      mmcv.ops.deform_conv (1.3.8-1.4.0)    (CenterHead's DCN)
 """
 import ctypes as C
 import math
@@ -949,3 +951,98 @@ class RoIAwarePool3d(nn.Module):
 
     def forward(self, rois, pts, pts_feature):
         return RoIAwarePool3dFunction.apply(rois, pts, pts_feature, self.out_size, self.max_pts_per_voxel, self.mode)
+
+
+# ----------------------------------------------------------------------------------------------
+# deformable convolution (mmcv.ops.deform_conv 1.3.8-1.4.0: deform_conv2d / DeformConv2dFunction)
+# ----------------------------------------------------------------------------------------------
+L.SIGNATURES["sstb200_dcn_forward"] = (C.c_int, [L.vp, L.P_i32, L.vp, L.vp, L.vp, L.vp])
+L.SIGNATURES["sstb200_dcn_backward_workspace_bytes"] = (C.c_int, [L.vp, L.P_i32, L.P_i64])
+L.SIGNATURES["sstb200_dcn_backward"] = (C.c_int, [L.vp, L.P_i32, L.vp, L.vp, L.vp, L.vp, L.vp, C.c_int64, L.vp, L.vp, L.vp])
+
+
+def _dcn_pair(v, name):
+    v = (v, v) if isinstance(v, int) else tuple(v)
+    if len(v) != 2 or not all(isinstance(i, int) for i in v):
+        raise L.SSTB200Error(f"deform_conv2d: {name} must be an int or a pair of ints, got {v!r}")
+    return v
+
+
+def _dcn_geom(input, offset, weight, stride, padding, dilation, groups, deform_groups):
+    """validated geom[15] of the C ABI for fp32 CUDA tensors of mmcv's shapes"""
+    for name, t in (("input", input), ("offset", offset), ("weight", weight)):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or t.dim() != 4:
+            raise L.SSTB200Error(f"deform_conv2d: {name} must be a 4-d float32 CUDA tensor (there is no CPU or fp16 path)")
+    (sh, sw), (ph, pw), (dh, dw) = _dcn_pair(stride, "stride"), _dcn_pair(padding, "padding"), _dcn_pair(dilation, "dilation")
+    N, Cin, H, W = input.shape
+    Cout, cg, kh, kw = weight.shape
+    if groups < 1 or deform_groups < 1 or Cin != cg * groups or Cout % groups or Cin % deform_groups:
+        raise L.SSTB200Error(f"deform_conv2d: input {tuple(input.shape)} / weight {tuple(weight.shape)} do not fit groups {groups} and "
+                             f"deform_groups {deform_groups}")
+    if min(sh, sw, dh, dw) < 1 or min(ph, pw) < 0:
+        raise L.SSTB200Error("deform_conv2d: stride and dilation must be >= 1, padding >= 0")
+    Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) // sh + 1
+    Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) // sw + 1
+    if Ho < 1 or Wo < 1 or tuple(offset.shape) != (N, 2 * deform_groups * kh * kw, Ho, Wo):
+        raise L.SSTB200Error(f"deform_conv2d: offset {tuple(offset.shape)} is not [N, 2 * deform_groups * kh * kw, Ho, Wo] = "
+                             f"{(N, 2 * deform_groups * kh * kw, Ho, Wo)}")
+    if not (input.device == offset.device == weight.device):
+        raise L.SSTB200Error("deform_conv2d: input, offset and weight must be on one device")
+    return L.arr(C.c_int32, [N, Cin, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, groups, deform_groups]), (N, Cout, Ho, Wo)
+
+
+class DeformConv2dFunction(Function):
+    """mmcv's DeformConv2dFunction.apply(input, offset, weight, stride, padding, dilation, groups, deform_groups, bias, im2col_step).
+    Backward re-samples (nothing beyond the inputs is saved) and is deterministic: no float atomics."""
+
+    @staticmethod
+    def forward(ctx, input, offset, weight, stride=1, padding=0, dilation=1, groups=1, deform_groups=1, bias=False, im2col_step=32):
+        if bias:
+            raise L.SSTB200Error("deform_conv2d: bias=True is not supported (as in mmcv's DeformConv2d)")
+        geom, out_shape = _dcn_geom(input, offset, weight, stride, padding, dilation, groups, deform_groups)
+        x, off, w = input.contiguous(), offset.contiguous(), weight.contiguous()
+        y = torch.empty(out_shape, dtype=torch.float32, device=x.device)
+        c = L.ctx(x.device)
+        L.check(c, L.lib().sstb200_dcn_forward(c, geom, L.ptr(x), L.ptr(off), L.ptr(w), L.ptr(y)))
+        ctx.save_for_backward(x, off, w)
+        ctx.geom = list(geom)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        x, off, w = ctx.saved_tensors
+        gx, goff, gw = deform_conv2d_backward(x, off, w, grad_y, ctx.geom, *ctx.needs_input_grad[:3])
+        return gx, goff, gw, None, None, None, None, None, None, None
+
+
+def deform_conv2d_backward(x, offset, weight, grad_y, geom, want_x=True, want_offset=True, want_weight=True):
+    """(grad_x, grad_offset, grad_weight); a gradient not wanted is None and is not computed"""
+    geom = L.arr(C.c_int32, list(geom))
+    gy = grad_y.contiguous()
+    gx = torch.empty_like(x) if want_x else None
+    goff = torch.empty_like(offset) if want_offset else None
+    gw = torch.empty_like(weight) if want_weight else None
+    if not (want_x or want_offset or want_weight):
+        return gx, goff, gw
+    c = L.ctx(x.device)
+    nbytes = C.c_int64()
+    L.check(c, L.lib().sstb200_dcn_backward_workspace_bytes(c, geom, C.byref(nbytes)))
+    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=x.device)
+    L.check(c, L.lib().sstb200_dcn_backward(c, geom, L.ptr(x), L.ptr(offset), L.ptr(weight), L.ptr(gy), L.ptr(ws), nbytes.value,
+                                            L.ptr(gx), L.ptr(goff), L.ptr(gw)))
+    return gx, goff, gw
+
+
+def deform_conv2d_workspace_bytes(input, offset, weight, stride=1, padding=0, dilation=1, groups=1, deform_groups=1):
+    """device bytes the backward of this call borrows (caller-owned workspace of sstb200_dcn_backward)"""
+    geom, _ = _dcn_geom(input, offset, weight, stride, padding, dilation, groups, deform_groups)
+    c = L.ctx(input.device)
+    nbytes = C.c_int64()
+    L.check(c, L.lib().sstb200_dcn_backward_workspace_bytes(c, geom, C.byref(nbytes)))
+    return nbytes.value
+
+
+def deform_conv2d(input, offset, weight, stride=1, padding=0, dilation=1, groups=1, deform_groups=1, bias=False, im2col_step=32):
+    """mmcv.ops.deform_conv2d: fp32 NCHW input [N, Cin, H, W], offset [N, 2 dg kh kw, Ho, Wo], weight [Cout, Cin / groups, kh, kw] ->
+    [N, Cout, Ho, Wo].  im2col_step is accepted and ignored (one launch covers the batch)."""
+    return DeformConv2dFunction.apply(input, offset, weight, stride, padding, dilation, groups, deform_groups, bias, im2col_step)
