@@ -212,8 +212,10 @@ int sstb200_linear(sstb200_ctx* ctx, const float* A, const float* W, const float
  * (mmdet3d/models/voxel_encoders/voxel_encoder.py:229-298 and :551-612; layers utils.py:107-144).
  * points [P,in_channels] fp32, coors [P,4] (b,z,y,x).  Output rows are the non-empty voxels sorted by
  * (b,z,y,x); capacity P.  drop_first_voxel_per_sample = 1 reproduces DynamicVFE's DynamicScatter behaviour
- * (scatter_points_cuda.cu:207-210 through the per-sample loop scatter_points.py:85-99); DynamicScatterVFE
- * (torch.unique based) keeps every voxel. */
+ * (scatter_points_cuda.cu:207-210 through the per-sample loop scatter_points.py:85-99): a sample loses its first
+ * voxel unless one of its points has a negative z, y or x (then the removed row is that point's (-1,-1,-1) row).
+ * Points with a negative or out-of-canvas coordinate belong to no voxel.  DynamicScatterVFE (torch.unique based)
+ * keeps every voxel. */
 typedef struct {
   int32_t in_channels;       /* raw point dims F (before decoration) */
   int32_t num_layers;        /* 1 or 2 */

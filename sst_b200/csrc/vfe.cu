@@ -35,29 +35,31 @@ __global__ void fold_bn_kernel(const float* __restrict__ w, const float* __restr
 }
 
 // rank -> output row with the reference's "first sorted row of every sample is removed" rule
-// (scatter_points_cuda.cu:207-210 applied per sample by scatter_points.py:85-99).
+// (scatter_points_cuda.cu:207-210 applied per sample by scatter_points.py:85-99).  The removed row is the sample's
+// (-1,-1,-1) row when one of its points has a negative coordinate, so only samples without such a point lose a real voxel.
 struct SampleQuirk {
   const uint32_t* word_prefix;
   size_t words_per_sample;
   int batch;
   int enabled;
+  const int32_t* has_invalid;  // [batch]: the sample has a point with a negative (z, y, x) coordinate
 };
+__device__ __forceinline__ bool quirk_drops(const SampleQuirk& q, int b) {
+  long long f0 = q.word_prefix[(size_t)b * q.words_per_sample], f1 = q.word_prefix[(size_t)(b + 1) * q.words_per_sample];
+  return f1 > f0 && !q.has_invalid[b];
+}
 __device__ __forceinline__ long long quirk_row(const SampleQuirk& q, long long rank, int b) {
   if (!q.enabled) return rank;
-  long long first_b = q.word_prefix[(size_t)b * q.words_per_sample];
-  if (rank == first_b) return -1;
+  if (quirk_drops(q, b) && rank == (long long)q.word_prefix[(size_t)b * q.words_per_sample]) return -1;
   int shift = 0;
-  for (int i = 0; i <= b; i++) {
-    long long f0 = q.word_prefix[(size_t)i * q.words_per_sample], f1 = q.word_prefix[(size_t)(i + 1) * q.words_per_sample];
-    shift += (f1 > f0);
-  }
+  for (int i = 0; i <= b; i++) shift += quirk_drops(q, i);
   return rank - shift;
 }
 
 template <typename TC, bool SM>
 __global__ void __launch_bounds__(SM ? 1024 : 256) vfe_mark_kernel(const TC* __restrict__ coors, int P, int B, int Z, int Y, int X, size_t cells_pad,
                                 long long* __restrict__ keys, uint32_t* __restrict__ bitmap, int32_t* __restrict__ flags,
-                                uint32_t nwords) {
+                                int32_t* __restrict__ sample_invalid, uint32_t nwords) {
   pdl_wait();
   pdl_launch();
   extern __shared__ uint32_t mark_sbm[];  // SM: block-private bitmap (see mark_rows_kernel in index.cuh)
@@ -71,6 +73,7 @@ __global__ void __launch_bounds__(SM ? 1024 : 256) vfe_mark_kernel(const TC* __r
     if (b < 0 || b >= B || z < 0 || z >= Z || y < 0 || y >= Y || x < 0 || x >= X) {
       keys[i] = -1;
       flags[0] = 1;
+      if (b >= 0 && b < B && (z < 0 || y < 0 || x < 0)) sample_invalid[b] = 1;  // the sample's (-1,-1,-1) row (SampleQuirk)
       continue;
     }
     long long key = b * (long long)cells_pad + (z * Y + y) * X + x;
@@ -111,8 +114,7 @@ __global__ void vfe_emit_kernel(const uint32_t* __restrict__ bitmap, const uint3
     long long t = *total;
     if (q.enabled) {
       int ne = 0;
-      for (int i = 0; i < q.batch; i++)
-        ne += q.word_prefix[(size_t)(i + 1) * q.words_per_sample] > q.word_prefix[(size_t)i * q.words_per_sample];
+      for (int i = 0; i < q.batch; i++) ne += quirk_drops(q, i);
       t -= ne;
     }
     *num_out = (int32_t)t;
@@ -405,16 +407,22 @@ __device__ __forceinline__ void tile_decorate(const VfeDev& v, const float* __re
   }
 }
 
-// column-wise segmented max over the tile's rows (rows sorted by voxel); tile [VT][ld] fp32 in smem.  blockDim.x / C row
-// groups work in parallel, each on VT / groups consecutive rows; a segment fully inside a group's rows is written with a
+// column-wise segmented max over the tile's rows (rows sorted by voxel); tile [VT][ld] fp32 in smem.  VFE_TILE_THREADS / C row
+// groups work in parallel, each on segmax_rows<C>() consecutive rows; a segment fully inside a group's rows is written with a
 // plain store, the first / last segment of a group may continue in a neighbouring group or tile -> integer atomicMax on the
-// float bits (values are >= 0 after ReLU; the rows concerned are zeroed beforehand by vfe_zero_edges_kernel).
-#define VSUB 32  // finest row-group granularity used by the kernels below
-__device__ __forceinline__ void tile_segmax(const float* tile, int ld, const int* sVox, int nrow, int C, float* __restrict__ out) {
-  const int groups = blockDim.x / C;
-  const int rows_per = VT / groups;
+// float bits (values are >= 0 after ReLU; the rows concerned are zeroed beforehand by vfe_zero_edges_kernel<TM, C>, which
+// walks the same row groups).
+#define VFE_TILE_THREADS 256  // block size of the tile kernels
+template <int C>
+__host__ __device__ constexpr int segmax_rows() {  // rows per row group of tile_segmax<C>: 16 for C = 32, 32 for 64, 64 for 128
+  static_assert(VFE_TILE_THREADS % C == 0 && VT % (VFE_TILE_THREADS / C) == 0, "tile_segmax: row groups must tile VT");
+  return VT / (VFE_TILE_THREADS / C);
+}
+template <int C>
+__device__ __forceinline__ void tile_segmax(const float* tile, int ld, const int* sVox, int nrow, float* __restrict__ out) {
+  constexpr int rows_per = segmax_rows<C>();
   const int c = threadIdx.x % C, grp = threadIdx.x / C;
-  if (grp >= groups) return;
+  if (grp >= VT / rows_per) return;
   const int r0 = grp * rows_per, r1 = min(r0 + rows_per, nrow);
   if (r0 >= r1) return;
   int seg = sVox[r0];
@@ -435,7 +443,7 @@ __device__ __forceinline__ void tile_segmax(const float* tile, int ld, const int
 }
 
 template <typename TC, typename TM, int C0>
-__global__ void __launch_bounds__(256) vfe_l0_tile_kernel(VfeDev v, const float* __restrict__ pts, const TC* __restrict__ coors,
+__global__ void __launch_bounds__(VFE_TILE_THREADS) vfe_l0_tile_kernel(VfeDev v, const float* __restrict__ pts, const TC* __restrict__ coors,
                                                           const uint32_t* __restrict__ offsets, const int32_t* __restrict__ order,
                                                           const TM* __restrict__ map, const int32_t* __restrict__ nvox_dev,
                                                           const float* __restrict__ vmean, float* __restrict__ vf0,
@@ -487,13 +495,13 @@ __global__ void __launch_bounds__(256) vfe_l0_tile_kernel(VfeDev v, const float*
       }
     }
     __syncthreads();
-    tile_segmax(sY, C0 + 1, sVox, nrow, C0, vf0);
+    tile_segmax<C0>(sY, C0 + 1, sVox, nrow, vf0);
   }
 }
 
 // layer 1 on tensor cores.  K = 2*C0 (== 128 for C0 = 64), N = C1 (128).
 template <typename TC, typename TM, int C0, int C1>
-__global__ void __launch_bounds__(256) vfe_l1_umma_kernel(VfeDev v, const float* __restrict__ pts, const TC* __restrict__ coors,
+__global__ void __launch_bounds__(VFE_TILE_THREADS) vfe_l1_umma_kernel(VfeDev v, const float* __restrict__ pts, const TC* __restrict__ coors,
                                                           const uint32_t* __restrict__ offsets, const int32_t* __restrict__ order,
                                                           const TM* __restrict__ map, const int32_t* __restrict__ nvox_dev,
                                                           const float* __restrict__ vmean, const float* __restrict__ vf0,
@@ -614,21 +622,22 @@ __global__ void __launch_bounds__(256) vfe_l1_umma_kernel(VfeDev v, const float*
       });
     }
     __syncthreads();
-    tile_segmax(sTile, C1 + 1, sVox, nrow, C1, vf1);
+    tile_segmax<C1>(sTile, C1 + 1, sVox, nrow, vf1);
   }
 }
 
 
-// rows of `out` that may be reached by atomicMax from two tiles (first / last voxel of every tile) start at 0
-template <typename TM>
+// rows of `out` that tile_segmax<C> reaches by atomicMax (first / last voxel of every row group of every tile) start at 0
+template <typename TM, int C>
 __global__ void vfe_zero_edges_kernel(const uint32_t* __restrict__ offsets, const int32_t* __restrict__ order,
-                                      const TM* __restrict__ map, const int32_t* __restrict__ nvox_dev, int C, float* __restrict__ out) {
+                                      const TM* __restrict__ map, const int32_t* __restrict__ nvox_dev, float* __restrict__ out) {
   pdl_wait();
   pdl_launch();
+  constexpr int R = segmax_rows<C>();
   const int M = *nvox_dev;
   const int nvalid = M > 0 ? (int)offsets[M] : 0;
-  for (int t = blockIdx.x; t * VSUB < nvalid; t += gridDim.x) {
-    int k0 = t * VSUB, k1 = min(k0 + VSUB, nvalid) - 1;
+  for (int t = blockIdx.x; t * R < nvalid; t += gridDim.x) {
+    int k0 = t * R, k1 = min(k0 + R, nvalid) - 1;
     int v0 = (int)map[order[k0]], v1 = (int)map[order[k1]];
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
       out[(size_t)v0 * C + c] = 0.f;
@@ -645,9 +654,9 @@ static int launch_vfe_tiles(sstb200_ctx* c, const VfeDev& v, const float* pts, c
   int grid = c->num_sms * 3;
   launch_pdl(vfe_mean_kernel, dim3(c->num_sms * 8), dim3(256), (size_t)(0), st, pts, v.F, r.offsets, r.order, num_dev, vmean);
   float* dst0 = (C1 > 0) ? vf0 : out;
-  launch_pdl(vfe_zero_edges_kernel<TM>, dim3(c->num_sms * 8), dim3(64), (size_t)(0), st, r.offsets, r.order, map, num_dev, C0, dst0);
+  launch_pdl(vfe_zero_edges_kernel<TM, C0>, dim3(c->num_sms * 8), dim3(64), (size_t)(0), st, r.offsets, r.order, map, num_dev, dst0);
   size_t smem0 = (size_t)VT * (C0 + 1) * 4;
-  launch_pdl(vfe_l0_tile_kernel<TC, TM, C0>, dim3(grid), dim3(256), (size_t)(smem0), st, v, pts, coors, r.offsets, r.order, map, num_dev, vmean, dst0,
+  launch_pdl(vfe_l0_tile_kernel<TC, TM, C0>, dim3(grid), dim3(VFE_TILE_THREADS), (size_t)(smem0), st, v, pts, coors, r.offsets, r.order, map, num_dev, vmean, dst0,
              (C1 > 0 && umma_l1) ? y0buf : (__nv_bfloat16*)nullptr);
   *l1_done = false;
   if (C1 > 0 && umma_l1) {
@@ -657,8 +666,8 @@ static int launch_vfe_tiles(sstb200_ctx* c, const VfeDev& v, const float* pts, c
     auto kern = vfe_l1_umma_kernel<TC, TM, C0, C1s>;
     static SmemAttr sa;
     CUDA_TRY(c, ensure_smem(c, sa, kern, smem1));
-    launch_pdl(vfe_zero_edges_kernel<TM>, dim3(c->num_sms * 8), dim3(64), (size_t)(0), st, r.offsets, r.order, map, num_dev, C1s, out);
-    launch_pdl(kern, dim3(grid), dim3(256), (size_t)(smem1), st, v, pts, coors, r.offsets, r.order, map, num_dev, vmean, vf0, out,
+    launch_pdl(vfe_zero_edges_kernel<TM, C1s>, dim3(c->num_sms * 8), dim3(64), (size_t)(0), st, r.offsets, r.order, map, num_dev, out);
+    launch_pdl(kern, dim3(grid), dim3(VFE_TILE_THREADS), (size_t)(smem1), st, v, pts, coors, r.offsets, r.order, map, num_dev, vmean, vf0, out,
                (const __nv_bfloat16*)y0buf);
     *l1_done = true;
   }
@@ -777,31 +786,32 @@ static int vfe_forward_impl(sstb200_ctx* c, const sstb200_vfe_cfg* cfg, const fl
   if (T > ((long long)1 << 34)) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "voxel grid too large for bitmap rank (%lld cells)", T);
   arena_reset(c);
   int rc = arena_reserve(c, key_index_bytes(P, T) + csr_bytes(P, P) + al256((size_t)P * 4) * 3 + al256((size_t)P * 3 * 4) +
-                                al256((size_t)P * C0 * 4) + al256((size_t)P * C0 * 2 + 128) + al256((size_t)(C0 + C1) * 8) + 8192 +
+                                al256((size_t)P * C0 * 4) + al256((size_t)P * C0 * 2 + 128) + al256((size_t)(C0 + C1) * 8) + al256((size_t)B * 4) + 8192 +
                                 (wide ? al256((size_t)P * D0 * 4) + 4 * al256((size_t)P * (C0 > C1 ? C0 : C1) * 4) + al256((size_t)P * 8) : 0));
   if (rc) return rc;
   KeyIndex k;
   rc = key_index_alloc(c, k, P, T);
   if (rc) return rc;
-  int32_t* count = arena_alloc<int32_t>(c, (size_t)P + 2);
+  int32_t* count = arena_alloc<int32_t>(c, (size_t)P + 2 + B);  // [P + 2] voxel point counts | [B] per-sample "has invalid" flags
   int32_t* map32 = inverse ? nullptr : arena_alloc<int32_t>(c, P);
   float* vmean = arena_alloc<float>(c, (size_t)P * 3);
   float* vf0 = arena_alloc<float>(c, (size_t)P * C0);
   float* fold = arena_alloc<float>(c, 2 * (size_t)(C0 + C1) + 8);
   __nv_bfloat16* y0buf = arena_alloc<__nv_bfloat16>(c, (size_t)P * C0 + 64);  // layer-0 point features (bf16, CSR order) for the tensor-core layer 1
   if (!count || !vmean || !vf0 || !fold || !y0buf) return sstb_fail(c, SSTB_ERR_WORKSPACE, "vfe: arena");
-  CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)P + 2) * 4, c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)P + 2 + B) * 4, c->stream));
+  int32_t* sample_invalid = count + P + 2;
   int nb = (P + 255) / 256;
   if (k.nwords <= 12 * 1024) {  // <= 48 KB: block-private bitmap
     int mg = (P + 1023) / 1024;
     if (mg > c->num_sms) mg = c->num_sms;
     launch_pdl(vfe_mark_kernel<TC, true>, dim3(mg), dim3(1024), k.nwords * 4, c->stream, coors, P, B, Z, Y, X, cells_pad, k.keys, k.bitmap, k.flags,
-               (uint32_t)k.nwords);
+               sample_invalid, (uint32_t)k.nwords);
   } else {
-    launch_pdl(vfe_mark_kernel<TC, false>, dim3(nb), dim3(256), (size_t)(0), c->stream, coors, P, B, Z, Y, X, cells_pad, k.keys, k.bitmap, k.flags, 0u);
+    launch_pdl(vfe_mark_kernel<TC, false>, dim3(nb), dim3(256), (size_t)(0), c->stream, coors, P, B, Z, Y, X, cells_pad, k.keys, k.bitmap, k.flags, sample_invalid, 0u);
   }
   key_index_scan(c, k);
-  SampleQuirk q{k.word_prefix, cells_pad / 32, B, cfg->drop_first_voxel_per_sample != 0};
+  SampleQuirk q{k.word_prefix, cells_pad / 32, B, cfg->drop_first_voxel_per_sample != 0, sample_invalid};
   int eg = (int)((k.nwords * 4 + 63) / 64);
   if (eg > c->num_sms * 32) eg = c->num_sms * 32;
   launch_pdl(vfe_emit_kernel<TC>, dim3(eg), dim3(64), (size_t)(0), c->stream, k.bitmap, k.word_prefix, k.nwords, cells_pad, Y, X, q, out_coors, k.total, num_dev);
