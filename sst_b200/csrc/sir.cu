@@ -410,6 +410,8 @@ extern "C" int sstb200_sir_layer_forward_ex(sstb200_ctx* c, const sstb200_sir_la
   float* gterm = arena_alloc<float>(c, (size_t)G * Cmax);
   if (!gord || !gterm) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
   if (bf16) {
+    // kernel B reads the pooled layer-0 features back from out_group as float4
+    CHECK_ARG(c, ((uintptr_t)out_group & 15) == 0);
     __nv_bfloat16* p0buf = arena_alloc<__nv_bfloat16>(c, ((size_t)N + 128) * 128);
     if (!p0buf) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
     rc = sstb_sir_layer_bf16(c, L, in_feats, f_cluster, (const long long*)inv, order, N, G, p0buf, gord, gterm, out_point, out_point_ld, out_group, in_ld, in_gap_at,

@@ -271,7 +271,8 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
       // epilogue rel3: LayerNorm over cin, act, gate with [xyz / normalizer || feats] -> x0 (bf16 A operand of layer 0)
       const int qb = quarter * NQC;
       const int nvalid = min(max(cin - qb, 0), NQC);  // warp-uniform: valid channels of this quarter
-      // columns >= cin are exactly 0 (zero weight rows), so plain sums work; the variance is corrected for them below
+      // columns >= cin are exactly 0 (zero weight rows), so the plain sum gives the mean; the variance sums the valid columns only
+      // (subtracting the pad columns' (KP - cin) mean^2 afterwards cancels when the channels share a large common part)
       float s = 0.f;
 #pragma unroll
       for (int i = 0; i < NQC; i++) s += v[i];
@@ -281,13 +282,12 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
       float q = 0.f;
 #pragma unroll
       for (int i = 0; i < NQC; i++) {
-        float t = v[i] - mean;
+        float t = i < nvalid ? v[i] - mean : 0.f;
         q = fmaf(t, t, q);
       }
       redB[quarter][lrow] = q;
       __syncthreads();
-      const float qsum = redB[0][lrow] + redB[1][lrow] + redB[2][lrow] + redB[3][lrow] - (float)(KP - cin) * mean * mean;
-      const float rstd = rsqrtf(fmaxf(qsum, 0.f) / (float)cin + d.eps);
+      const float rstd = rsqrtf((redB[0][lrow] + redB[1][lrow] + redB[2][lrow] + redB[3][lrow]) / (float)cin + d.eps);
       const float* frow = sIn + lrow * pitch_in;  // rows past the end hold stale data: their x0 / p0 rows are never used
 #pragma unroll
       for (int j = 0; j < NQC / 8; j++) {
@@ -370,7 +370,7 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
 template <int ACT>
 __global__ void __launch_bounds__(NT, 1) sir_b_kernel(SirDev d, const __nv_bfloat16* __restrict__ p0buf, const float* __restrict__ g0 /*[G, ldg]*/,
                                                       int ldg, const long long* __restrict__ inv, const int32_t* __restrict__ order, int N,
-                                                      float* __restrict__ out_point, int ldo, uint32_t* __restrict__ gord) {
+                                                      float* __restrict__ out_point, int ldo, bool vec_out, uint32_t* __restrict__ gord) {
   pdl_wait();
   pdl_launch();
   extern __shared__ uint8_t sirb_raw[];
@@ -471,7 +471,7 @@ __global__ void __launch_bounds__(NT, 1) sir_b_kernel(SirDev d, const __nv_bfloa
     warp_segmax_ord(v, sSeg[lrow], quarter * H, gord);
     if (lrow < nrow) {  // fp32 row segment (128 B) to the caller's buffer, original point order
       float* orow = out_point + (size_t)sRow[lrow] * ldo + quarter * H;
-      if ((ldo & 3) == 0) {
+      if (vec_out) {
 #pragma unroll
         for (int j = 0; j < H / 4; j++) reinterpret_cast<float4*>(orow)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
       } else {
@@ -530,6 +530,9 @@ int sstb_sir_layer_bf16(sstb200_ctx* c, const sstb200_sir_layer* L, const float*
   const int grid = ntiles < c->num_sms ? ntiles : c->num_sms;
   const size_t gn = (size_t)G * SC;
   const int Cg = 2 * SC;
+  // kernel B stores point rows as float4 only when every row segment is 16-byte aligned: a view such as buf[:, 1:129] of a buffer
+  // with 132 columns has ldo % 4 == 0 but a base 4 bytes off
+  const bool vec_out = ldo % 4 == 0 && (reinterpret_cast<uintptr_t>(out_point) & 15) == 0;
   CUDA_TRY(c, cudaMemsetAsync(gord, 0, gn * 4, st));
 #define SIR_A(KPV, ACTV)                                                                                                          \
   do {                                                                                                                            \
@@ -552,7 +555,7 @@ int sstb_sir_layer_bf16(sstb200_ctx* c, const sstb200_sir_layer* L, const float*
   do {                                                                                                                  \
     static SmemAttr sa;                                                                                                 \
     CUDA_TRY(c, ensure_smem(c, sa, sir_b_kernel<ACTV>, smemB));                                                         \
-    launch_pdl(sir_b_kernel<ACTV>, dim3(grid), dim3(NT), smemB, st, d, (const __nv_bfloat16*)p0buf, (const float*)out_group, Cg, inv, order, N, out_point, ldo, gord); \
+    launch_pdl(sir_b_kernel<ACTV>, dim3(grid), dim3(NT), smemB, st, d, (const __nv_bfloat16*)p0buf, (const float*)out_group, Cg, inv, order, N, out_point, ldo, vec_out, gord); \
   } while (0)
   if (L->act == 2) SIR_B(2);
   else SIR_B(1);
