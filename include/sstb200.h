@@ -616,7 +616,10 @@ int sstb200_roiaware_pool3d_backward(sstb200_ctx* ctx, int num_pts, int channels
  *   NULL (not computed); the others are fully written.  Caller-owned workspace of sstb200_dcn_backward_workspace_bytes(geom) bytes; no
  *   float atomics, so two calls give bit-identical results.  No sync.
  * Errors: a size < 1, negative padding, Cin or Cout not divisible by groups, Cin not by dg, a kernel larger than the padded input
- * (SSTB_ERR_ARG); 4 N dg K Ho Wo or N dg H W reaching 2^32, N > 65535 (SSTB_ERR_UNSUPPORTED); a short workspace (SSTB_ERR_WORKSPACE). */
+ * (SSTB_ERR_ARG); 4 N dg K Ho Wo reaching 2^32, N dg H W reaching 2^32 - 1, N > 65535, groups * ceil(Cin / groups * K / 16) or
+ * groups * ceil(Cout / groups / 16) above 65535 (SSTB_ERR_UNSUPPORTED); a short workspace (SSTB_ERR_WORKSPACE).  The backward and its
+ * workspace query sort the M = 4 N dg K Ho Wo sample corners with an int item count, so they also refuse M >= 2^31 (SSTB_ERR_UNSUPPORTED);
+ * the forward does not sort and keeps the 2^32 limit. */
 int sstb200_dcn_forward(sstb200_ctx* ctx, const int32_t geom[15], const float* x, const float* offset, const float* weight, float* y);
 int sstb200_dcn_backward_workspace_bytes(sstb200_ctx* ctx, const int32_t geom[15], int64_t* bytes);
 int sstb200_dcn_backward(sstb200_ctx* ctx, const int32_t geom[15], const float* x, const float* offset, const float* weight,

@@ -355,6 +355,16 @@ int dcn_geom(sstb200_ctx* c, const int32_t* a, DcnGeom& g) {
   return SSTB_OK;
 }
 
+// the backward sorts M = 4 N dg K Ho Wo (key, value) pairs, and cub's radix sort takes an int item count
+int dcn_bwd_geom(sstb200_ctx* c, const int32_t* a, DcnGeom& g) {
+  const int rc = dcn_geom(c, a, g);
+  if (rc) return rc;
+  const long long M = 4 * g.NP * g.D * g.K;
+  if (M > 0x7fffffffll)
+    return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "dcn_backward: %lld sample corners exceed the radix sort's 2^31 - 1 items", M);
+  return SSTB_OK;
+}
+
 int dcn_bn(int Og) { return Og <= 16 ? 16 : Og <= 32 ? 32 : 64; }
 
 cudaError_t launch_nhwc(cudaStream_t st, const float* in, int N, int C, long long HW, float* out) {
@@ -424,7 +434,7 @@ extern "C" int sstb200_dcn_forward(sstb200_ctx* c, const int32_t geom[15], const
 
 extern "C" int sstb200_dcn_backward_workspace_bytes(sstb200_ctx* c, const int32_t geom[15], int64_t* bytes) {
   DcnGeom g;
-  int rc = dcn_geom(c, geom, g);
+  int rc = dcn_bwd_geom(c, geom, g);
   if (rc) return rc;
   CHECK_ARG(c, bytes);
   *bytes = (int64_t)dcn_bwd_layout(g).total;
@@ -435,7 +445,7 @@ extern "C" int sstb200_dcn_backward(sstb200_ctx* c, const int32_t geom[15], cons
                                     const float* grad_y, void* workspace, int64_t workspace_bytes, float* grad_x, float* grad_offset,
                                     float* grad_weight) {
   DcnGeom g;
-  int rc = dcn_geom(c, geom, g);
+  int rc = dcn_bwd_geom(c, geom, g);
   if (rc) return rc;
   CHECK_ARG(c, x && offset && weight && grad_y && workspace);
   const DcnBwdLayout l = dcn_bwd_layout(g);
