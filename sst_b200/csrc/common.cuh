@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -179,6 +180,75 @@ __device__ __forceinline__ float ord2f(unsigned u) {
 }
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+
+// exact-form GELU (x * Phi(x)) with erf from Abramowitz-Stegun 7.1.26 (|err| <= 1.5e-7): ~12 instructions instead of
+// erff's ~30, same accuracy class as fp32 erff for an output that is rounded to bf16 anyway.
+__device__ __forceinline__ float gelu_fast(float x) {
+  const float z = fabsf(x) * 0.70710678118654752440f;
+  float t;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.3275911f, z, 1.0f)));  // MUFU.RCP (__frcp_rn is a ~25-instruction subroutine)
+  float p = fmaf(1.061405429f, t, -1.453152027f);
+  p = fmaf(p, t, 1.421413741f);
+  p = fmaf(p, t, -0.284496736f);
+  p = fmaf(p, t, 0.254829592f);
+  const float e = 1.0f - p * t * __expf(-z * z);   // erf(|x|/sqrt2)
+  return 0.5f * x * (1.0f + copysignf(e, x));
+}
+
+// exact-form GELU with one MUFU op and 9 ALU instructions, for epilogues where GELU dominates the instruction stream.
+// x Phi(x) = max(x, 0) - |x| Q(|x|), Q(a) = Phi(-a) the normal tail, and log2 Q(a) is smooth on [0, 6]: a degree-6 polynomial
+// (weighted minimax) holds it to 1.3e-7 of the GELU, max abs error 2.4e-7 over [-12, 12] (half an fp32 ulp of x where x ~ 4),
+// at most 0.2 fp16 ulp of the result.  Past |x| = 6 the tail term stays below 1.2e-8 (rounds to 0 in fp16) and is clamped there.
+// tests/test_gpu_sra_chain_epilogue.py mirrors this exact fp32 sequence.
+__device__ __forceinline__ float gelu_ex2(float x) {
+  const float a = fminf(fabsf(x), 6.0f);
+  float p = fmaf(3.50552036e-05f, a, -7.84027274e-04f);
+  p = fmaf(p, a, 8.12153984e-03f);
+  p = fmaf(p, a, -5.34629487e-02f);
+  p = fmaf(p, a, -4.58742619e-01f);
+  p = fmaf(p, a, -1.15120757e+00f);
+  p = fmaf(p, a, -9.99992907e-01f);   // log2 Q(a)
+  float q;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(q) : "f"(p));   // MUFU.EX2
+  return fmaf(-fabsf(x), q, fmaxf(x, 0.0f));
+}
+
+// d/dz [z Phi(z)] = Phi(z) + z phi(z)
+__device__ __forceinline__ float gelu_grad(float z) {
+  const float cdf = 0.5f * (1.0f + erff(z * 0.70710678118654752440f));
+  return cdf + z * 0.3989422804014327f * __expf(-0.5f * z * z);
+}
+
+// ---- 16-bit pairs --------------------------------------------------------------------------------------------------------------
+// Two fp32 values rounded to nearest into one 32-bit word, a in the low half.  FMT selects the 16-bit format of the pack_h16 /
+// unpack_h16 forms: IEEE fp16 or bf16.
+enum { FMT_F16 = 0, FMT_BF16 = 1 };
+__device__ __forceinline__ uint32_t pack_f16(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+template <int FMT>
+__device__ __forceinline__ uint32_t pack_h16(float a, float b) {
+  return FMT == FMT_BF16 ? pack_bf16(a, b) : pack_f16(a, b);
+}
+template <int FMT>
+__device__ __forceinline__ float2 unpack_h16(uint32_t u) {
+  if (FMT == FMT_BF16) return __bfloat1622float2(*reinterpret_cast<__nv_bfloat162*>(&u));
+  return __half22float2(*reinterpret_cast<__half2*>(&u));
+}
+// 8 consecutive fp32 values -> one 16-byte piece of 16-bit values
+template <int FMT>
+__device__ __forceinline__ int4 pack8_h16(const float* f) {
+  return make_int4((int)pack_h16<FMT>(f[0], f[1]), (int)pack_h16<FMT>(f[2], f[3]), (int)pack_h16<FMT>(f[4], f[5]), (int)pack_h16<FMT>(f[6], f[7]));
+}
+template <int FMT>
+__device__ __forceinline__ int4 pack8_h16(float4 a, float4 b) {
+  return make_int4((int)pack_h16<FMT>(a.x, a.y), (int)pack_h16<FMT>(a.z, a.w), (int)pack_h16<FMT>(b.x, b.y), (int)pack_h16<FMT>(b.z, b.w));
+}
 
 // ---- generic exclusive scan over uint32 values ----------------------------------------------
 // ONE launch, any length: single-pass chained scan with decoupled look-back.  Tiles of 256 threads x 8 items are

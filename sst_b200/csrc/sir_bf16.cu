@@ -14,7 +14,7 @@
 #include <stdarg.h>
 #include "index.cuh"
 #include "sra.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -41,7 +41,7 @@ __device__ __forceinline__ float gelu_as(float x) {
 template <int ACT>
 __device__ __forceinline__ float act_f(float x) { return ACT == 2 ? gelu_as(x) : fmaxf(x, 0.f); }
 
-// fp32 weight block W[r, col0 + k] (r < nrows, k < ncols) -> bf16 K-major SWIZZLE_128B operand of NR rows x KPAD columns
+// fp32 weight block W[r, col0 + k] (r < nrows, k < ncols) -> bf16 wgmma operand (wgmma.cuh) of NR rows x KPAD columns
 __device__ __forceinline__ void stage_weight(uint8_t* dst, int NR, int KPAD, const float* __restrict__ W, int ld, int col0, int nrows,
                                              int ncols) {
   const int pieces = NR * (KPAD / 8);
@@ -53,13 +53,7 @@ __device__ __forceinline__ void stage_weight(uint8_t* dst, int NR, int KPAD, con
       int k = j * 8 + i;
       f[i] = (r < nrows && k < ncols) ? __ldg(W + (size_t)r * ld + col0 + k) : 0.f;
     }
-    int4 q;
-    q.x = (int)pack_bf16(f[0], f[1]);
-    q.y = (int)pack_bf16(f[2], f[3]);
-    q.z = (int)pack_bf16(f[4], f[5]);
-    q.w = (int)pack_bf16(f[6], f[7]);
-    const int c = j >> 3, jj = j & 7;
-    *reinterpret_cast<int4*>(dst + (size_t)c * NR * 128 + r * 128 + ((jj ^ (r & 7)) << 4)) = q;
+    *reinterpret_cast<int4*>(dst + sw128_off(NR, r, j)) = pack8_h16<FMT_BF16>(f);
   }
 }
 
@@ -231,14 +225,9 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
 #pragma unroll
         for (int o = 0; o < 8; o++) h2[o] = alive ? act_f<ACT>((h2[o] - mean) * rstd * sG2[part * 8 + o] + sBt2[part * 8 + o]) : 0.f;
       }
-      int4 q4;
-      q4.x = (int)pack_bf16(h2[0], h2[1]);
-      q4.y = (int)pack_bf16(h2[2], h2[3]);
-      q4.z = (int)pack_bf16(h2[4], h2[5]);
-      q4.w = (int)pack_bf16(h2[6], h2[7]);
-      *reinterpret_cast<int4*>(sA3 + r * 128 + ((part ^ (r & 7)) << 4)) = q4;
+      *reinterpret_cast<int4*>(sA3 + sw128_off(ST, r, part)) = pack8_h16<FMT_BF16>(h2);
       // K columns R2..63 are zero (the previous tile's accumulators overwrote them)
-      *reinterpret_cast<int4*>(sA3 + r * 128 + (((part + 4) ^ (r & 7)) << 4)) = make_int4(0, 0, 0, 0);
+      *reinterpret_cast<int4*>(sA3 + sw128_off(ST, r, part + 4)) = make_int4(0, 0, 0, 0);
     }
     asm volatile("cp.async.wait_all;\n" ::: "memory");
     fence_async_smem();
@@ -306,14 +295,9 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
             }
             y[i] = o;
           }
-          pk.x = (int)pack_bf16(y[0], y[1]);
-          pk.y = (int)pack_bf16(y[2], y[3]);
-          pk.z = (int)pack_bf16(y[4], y[5]);
-          pk.w = (int)pack_bf16(y[6], y[7]);
+          pk = pack8_h16<FMT_BF16>(y);
         }
-        const int k8 = qb / 8 + j;
-        const int c = k8 >> 3, jj = k8 & 7;
-        *reinterpret_cast<int4*>(sA0 + (size_t)c * ST * 128 + lrow * 128 + ((jj ^ (lrow & 7)) << 4)) = pk;
+        *reinterpret_cast<int4*>(sA0 + sw128_off(ST, lrow, qb / 8 + j)) = pk;
       }
     }
     fence_async_smem();
@@ -346,14 +330,7 @@ __global__ void __launch_bounds__(NT, 1) sir_a_kernel(SirDev d, const float* __r
       if (lrow < nrow) {
         int4* dst = reinterpret_cast<int4*>(p0buf + (size_t)(k0 + lrow) * SC + quarter * H);
 #pragma unroll
-        for (int j = 0; j < H / 8; j++) {
-          int4 pk;
-          pk.x = (int)pack_bf16(v[j * 8 + 0], v[j * 8 + 1]);
-          pk.y = (int)pack_bf16(v[j * 8 + 2], v[j * 8 + 3]);
-          pk.z = (int)pack_bf16(v[j * 8 + 4], v[j * 8 + 5]);
-          pk.w = (int)pack_bf16(v[j * 8 + 6], v[j * 8 + 7]);
-          dst[j] = pk;
-        }
+        for (int j = 0; j < H / 8; j++) dst[j] = pack8_h16<FMT_BF16>(v + j * 8);
       }
     }
     if (tid < ST) {
@@ -410,12 +387,7 @@ __global__ void __launch_bounds__(NT, 1) sir_b_kernel(SirDev d, const __nv_bfloa
     }
     for (int idx = tid; idx < ST * (SC / 8); idx += NT) {
       int r = idx / (SC / 8), j = idx % (SC / 8);
-      int c = j >> 3, jj = j & 7;
-      uint8_t* dst = sA + (size_t)c * ST * 128 + r * 128 + ((jj ^ (r & 7)) << 4);
-      if (r < nrow)
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_u32(dst)), "l"(p0buf + (size_t)(k0 + r) * SC + j * 8) : "memory");
-      else
-        *reinterpret_cast<int4*>(dst) = make_int4(0, 0, 0, 0);
+      cp_async_piece_or_zero(sA + sw128_off(ST, r, j), p0buf + (size_t)(k0 + r) * SC + j * 8, r < nrow);
     }
     // second half of the K extent: the group's pooled layer-0 features (fp32 -> bf16), 4 pieces in flight per thread
     {
@@ -435,13 +407,7 @@ __global__ void __launch_bounds__(NT, 1) sir_b_kernel(SirDev d, const __nv_bfloa
       for (int u = 0; u < 4; u++) {
         int idx = tid + u * NT;
         int r = idx / (SC / 8), j = idx % (SC / 8) + SC / 8;
-        int4 q;
-        q.x = (int)pack_bf16(a[u].x, a[u].y);
-        q.y = (int)pack_bf16(a[u].z, a[u].w);
-        q.z = (int)pack_bf16(bq[u].x, bq[u].y);
-        q.w = (int)pack_bf16(bq[u].z, bq[u].w);
-        int c = j >> 3, jj = j & 7;
-        *reinterpret_cast<int4*>(sA + (size_t)c * ST * 128 + r * 128 + ((jj ^ (r & 7)) << 4)) = q;
+        *reinterpret_cast<int4*>(sA + sw128_off(ST, r, j)) = pack8_h16<FMT_BF16>(a[u], bq[u]);
       }
     }
     asm volatile("cp.async.wait_all;\n" ::: "memory");

@@ -12,7 +12,7 @@
 #include <stdarg.h>
 #include <cuda_fp16.h>
 #include "index.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include "sra.cuh"
 
 namespace {
@@ -307,7 +307,7 @@ __global__ void __launch_bounds__(256) spconv_dw_kernel(const float* __restrict_
 // ------------------------------------------------------------------------------------------------------------------------------
 // tensor-core implicit GEMM (precision 'bf16' = 16-bit operands, fp32 accumulation): 128-row output tile x NT output channels per
 // CTA, accumulators [128, NT] fp32 in registers across ALL kernel offsets (warpgroup g owns rows [64 g, 64 g + 64)), operands IEEE
-// fp16 in the K-major SWIZZLE_128B layout (same staging / descriptors as umma_gemm.cuh).  K is walked in stages of (kernel offset,
+// fp16 in the wgmma operand format (wgmma.cuh, staged as in wgmma_gemm.cuh).  K is walked in stages of (kernel offset,
 // 64 input channels): the 256 threads gather the 128 neighbour rows (fp32 -> fp16 on the fly, absent neighbours = zero rows that are
 // neither loaded nor converted) and the [NT, 64] weight slab into one of NS operand buffers, each warpgroup issues 4 wgmma (K = 16
 // each) as one commit group; the global loads run TWO stages ahead in two register sets (the deep levels of a U-Net are a few CTAs
@@ -394,7 +394,7 @@ struct SpStageRegs {
 // ones keep an absolute error of 2^-25 scaled = 2^-38 of that largest element, which is below the fp32 rounding of the sum they
 // are added to.
 template <int NT, int NS, bool SPLIT>
-__global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma_kernel(SpArgs g) {
+__global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_wgmma_kernel(SpArgs g) {
   pdl_wait();
   pdl_launch();
   extern __shared__ uint8_t sp_smem_raw[];
@@ -484,6 +484,8 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
 #pragma unroll
     for (int u = 0; u < 4; u++) {
       const int r = my_r + 32 * u;
+      // piece my_jj of row r in the operand format of wgmma.cuh, spelled out: through sw128_off this kernel needs more registers
+      // and spills
       const int off = r * 128 + ((my_jj ^ (r & 7)) << 4);
       int4 v = make_int4(0, 0, 0, 0), vl = make_int4(0, 0, 0, 0);
       if ((R.valid >> u) & 1u) {
@@ -569,8 +571,8 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_umma
 }
 
 template <int NT, int NS, bool SPLIT>
-static int launch_spconv_umma(sstb200_ctx* c, const SpArgs& g) {
-  auto kern = spconv_umma_kernel<NT, NS, SPLIT>;
+static int launch_spconv_wgmma(sstb200_ctx* c, const SpArgs& g) {
+  auto kern = spconv_wgmma_kernel<NT, NS, SPLIT>;
   static SmemAttr sa;
   const size_t smem = (size_t)NS * (SPLIT ? 2 : 1) * (SPU_A_BYTES + NT * 128) + 1024;
   CUDA_TRY(c, ensure_smem(c, sa, kern, smem));
@@ -580,15 +582,15 @@ static int launch_spconv_umma(sstb200_ctx* c, const SpArgs& g) {
   return SSTB_OK;
 }
 
-static int dispatch_spconv_umma(sstb200_ctx* c, const SpArgs& g, bool split) {
+static int dispatch_spconv_wgmma(sstb200_ctx* c, const SpArgs& g, bool split) {
   // 128 output channels per CTA at most: a warpgroup's [64, NT] fp32 accumulators take NT / 2 registers per thread, beside the
   // two register sets of staged operands
   if (split) {
-    if (g.Cout % 128 == 0) return launch_spconv_umma<128, 2, true>(c, g);
-    return launch_spconv_umma<64, 3, true>(c, g);
+    if (g.Cout % 128 == 0) return launch_spconv_wgmma<128, 2, true>(c, g);
+    return launch_spconv_wgmma<64, 3, true>(c, g);
   }
-  if (g.Cout % 128 == 0) return launch_spconv_umma<128, 3, false>(c, g);
-  return launch_spconv_umma<64, 3, false>(c, g);
+  if (g.Cout % 128 == 0) return launch_spconv_wgmma<128, 3, false>(c, g);
+  return launch_spconv_wgmma<64, 3, false>(c, g);
 }
 
 // W fp32 -> (hi, lo) fp16, elementwise
@@ -765,7 +767,7 @@ extern "C" int sstb200_spconv_forward(sstb200_ctx* c, const float* feats, int n_
   g.Whi = (const __half*)weight_h16;
   g.Wlo = g.Whi + (size_t)kernel_volume * c_out * c_in;   // FP32_TC: the residue copy follows the hi copy
   g.Cout = c_out, g.scale = scale, g.shift = shift, g.residual = residual, g.ldr = c_out, g.act = relu ? 1 : 0, g.out = out, g.ldo = c_out;
-  return dispatch_spconv_umma(c, g, precision == SSTB200_PREC_FP32_TC);
+  return dispatch_spconv_wgmma(c, g, precision == SSTB200_PREC_FP32_TC);
 }
 
 // fp32-tolerance row GEMM on the tensor core (used by the fp32 mode of the SRA encoder, csrc/sra_fp32.cu):
@@ -783,7 +785,7 @@ int sstb_gemm_rows_x3(sstb200_ctx* c, const float* A, int lda, const float* W, c
   g.rexp = nullptr, g.wun = nullptr;   // operands converted as they are: see sra.cuh for the range this leaves the caller
   g.feats = A, g.lda = lda, g.Cin = K, g.nbr = nullptr, g.n_out = M_cap, g.n_dev = M_dev, g.KV = 1, g.Whi = hi, g.Wlo = lo, g.Cout = N;
   g.scale = nullptr, g.shift = bias, g.residual = res, g.ldr = ldr, g.act = act, g.out = out, g.ldo = ldo;
-  return dispatch_spconv_umma(c, g, true);
+  return dispatch_spconv_wgmma(c, g, true);
 }
 
 extern "C" int sstb200_spconv_backward_weight(sstb200_ctx* c, const float* feats, int c_in, const int32_t* nbr, int n_out, int kernel_volume,

@@ -153,14 +153,6 @@ __device__ __forceinline__ void mma_f16_16816(float* c, const uint32_t* a, uint3
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__device__ __forceinline__ uint32_t pack2_f16(float a, float b) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ uint32_t pack2_bf16(float a, float b) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
 
 
 // ------------------------------------------------------------------------------------------------
@@ -427,14 +419,14 @@ static __global__ void __launch_bounds__(256, 3) win_attn_batch_kernel(const __h
       if (tok0 >= 0) {
         uint32_t* op0 = reinterpret_cast<uint32_t*>(out + (size_t)tok0 * D + (hs * NHL + hl) * DH);
         const float i0 = __fdividef(1.0f, l0);
-        op0[t4] = (OUT_BF16 ? pack2_bf16 : pack2_f16)(o[0][0] * i0, o[0][1] * i0);
-        op0[t4 + 4] = (OUT_BF16 ? pack2_bf16 : pack2_f16)(o[1][0] * i0, o[1][1] * i0);
+        op0[t4] = (OUT_BF16 ? pack_bf16 : pack_f16)(o[0][0] * i0, o[0][1] * i0);
+        op0[t4 + 4] = (OUT_BF16 ? pack_bf16 : pack_f16)(o[1][0] * i0, o[1][1] * i0);
       }
       if (tok1 >= 0) {
         uint32_t* op1 = reinterpret_cast<uint32_t*>(out + (size_t)tok1 * D + (hs * NHL + hl) * DH);
         const float i1 = __fdividef(1.0f, l1);
-        op1[t4] = (OUT_BF16 ? pack2_bf16 : pack2_f16)(o[0][2] * i1, o[0][3] * i1);
-        op1[t4 + 4] = (OUT_BF16 ? pack2_bf16 : pack2_f16)(o[1][2] * i1, o[1][3] * i1);
+        op1[t4] = (OUT_BF16 ? pack_bf16 : pack_f16)(o[0][2] * i1, o[0][3] * i1);
+        op1[t4 + 4] = (OUT_BF16 ? pack_bf16 : pack_f16)(o[1][2] * i1, o[1][3] * i1);
       }
     }
   }

@@ -2,7 +2,7 @@
 // throughput, 8x smaller operand rounding than bf16, and the reference's own mixed-precision setting is fp16,
 // configs/sst_refactor/sst_waymoD5_1x_3class_8heads_v2.py:82): wgmma GEMMs with fp32 accumulators.
 //
-// Per layer: the QKV projection (generic GEMM kernel of csrc/umma_gemm.cuh: C[128-row tile, NT] = A[128, K] . W[NT, K]^T,
+// Per layer: the QKV projection (generic GEMM kernel of csrc/wgmma_gemm.cuh: C[128-row tile, NT] = A[128, K] . W[NT, K]^T,
 // A converted on the fly from fp32 rows + positional embedding, fp16 q|k|v out), the ragged window attention, and the fused
 // post-attention chain of csrc/sra_chain2.cu (out-projection + LN1 + FFN + LN2, in the encoder stack also the next layer's
 // QKV), so the stack takes 2 launches per layer.  fp32 stays the type of the residual stream, softmax, LayerNorm and all
@@ -11,8 +11,8 @@
 #include <cuda_fp16.h>
 #include "sra.cuh"
 #include "sra_attn.cuh"
-#include "umma.cuh"
-#include "umma_gemm.cuh"
+#include "wgmma.cuh"
+#include "wgmma_gemm.cuh"
 
 namespace {
 
@@ -37,7 +37,7 @@ int qkv_gemm(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb200_sra_plan*
   g.out_h16 = qkv;
   g.ldo = 3 * d;
   g.out_row_map = nullptr;  // q|k|v, att and the residual stream all live in flat token order; attention gathers its windows
-  return f16_out ? launch_umma<128, 128, PRO_F32, EPI_F16>(c, g, 3) : launch_umma<128, 128, PRO_F32, EPI_H16>(c, g, 3);
+  return f16_out ? launch_wgmma_gemm<128, 128, PRO_F32, EPI_F16>(c, g, 3) : launch_wgmma_gemm<128, 128, PRO_F32, EPI_H16>(c, g, 3);
 }
 
 }  // namespace

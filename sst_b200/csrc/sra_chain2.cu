@@ -30,7 +30,6 @@
 #include <cuda_fp16.h>
 #include "sra.cuh"
 #include "tma.cuh"
-#include "umma_gemm.cuh"
 
 namespace {
 
@@ -78,7 +77,9 @@ __device__ __forceinline__ void issue_chunk(const Chain2Maps& m, int j, uint32_t
   tma_load_2d(dst + SLOT / 2, map, k0 + 64, n0, bar);
 }
 
-// 16-bit pair (columns k, k + 1) of row `row` into a 64-row K-major SWIZZLE_128B operand
+// 16-bit pair (columns k, k + 1) of row `row` into a 64-row wgmma operand (format in wgmma.cuh).  The address is spelled out
+// rather than taken from sw128_off: with k = 128 h + c (GEMM2's epilogue) only the masked form (k & 63) >> 3 lets the compiler
+// fold the piece index; sw128_off's (k >> 3) & 7 costs the kernel ~100 more instructions.
 __device__ __forceinline__ void st_op(uint32_t buf, int row, int k, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(buf + (k >> 6) * OPH + row * 128 + ((((k & 63) >> 3) ^ (row & 7)) << 4) + (k & 7) * 2), "r"(v) : "memory");
 }

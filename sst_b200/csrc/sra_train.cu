@@ -8,7 +8,7 @@
 // operands and saved activations are bf16 (gradients need the fp32 exponent range, so no loss scaling), accumulation, softmax,
 // LayerNorm, residual stream, weight gradients and the optimizer state are fp32.
 //
-// Per layer, forward:   qkv = [x+pos | x] Wqkv^T        wgmma GEMM (csrc/umma_gemm.cuh)  , q|k|v fp16 for the attention kernel
+// Per layer, forward:   qkv = [x+pos | x] Wqkv^T        wgmma GEMM (csrc/wgmma_gemm.cuh) , q|k|v fp16 for the attention kernel
 //                       att = windowed softmax(q k^T) v  csrc/sra_attn.cuh (bf16 output; plain or cosine logits)
 //                       x1 = LN1(x + att Wo^T + bo)      wgmma GEMM + LN epilogue, keeps t1   = pre-LN sum
 //                       h  = GELU(z), z = x1 W1^T + b1   wgmma GEMM, keeps z  
@@ -20,8 +20,8 @@
 #include <cuda_fp16.h>
 #include "sra.cuh"
 #include "sra_attn.cuh"
-#include "umma.cuh"
-#include "umma_gemm.cuh"
+#include "wgmma.cuh"
+#include "wgmma_gemm.cuh"
 
 namespace {
 
@@ -251,8 +251,7 @@ __global__ void __launch_bounds__(256) dw_gemm_kernel(DwArgs g) {
               }
             }
           }
-          *reinterpret_cast<int4*>(sX + (buf * DW_ROWS + r) * DW_PITCH + pc * 8) =
-              make_int4((int)pack_bf16(f[0], f[1]), (int)pack_bf16(f[2], f[3]), (int)pack_bf16(f[4], f[5]), (int)pack_bf16(f[6], f[7]));
+          *reinterpret_cast<int4*>(sX + (buf * DW_ROWS + r) * DW_PITCH + pc * 8) = pack8_h16<FMT_BF16>(f);
         }
       }
       asm volatile("cp.async.commit_group;\n" ::: "memory");
@@ -772,7 +771,7 @@ extern "C" int sstb200_sra_stack_forward_train(sstb200_ctx* c, const sstb200_sra
     g.M_cap = n, g.A = xin, g.lda = DM, g.W = L->in_proj_w_f16, g.bias = L->in_proj_b;
     g.pos_tab = P->pos_table, g.pos_code = P->pos_code, g.posL = P->pos_L, g.pos_maxw = P->pos_maxw, g.pos_ndim = P->pos_ndim, g.pos_ntiles = 2;
     g.out_h16 = lw + w.qkv, g.ldo = 3 * DM;
-    if ((rc = launch_umma<128, 128, PRO_F32, EPI_F16, FMT_BF16>(c, g, 3))) return rc;
+    if ((rc = launch_wgmma_gemm<128, 128, PRO_F32, EPI_F16, FMT_BF16>(c, g, 3))) return rc;
     // 2. attention (bf16 output)
     if ((rc = sstb_win_attn_batch(c, reinterpret_cast<const __half*>(lw + w.qkv), P->num_windows_dev, P->win_offsets, P->win_batch, n, P->tok_perm,
                                   lw + w.att, /*out_bf16=*/true, L->tau, L->tau_n, L->tau_min)))
@@ -781,16 +780,16 @@ extern "C" int sstb200_sra_stack_forward_train(sstb200_ctx* c, const sstb200_sra
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = lw + w.att, g.lda = DM, g.W = L->out_proj_w_f16, g.bias = L->out_proj_b, g.res = xin, g.gamma = L->norm1_w, g.beta = L->norm1_b;
     g.eps = L->norm_eps, g.out_f32 = reinterpret_cast<float*>(lw + w.x1), g.out_h16 = lw + w.x1b, g.ldo = DM, g.out_pre = reinterpret_cast<float*>(lw + w.t1);
-    if ((rc = launch_umma<128, 128, PRO_H16, EPI_RES_LN, FMT_BF16>(c, g, 1))) return rc;
+    if ((rc = launch_wgmma_gemm<128, 128, PRO_H16, EPI_RES_LN, FMT_BF16>(c, g, 1))) return rc;
     // 4. h = GELU(z), z = x1 W1^T + b1
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = lw + w.x1b, g.lda = DM, g.W = L->lin1_w_f16, g.bias = L->lin1_b, g.out_h16 = lw + w.h, g.out_pre16 = lw + w.z, g.ldo = DFF;
-    if ((rc = launch_umma<128, 128, PRO_H16, EPI_H16_GELU, FMT_BF16>(c, g, 2))) return rc;
+    if ((rc = launch_wgmma_gemm<128, 128, PRO_H16, EPI_H16_GELU, FMT_BF16>(c, g, 2))) return rc;
     // 5. y = LN2(x1 + h W2^T + b2), keep t2
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = lw + w.h, g.lda = DFF, g.W = L->lin2_w_f16, g.bias = L->lin2_b, g.res = reinterpret_cast<float*>(lw + w.x1), g.gamma = L->norm2_w;
     g.beta = L->norm2_b, g.eps = L->norm_eps, g.out_f32 = y, g.out_pre = reinterpret_cast<float*>(lw + w.t2);
-    if ((rc = launch_umma<256, 128, PRO_H16, EPI_RES_LN, FMT_BF16>(c, g, 1))) return rc;
+    if ((rc = launch_wgmma_gemm<256, 128, PRO_H16, EPI_RES_LN, FMT_BF16>(c, g, 1))) return rc;
     xin = y;
   }
   return SSTB_OK;
@@ -835,13 +834,13 @@ extern "C" int sstb200_sra_stack_backward(sstb200_ctx* c, const sstb200_sra_laye
     // dz = (dt2 W2) * gelu'(z)
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = dtb, g.lda = DM, g.W = T->lin2_wt, g.out_h16 = dzb, g.aux16 = lw + w.z, g.ldo = DFF;
-    if ((rc = launch_umma<128, 128, PRO_H16, EPI_GELUGRAD, FMT_BF16>(c, g, 2))) return rc;
+    if ((rc = launch_wgmma_gemm<128, 128, PRO_H16, EPI_GELUGRAD, FMT_BF16>(c, g, 2))) return rc;
     // dW1 += dz^T x1, d b1 += colsum(dz)
     if ((rc = launch_dw(c, dzb, DFF, DFF, reinterpret_cast<const __nv_bfloat16*>(lw + w.x1b), nullptr, DM, DM, nullptr, G->lin1_w, n, G->lin1_b))) return rc;
     // dx1 = dt2 + dz W1
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = dzb, g.lda = DFF, g.W = T->lin1_wt, g.res = dt, g.out_f32 = dx1;
-    if ((rc = launch_umma<256, 128, PRO_H16, EPI_ADD_F32, FMT_BF16>(c, g, 1))) return rc;
+    if ((rc = launch_wgmma_gemm<256, 128, PRO_H16, EPI_ADD_F32, FMT_BF16>(c, g, 1))) return rc;
     // LN1': dt1, d gamma1, d beta1, d bo
     if ((rc = launch_ln_bwd(c, dx1, reinterpret_cast<const float*>(lw + w.t1), L->norm1_w, L->norm_eps, n, dt, dtb, G->norm1_w, G->norm1_b,
                             G->out_proj_b)))
@@ -850,7 +849,7 @@ extern "C" int sstb200_sra_stack_backward(sstb200_ctx* c, const sstb200_sra_laye
     if ((rc = launch_dw(c, dtb, DM, DM, reinterpret_cast<const __nv_bfloat16*>(lw + w.att), nullptr, DM, DM, nullptr, G->out_proj_w, n))) return rc;
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = dtb, g.lda = DM, g.W = T->out_proj_wt, g.bias = nullptr, g.out_h16 = dattb, g.ldo = DM;
-    if ((rc = launch_umma<128, 128, PRO_H16, EPI_H16, FMT_BF16>(c, g, 1))) return rc;
+    if ((rc = launch_wgmma_gemm<128, 128, PRO_H16, EPI_H16, FMT_BF16>(c, g, 1))) return rc;
     // attention'
     if ((rc = launch_attn_bwd(c, reinterpret_cast<const __half*>(lw + w.qkv), reinterpret_cast<const __nv_bfloat16*>(lw + w.att), dattb, P, L, G->tau,
                               dqkv)))
@@ -862,7 +861,7 @@ extern "C" int sstb200_sra_stack_backward(sstb200_ctx* c, const sstb200_sra_laye
     // dx = dt1 + dqkv Wqkv
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = dqkv, g.lda = 3 * DM, g.W = T->in_proj_wt, g.res = dt, g.out_f32 = dxo;
-    if ((rc = launch_umma<384, 128, PRO_H16, EPI_ADD_F32, FMT_BF16>(c, g, 1))) return rc;
+    if ((rc = launch_wgmma_gemm<384, 128, PRO_H16, EPI_ADD_F32, FMT_BF16>(c, g, 1))) return rc;
     dcur = dxo;
   }
   return SSTB_OK;

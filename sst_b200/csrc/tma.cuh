@@ -5,7 +5,7 @@
 // instructions on address arithmetic for operand staging.
 #pragma once
 #include <cuda.h>
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 

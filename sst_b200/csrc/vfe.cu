@@ -8,7 +8,7 @@
 #include <stdarg.h>
 #include "index.cuh"
 #include "sra.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 struct VfeDev {
   int F, D0, C0, C1, nlayers;
@@ -335,7 +335,7 @@ __global__ void __launch_bounds__(256) vfe_fused_kernel(VfeDev v, const float* _
 // Tile path (max pooling): points are visited in CSR (voxel-sorted) order in tiles of 128.
 //   vfe_mean_kernel     per-voxel xyz mean (4 lanes per voxel, fp64 accumulate)
 //   vfe_l0_tile_kernel  decorate + layer 0 (FFMA, fp32 exact) + in-tile segmented max -> vf0 [M,C0]
-//   vfe_l1_umma_kernel  A = bf16([y0 || vf0[voxel]]) [128 x 2*C0], B = bf16(W1) -> wgmma (two warpgroups of 64 rows),
+//   vfe_l1_wgmma_kernel A = bf16([y0 || vf0[voxel]]) [128 x 2*C0], B = bf16(W1) -> wgmma (two warpgroups of 64 rows),
 //                       epilogue BN+ReLU from the accumulator fragments into an smem tile, in-tile segmented max -> vf1 [M,C1]
 // Post-ReLU values are >= 0, so the max across tile edges is an integer atomicMax on the float bits
 // (exact, order independent); segments interior to a tile are written with plain stores.
@@ -501,7 +501,7 @@ __global__ void __launch_bounds__(VFE_TILE_THREADS) vfe_l0_tile_kernel(VfeDev v,
 
 // layer 1 on tensor cores.  K = 2*C0 (== 128 for C0 = 64), N = C1 (128).
 template <typename TC, typename TM, int C0, int C1>
-__global__ void __launch_bounds__(VFE_TILE_THREADS) vfe_l1_umma_kernel(VfeDev v, const float* __restrict__ pts, const TC* __restrict__ coors,
+__global__ void __launch_bounds__(VFE_TILE_THREADS) vfe_l1_wgmma_kernel(VfeDev v, const float* __restrict__ pts, const TC* __restrict__ coors,
                                                           const uint32_t* __restrict__ offsets, const int32_t* __restrict__ order,
                                                           const TM* __restrict__ map, const int32_t* __restrict__ nvox_dev,
                                                           const float* __restrict__ vmean, const float* __restrict__ vf0,
@@ -533,7 +533,7 @@ __global__ void __launch_bounds__(VFE_TILE_THREADS) vfe_l1_umma_kernel(VfeDev v,
     sS1[i] = v.s1[i];
     sT1[i] = v.t1[i];
   }
-  // B operand: W1 [C1, K] fp32 -> bf16, K-major SWIZZLE_128B, once per CTA (4 pieces in flight per thread)
+  // B operand: W1 [C1, K] fp32 -> bf16 wgmma operand, once per CTA (4 pieces in flight per thread)
   for (int i0 = tid; i0 < C1 * (K / 8); i0 += blockDim.x * 4) {
     float4 f0[4], f1[4];
 #pragma unroll
@@ -550,13 +550,7 @@ __global__ void __launch_bounds__(VFE_TILE_THREADS) vfe_l1_umma_kernel(VfeDev v,
       int idx = i0 + u * blockDim.x;
       if (idx < C1 * (K / 8)) {
         int r = idx / (K / 8), j = idx % (K / 8);
-        int4 q;
-        q.x = (int)pack_bf16(f0[u].x, f0[u].y);
-        q.y = (int)pack_bf16(f0[u].z, f0[u].w);
-        q.z = (int)pack_bf16(f1[u].x, f1[u].y);
-        q.w = (int)pack_bf16(f1[u].z, f1[u].w);
-        int c = j >> 3, jj = j & 7;
-        *reinterpret_cast<int4*>(sB + (size_t)c * C1 * 128 + r * 128 + ((jj ^ (r & 7)) << 4)) = q;
+        *reinterpret_cast<int4*>(sB + sw128_off(C1, r, j)) = pack8_h16<FMT_BF16>(f0[u], f1[u]);
       }
     }
   }
@@ -569,13 +563,7 @@ __global__ void __launch_bounds__(VFE_TILE_THREADS) vfe_l1_umma_kernel(VfeDev v,
     // kernel: plain cp.async into the swizzled operand; (2) the voxel's layer-0 max is gathered 4 rows in flight
     for (int idx = tid; idx < VT * (C0 / 8); idx += blockDim.x) {
       int r = idx / (C0 / 8), j = idx % (C0 / 8);
-      int c = j >> 3, jj = j & 7;
-      uint8_t* dst = sA + (size_t)c * VT * 128 + r * 128 + ((jj ^ (r & 7)) << 4);
-      if (r < nrow) {
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_u32(dst)), "l"(y0buf + (size_t)(k0 + r) * C0 + j * 8) : "memory");
-      } else {
-        *reinterpret_cast<int4*>(dst) = make_int4(0, 0, 0, 0);
-      }
+      cp_async_piece_or_zero(sA + sw128_off(VT, r, j), y0buf + (size_t)(k0 + r) * C0 + j * 8, r < nrow);
     }
     for (int i0 = tid; i0 < VT * (C0 / 8); i0 += blockDim.x * 4) {
       float4 g0[4], g1[4];
@@ -595,13 +583,7 @@ __global__ void __launch_bounds__(VFE_TILE_THREADS) vfe_l1_umma_kernel(VfeDev v,
         int idx = i0 + u * blockDim.x;
         if (idx < VT * (C0 / 8)) {
           int r = idx / (C0 / 8), j = idx % (C0 / 8) + C0 / 8;
-          int4 q;
-          q.x = (int)pack_bf16(g0[u].x, g0[u].y);
-          q.y = (int)pack_bf16(g0[u].z, g0[u].w);
-          q.z = (int)pack_bf16(g1[u].x, g1[u].y);
-          q.w = (int)pack_bf16(g1[u].z, g1[u].w);
-          int c = j >> 3, jj = j & 7;
-          *reinterpret_cast<int4*>(sA + (size_t)c * VT * 128 + r * 128 + ((jj ^ (r & 7)) << 4)) = q;
+          *reinterpret_cast<int4*>(sA + sw128_off(VT, r, j)) = pack8_h16<FMT_BF16>(g0[u], g1[u]);
         }
       }
     }
@@ -648,7 +630,7 @@ __global__ void vfe_zero_edges_kernel(const uint32_t* __restrict__ offsets, cons
 
 template <typename TC, typename TM, int C0, int C1>
 static int launch_vfe_tiles(sstb200_ctx* c, const VfeDev& v, const float* pts, const TC* coors, const Csr& r, const TM* map,
-                            const int32_t* num_dev, float* vmean, float* vf0, float* out, bool umma_l1, bool* l1_done,
+                            const int32_t* num_dev, float* vmean, float* vf0, float* out, bool wgmma_l1, bool* l1_done,
                             __nv_bfloat16* y0buf) {
   cudaStream_t st = c->stream;
   int grid = c->num_sms * 3;
@@ -657,13 +639,13 @@ static int launch_vfe_tiles(sstb200_ctx* c, const VfeDev& v, const float* pts, c
   launch_pdl(vfe_zero_edges_kernel<TM, C0>, dim3(c->num_sms * 8), dim3(64), (size_t)(0), st, r.offsets, r.order, map, num_dev, dst0);
   size_t smem0 = (size_t)VT * (C0 + 1) * 4;
   launch_pdl(vfe_l0_tile_kernel<TC, TM, C0>, dim3(grid), dim3(VFE_TILE_THREADS), (size_t)(smem0), st, v, pts, coors, r.offsets, r.order, map, num_dev, vmean, dst0,
-             (C1 > 0 && umma_l1) ? y0buf : (__nv_bfloat16*)nullptr);
+             (C1 > 0 && wgmma_l1) ? y0buf : (__nv_bfloat16*)nullptr);
   *l1_done = false;
-  if (C1 > 0 && umma_l1) {
+  if (C1 > 0 && wgmma_l1) {
     constexpr int C1s = C1 > 0 ? C1 : 32;
     size_t opA = (size_t)VT * 2 * C0 * 2, opB = (size_t)C1s * 2 * C0 * 2, tile = (size_t)VT * (C1s + 1) * 4;
     size_t smem1 = opB + (opA > tile ? opA : tile) + 1024;
-    auto kern = vfe_l1_umma_kernel<TC, TM, C0, C1s>;
+    auto kern = vfe_l1_wgmma_kernel<TC, TM, C0, C1s>;
     static SmemAttr sa;
     CUDA_TRY(c, ensure_smem(c, sa, kern, smem1));
     launch_pdl(vfe_zero_edges_kernel<TM, C1s>, dim3(c->num_sms * 8), dim3(64), (size_t)(0), st, r.offsets, r.order, map, num_dev, out);
@@ -864,11 +846,11 @@ static int vfe_forward_impl(sstb200_ctx* c, const sstb200_vfe_cfg* cfg, const fl
   {
     // tile path (max pooling, the configurations on the hot path): layer 0 FFMA tiles; layer 1 on the tensor cores (wgmma) when bf16
     bool l1_done = false, tiled = false;
-    const bool umma = cfg->precision == SSTB200_PREC_BF16;
+    const bool wgmma = cfg->precision == SSTB200_PREC_BF16;
 #define VFE_TILE(a, b)                                                                                                          \
   if (!tiled && v.mode_max && C0 == a && C1 == b) {                                                                             \
-    if (inverse) rc = launch_vfe_tiles<TC, TC, a, b>(c, v, pts, coors, r, inverse, num_dev, vmean, vf0, out_feats, umma, &l1_done, y0buf); \
-    else rc = launch_vfe_tiles<TC, int32_t, a, b>(c, v, pts, coors, r, map32, num_dev, vmean, vf0, out_feats, umma, &l1_done, y0buf);    \
+    if (inverse) rc = launch_vfe_tiles<TC, TC, a, b>(c, v, pts, coors, r, inverse, num_dev, vmean, vf0, out_feats, wgmma, &l1_done, y0buf); \
+    else rc = launch_vfe_tiles<TC, int32_t, a, b>(c, v, pts, coors, r, map32, num_dev, vmean, vf0, out_feats, wgmma, &l1_done, y0buf);    \
     if (rc) return rc;                                                                                                          \
     tiled = true;                                                                                                               \
   }

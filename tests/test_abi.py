@@ -69,5 +69,5 @@ def test_sass_carries_the_hopper_instructions():
     for mnemonic in ("HGMMA.64x128x16.F32", "HGMMA.64x64x16.F32.BF16", "LDGSTS", "UTMALDG", "HMMA.16816.F32", "REDUX", "MUFU.TANH"):
         assert mnemonic in sass, f"{mnemonic} missing from the SASS of {so}"
     # every tensor-core kernel family is present
-    for kern in ("sra_chain2_kernel", "umma_gemm_kernel", "spconv_umma_kernel", "vfe_l1_umma_kernel", "sir_a_kernel", "sir_b_kernel"):
+    for kern in ("sra_chain2_kernel", "wgmma_gemm_kernel", "spconv_wgmma_kernel", "vfe_l1_wgmma_kernel", "sir_a_kernel", "sir_b_kernel"):
         assert kern in sass, kern

@@ -1,6 +1,6 @@
 """Epilogues of the fused post-attention chain (csrc/sra_chain2.cu): the GELU of its hidden layer and its two LayerNorms.
 
-- gelu_ex2 (csrc/umma_gemm.cuh), the GELU of the chain's GEMM2 epilogue, restated as its exact fp32 operation sequence in numpy
+- gelu_ex2 (csrc/common.cuh), the GELU of the chain's GEMM2 epilogue, restated as its exact fp32 operation sequence in numpy
   (fused multiply-adds rounded once, ex2 rounded to fp32) and held to the exact erf-GELU over [-12, 12]: at most 1e-6 absolute
   and at most one fp16 ulp of the result, which the kernel rounds to fp16.  The coefficients are read from the header.
 - LayerNorm shift-safety: the pre-norm rows of both LayerNorms carry a common offset of +1024 (out_proj.bias feeds LN1,
@@ -29,7 +29,7 @@ SHIFT = 1024.0
 
 
 def _gelu_ex2_coefficients():
-    src = open(os.path.join(ROOT, "sst_b200", "csrc", "umma_gemm.cuh")).read()
+    src = open(os.path.join(ROOT, "sst_b200", "csrc", "common.cuh")).read()
     body = src[src.index("float gelu_ex2(float x)"):]
     body = body[:body.index("\n}\n")]
     clamp = float(re.search(r"fminf\(fabsf\(x\), ([0-9.]+)f\)", body).group(1))

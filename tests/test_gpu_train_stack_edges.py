@@ -5,7 +5,7 @@ Everything but attention is row-tiled, and every tiling depends on the SM count 
   * the LayerNorm backward (ln_bwd_kernel) walks 8 rows per block and pass over 2 x SMs blocks;
   * the weight-gradient GEMM (dw_gemm_kernel + dw_reduce_kernel) splits the rows into 64-row-aligned splits, ceil(2 x SMs / blocks)
     of them, so past 64 x SMs rows (2 output blocks) or 128 x SMs rows (1 block) some splits are empty;
-  * the persistent wgmma GEMMs (launch_umma) run SMs x per_sm CTAs over ceil(n / 128) x ny items and wrap once there are more.
+  * the persistent wgmma GEMMs (launch_wgmma_gemm) run SMs x per_sm CTAs over ceil(n / 128) x ny items and wrap once there are more.
 `stack_edges` restates those formulas and yields the row counts on either side of each boundary.  A dropped or doubled row
 changes a dense-gradient sum by about 1 / n, far below the bf16 bounds, so every case also runs with an upstream gradient that is
 zero except on a few probe rows placed on those boundaries: then the weight, bias and LayerNorm gradients are sums over the
@@ -36,7 +36,7 @@ TOL_Y, TOL_G, TOL_TAU = 1e-2, 2e-2, 3e-2
 TOL_Y_ROW, TOL_DX_ROW = TOL_Y, TOL_G
 
 # ---------------------------------------------------------------------------------------------------------------------------------
-# the schedule of csrc/sra_train.cu and csrc/umma_gemm.cuh, restated
+# the schedule of csrc/sra_train.cu and csrc/wgmma_gemm.cuh, restated
 # ---------------------------------------------------------------------------------------------------------------------------------
 LN_WARPS = 8      # ln_bwd_kernel: 256 threads = 8 warps, one row per warp and pass; grid 2 x SMs (launch_ln_bwd)
 DW_ROWS = 64      # dw_gemm_kernel: rows per slab; a split's rows are rounded up to whole slabs
@@ -60,24 +60,24 @@ def dw_schedule(n, sms, blocks):
 DW_GEMMS = {"dW2": 2, "dW1": 2, "dWo": 1, "dWqk": 2, "dWv": 1}
 
 
-def umma_per_sm(K, NT, f32_stage):
-    """launch_umma: dynamic shared memory = max(operands, staging + accumulator tile) + 1 KB; CTAs per SM = 220 KB / (smem + 6 KB)."""
+def wgmma_per_sm(K, NT, f32_stage):
+    """launch_wgmma_gemm: dynamic shared memory = max(operands, staging + accumulator tile) + 1 KB; CTAs per SM = 220 KB / (smem + 6 KB)."""
     ops = 128 * K * 2 + NT * K * 2
     stage = 128 * NT * (4 if f32_stage else 2) + 128 * NT * 4
     return max(1, (220 * 1024) // (max(ops, stage) + 1024 + 6144))
 
 
 # wgmma GEMMs of the forward and backward: (K, NT, fp32 staging tile (EPI_RES_LN / EPI_ADD_F32), ny = n tiles per row tile)
-UMMA_GEMMS = {"qkv": (128, 128, False, 3), "out_proj_ln1": (128, 128, True, 1), "lin1_gelu": (128, 128, False, 2),
+WGMMA_GEMMS = {"qkv": (128, 128, False, 3), "out_proj_ln1": (128, 128, True, 1), "lin1_gelu": (128, 128, False, 2),
               "lin2_ln2": (256, 128, True, 1), "dz_gelugrad": (128, 128, False, 2), "dx1": (256, 128, True, 1),
               "datt": (128, 128, False, 1), "dx": (384, 128, True, 1)}
 
 
-def umma_schedule(n, sms, gemm):
-    """(items, grid) of launch_umma for `gemm` at n rows: items = ceil(n / 128) ny, grid = min(SMs per_sm, items)."""
-    K, NT, f32, ny = UMMA_GEMMS[gemm]
+def wgmma_schedule(n, sms, gemm):
+    """(items, grid) of launch_wgmma_gemm for `gemm` at n rows: items = ceil(n / 128) ny, grid = min(SMs per_sm, items)."""
+    K, NT, f32, ny = WGMMA_GEMMS[gemm]
     items = (n + 127) // 128 * ny
-    return items, min(sms * umma_per_sm(K, NT, f32), items)
+    return items, min(sms * wgmma_per_sm(K, NT, f32), items)
 
 
 def stack_edges(sms):
@@ -88,8 +88,8 @@ def stack_edges(sms):
     e["ln_pass-1"], e["ln_pass+1"] = p - 1, p + 1
     e["dw2_splits-1"], e["dw2_splits+1"] = 64 * sms - 1, 64 * sms + 1       # 2-block dW: SMs splits of 64 rows, then 128-row splits
     e["dw1_splits-1"], e["dw1_splits+1"] = 128 * sms - 1, 128 * sms + 1     # 1-block dW: 2 SMs splits; the 1-per-SM GEMMs wrap
-    for name, (K, NT, f32, ny) in UMMA_GEMMS.items():          # first row count at which some CTA takes a second item
-        wrap = 128 * (sms * umma_per_sm(K, NT, f32) // ny) + 1
+    for name, (K, NT, f32, ny) in WGMMA_GEMMS.items():          # first row count at which some CTA takes a second item
+        wrap = 128 * (sms * wgmma_per_sm(K, NT, f32) // ny) + 1
         if wrap not in e.values():
             e[f"{name}_wrap"] = wrap
     return e
@@ -119,13 +119,13 @@ def test_stack_edges_hit_every_boundary():
             empty = {n for n, (s, rp, ne) in zip(ns, sched) if ne < s}
             assert any(n + 2 in empty for n in full), name             # the two sides of the same boundary
         # wgmma GEMMs: the first row count at which a CTA takes a second item is tested, and one tile fewer wraps no CTA
-        for name, (K, NT, f32, ny) in UMMA_GEMMS.items():
-            cap = sms * umma_per_sm(K, NT, f32)
+        for name, (K, NT, f32, ny) in WGMMA_GEMMS.items():
+            cap = sms * wgmma_per_sm(K, NT, f32)
             first = 128 * (cap // ny) + 1
             assert first in ns, name
-            assert umma_schedule(first, sms, name)[0] > cap >= umma_schedule(first - 1, sms, name)[0], name
+            assert wgmma_schedule(first, sms, name)[0] > cap >= wgmma_schedule(first - 1, sms, name)[0], name
         # the q|k|v GEMM runs 2 CTAs per SM, the LayerNorm epilogues 1, the datt GEMM 2 (wraps at 256 SMs)
-        assert umma_per_sm(128, 128, False) == 2 and umma_per_sm(128, 128, True) == 1 and umma_per_sm(384, 128, True) == 1
+        assert wgmma_per_sm(128, 128, False) == 2 and wgmma_per_sm(128, 128, True) == 1 and wgmma_per_sm(384, 128, True) == 1
         assert e["qkv_wrap"] == 128 * (2 * sms // 3) + 1 and e["datt_wrap"] == 256 * sms + 1
 
 
