@@ -21,11 +21,13 @@
 // fence.proxy.async and a named barrier; the tile loop has no CTA-wide barrier.
 // Epilogues run on the accumulator fragments: a row's 128 columns sit in one lane quad, so LayerNorm statistics take two
 // xor-shuffles; x1 stays in registers from GEMM1 to GEMM3; x1, h, y and y + pos reach the next GEMM as 16-bit operands written
-// straight into the swizzled K-major layout.  Only x (residual), y and q|k|v touch global memory; q|k|v leave as 16-byte stores
-// after a transpose inside each lane quad (whole 32-byte sectors per warp store).  All rows are in flat token order.
+// into the swizzled K-major layout by stmatrix, 16 columns of a warp's 16 rows per instruction.  Only x (residual), y and q|k|v
+// touch global memory; each warp writes its 16 rows of a q|k|v chunk into shared memory the same way and copies them out as whole
+// 256-byte row segments.  All rows are in flat token order.
 //
 // Shared memory, per warpgroup (64 rows, K-major, 128B swizzle, 8 KB per 64-wide K block): X 16 KB (x1, then y) | T 16 KB (att) |
-// H 32 KB (hidden, four K blocks; y + pos aliased onto its first 16 KB once GEMM3 has retired); then the ring, 3 x 32 KB.
+// H 32 KB (hidden, four K blocks; y + pos aliased onto its first 16 KB once GEMM3 has retired, q|k|v staged in its upper 16 KB);
+// then the ring, 3 x 32 KB.
 #include <stdarg.h>
 #include <cuda_fp16.h>
 #include "sra.cuh"
@@ -58,10 +60,13 @@ struct Chain2Args {
   int affine;
   int M_cap;
   const int32_t* M_dev;
-  const float* pos_tab;          // next layer's per-axis positional table, added to y for the q|k chunks
+  // next layer's per-axis positional table, added to y for the q|k chunks.  Columns [32 grp, 32 grp + 32) lie inside one axis
+  // (posL % 32 == 0): pos_grp[grp] is that axis's first table row shifted back by the axis's first column, or null past the last
+  // axis; byte grp of pos_shift is 8 x the axis, the position of the row's code for it in pos_code.
+  const float* pos_grp[4];
   const int32_t* pos_code;
-  int posL, pos_maxw, pos_ndim;
-  int pos_axes;                  // byte grp: the axis of columns [32 grp, 32 grp + 32)
+  int posL;
+  int pos_shift;
 };
 
 // chunk j of a tile: 0 Wo | 1, 2 W1 rows 0-127, 128-255 | 3, 4 W2 K 0-127, 128-255 | 5, 6, 7 Wqkv rows 0-127, 128-255, 256-383
@@ -77,23 +82,26 @@ __device__ __forceinline__ void issue_chunk(const Chain2Maps& m, int j, uint32_t
   tma_load_2d(dst + SLOT / 2, map, k0 + 64, n0, bar);
 }
 
-// 16-bit pair (columns k, k + 1) of row `row` into a 64-row wgmma operand (format in wgmma.cuh).  The address is spelled out
-// rather than taken from sw128_off: with k = 128 h + c (GEMM2's epilogue) only the masked form (k & 63) >> 3 lets the compiler
-// fold the piece index; sw128_off's (k >> 3) & 7 costs the kernel ~100 more instructions.
-__device__ __forceinline__ void st_op(uint32_t buf, int row, int k, uint32_t v) {
-  asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(buf + (k >> 6) * OPH + row * 128 + ((((k & 63) >> 3) ^ (row & 7)) << 4) + (k & 7) * 2), "r"(v) : "memory");
+// Columns 16 p .. 16 p + 15 of fragment t (pairs 2p and 2p + 1 of rows ra and rb) as 16-bit operand pieces, by one stmatrix.x4
+// at the lane's stsm_base `ob` of a 64-row operand (format in wgmma.cuh).
+__device__ __forceinline__ void st_op16(uint32_t ob, int p, const float (&t)[64]) {
+  stsm_x4(ob, p, OPH, pack_f16(t[8 * p], t[8 * p + 1]), pack_f16(t[8 * p + 2], t[8 * p + 3]), pack_f16(t[8 * p + 4], t[8 * p + 5]),
+          pack_f16(t[8 * p + 6], t[8 * p + 7]));
 }
+
+// columns 8 j + cq, cq + 1 of a row whose pointer `p` already includes the lane's cq: one base address, j an immediate offset
+__device__ __forceinline__ float2 ldg2(const float* p, int j) { return __ldg(reinterpret_cast<const float2*>(p + 8 * j)); }
 
 // t = fragment of [64 rows x 128] (rows ra: t[4j], t[4j+1]; rb: t[4j+2], t[4j+3]; columns 8j + 2 (lane & 3)): per-row normalisation.
 // LayerNorm statistics take two passes over the register-resident rows, the mean and then the sum of centred squares, so a large
 // common offset in a row does not cancel the variance away as E[t^2] - mean^2 would.
 __device__ __forceinline__ void row_norm(float (&t)[64], const float* __restrict__ gam, const float* __restrict__ bet, float eps, bool affine) {
   const int cq = 2 * (threadIdx.x & 3);
+  gam += cq, bet += cq;
   if (affine) {   // eval BatchNorm folded to one scale and shift per channel
 #pragma unroll
     for (int j = 0; j < 16; j++) {
-      const int c = 8 * j + cq;
-      const float2 g2 = __ldg(reinterpret_cast<const float2*>(gam + c)), b2 = __ldg(reinterpret_cast<const float2*>(bet + c));
+      const float2 g2 = ldg2(gam, j), b2 = ldg2(bet, j);
       t[4 * j] = fmaf(t[4 * j], g2.x, b2.x);
       t[4 * j + 1] = fmaf(t[4 * j + 1], g2.y, b2.y);
       t[4 * j + 2] = fmaf(t[4 * j + 2], g2.x, b2.x);
@@ -128,8 +136,7 @@ __device__ __forceinline__ void row_norm(float (&t)[64], const float* __restrict
   const float rstd0 = rsqrtf(q0 * (1.f / D) + eps), rstd1 = rsqrtf(q1 * (1.f / D) + eps);
 #pragma unroll
   for (int j = 0; j < 16; j++) {
-    const int c = 8 * j + cq;
-    const float2 g2 = __ldg(reinterpret_cast<const float2*>(gam + c)), b2 = __ldg(reinterpret_cast<const float2*>(bet + c));
+    const float2 g2 = ldg2(gam, j), b2 = ldg2(bet, j);
     t[4 * j] = fmaf(t[4 * j] * rstd0, g2.x, b2.x);
     t[4 * j + 1] = fmaf(t[4 * j + 1] * rstd0, g2.y, b2.y);
     t[4 * j + 2] = fmaf(t[4 * j + 2] * rstd1, g2.x, b2.x);
@@ -137,35 +144,11 @@ __device__ __forceinline__ void row_norm(float (&t)[64], const float* __restrict
   }
 }
 
-// One row's 128 fp16 outputs held by a lane quad as 16 packed pairs (pair j: columns 8j + 2 (lane & 3), 8j + 2 (lane & 3) + 1).
-// A 4 x 4 transpose of each group of four pairs inside the quad gives every lane 8 consecutive columns, so each lane stores 16 B
-// and a warp writes whole 32-byte sectors instead of 4-byte pieces of them.  All lanes shuffle; `ok` only gates the stores.
-__device__ __forceinline__ void st_row_f16(__half* row, const uint32_t (&p)[16], bool ok) {
-  const int qd = threadIdx.x & 3;
-  const bool o = qd & 1, t = qd & 2;
-#pragma unroll
-  for (int m = 0; m < 4; m++) {
-    uint32_t v0 = p[4 * m], v1 = p[4 * m + 1], v2 = p[4 * m + 2], v3 = p[4 * m + 3];
-    // exchange across lane bit 0, then bit 1: afterwards slot k of lane qd holds lane k's pair of group 4m + qd
-    uint32_t r = __shfl_xor_sync(0xffffffffu, o ? v0 : v1, 1);
-    if (o) v0 = r; else v1 = r;
-    r = __shfl_xor_sync(0xffffffffu, o ? v2 : v3, 1);
-    if (o) v2 = r; else v3 = r;
-    r = __shfl_xor_sync(0xffffffffu, t ? v0 : v2, 2);
-    if (t) v0 = r; else v2 = r;
-    r = __shfl_xor_sync(0xffffffffu, t ? v1 : v3, 2);
-    if (t) v1 = r; else v3 = r;
-    if (ok) *reinterpret_cast<uint4*>(row + 8 * (4 * m + qd)) = make_uint4(v0, v1, v2, v3);
-  }
-}
-
-// Positional codes of one row for the 32 columns [32 grp, 32 grp + 32), which lie inside one axis (posL % 32 == 0): column c
-// adds pos_row(g, code, grp)[c], or nothing when the pointer is null (the columns lie past the last axis).
-__device__ __forceinline__ const float* pos_row(const Chain2Args& g, int code, int grp) {
-  const int axis = (g.pos_axes >> (8 * grp)) & 255;
-  if (axis >= g.pos_ndim) return nullptr;
-  const int cv = (code >> (8 * axis)) & 255;
-  return g.pos_tab + ((size_t)axis * (g.pos_maxw - 1) + cv) * g.posL;   // table row (axis, cv), shifted back by the axis's first column
+// Positional table row of one row (positional code `code`) for the 32 columns [32 grp, 32 grp + 32), offset by the lane's cq:
+// column 8 j + cq adds ldg2(pos_row(...), j).  Only for groups with g.pos_grp[grp] set.
+__device__ __forceinline__ const float* pos_row(const Chain2Args& g, int code, int grp, int cq) {
+  const int cv = (code >> ((g.pos_shift >> (8 * grp)) & 255)) & 255;
+  return g.pos_grp[grp] + (cv * g.posL + cq);
 }
 
 template <bool TAIL>
@@ -257,6 +240,7 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
 
   const int rl = 16 * ((tid >> 5) & 3) + (lane >> 2);   // fragment rows rl, rl + 8 of this warpgroup's half
   const int cq = 2 * (lane & 3);
+  const uint32_t oX = stsm_base(sX), oH = oX + (OFF_H - OFF_X);   // this lane's stmatrix row addresses in X and H
   uint32_t att_par = 0;
   float acc[64], x1[64];
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -271,11 +255,11 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
       wg_tile_mma<128, false, 8>(acc, sT, OPH, w, OPB, false);
     }
     // residual rows and positional codes load while the MMA runs
+    const float* xA = g.x + (size_t)rowA * D + cq;   // row rb is 8 rows further
 #pragma unroll
     for (int j = 0; j < 16; j++) {
-      const int c = 8 * j + cq;
-      const float2 ra = okA ? *reinterpret_cast<const float2*>(g.x + (size_t)rowA * D + c) : make_float2(0.f, 0.f);
-      const float2 rb = okB ? *reinterpret_cast<const float2*>(g.x + (size_t)rowB * D + c) : make_float2(0.f, 0.f);
+      const float2 ra = okA ? *reinterpret_cast<const float2*>(xA + 8 * j) : make_float2(0.f, 0.f);
+      const float2 rb = okB ? *reinterpret_cast<const float2*>(xA + 8 * D + 8 * j) : make_float2(0.f, 0.f);
       x1[4 * j] = ra.x, x1[4 * j + 1] = ra.y, x1[4 * j + 2] = rb.x, x1[4 * j + 3] = rb.y;
     }
     int codeA = 0, codeB = 0;
@@ -287,8 +271,7 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
     release(1);
 #pragma unroll
     for (int j = 0; j < 16; j++) {
-      const int c = 8 * j + cq;
-      const float2 b = __ldg(reinterpret_cast<const float2*>(g.bo + c));
+      const float2 b = ldg2(g.bo + cq, j);
       x1[4 * j] = acc[4 * j] + b.x + x1[4 * j];
       x1[4 * j + 1] = acc[4 * j + 1] + b.y + x1[4 * j + 1];
       x1[4 * j + 2] = acc[4 * j + 2] + b.x + x1[4 * j + 2];
@@ -296,11 +279,7 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
     }
     row_norm(x1, g.g1, g.be1, g.eps, g.affine);
 #pragma unroll
-    for (int j = 0; j < 16; j++) {
-      const int c = 8 * j + cq;
-      st_op(sX, rl, c, pack_f16(x1[4 * j], x1[4 * j + 1]));
-      st_op(sX, rl + 8, c, pack_f16(x1[4 * j + 2], x1[4 * j + 3]));
-    }
+    for (int p = 0; p < 8; p++) st_op16(oX, p, x1);
     wg_sync();   // also: every warp of this warpgroup has retired GEMM1, so T is free for the next tile's attention half
     if (leader && tile + (int)gridDim.x < ntiles) issue_att(tile + gridDim.x);
 
@@ -311,11 +290,16 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
       wgmma_wait<0>();
       release(1);
 #pragma unroll
-      for (int j = 0; j < 16; j++) {
-        const int c = 8 * j + cq;
-        const float2 b = __ldg(reinterpret_cast<const float2*>(g.b1 + 128 * h + c));
-        st_op(sH, rl, 128 * h + c, pack_f16(gelu_ex2(acc[4 * j] + b.x), gelu_ex2(acc[4 * j + 1] + b.y)));
-        st_op(sH, rl + 8, 128 * h + c, pack_f16(gelu_ex2(acc[4 * j + 2] + b.x), gelu_ex2(acc[4 * j + 3] + b.y)));
+      for (int p = 0; p < 8; p++) {
+        uint32_t v[4];
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+          const int j = 2 * p + i;
+          const float2 b = ldg2(g.b1 + 128 * h + cq, j);
+          v[2 * i] = pack_f16(gelu_ex2(acc[4 * j] + b.x), gelu_ex2(acc[4 * j + 1] + b.y));
+          v[2 * i + 1] = pack_f16(gelu_ex2(acc[4 * j + 2] + b.x), gelu_ex2(acc[4 * j + 3] + b.y));
+        }
+        stsm_x4(oH + h * 2 * OPH, p, OPH, v[0], v[1], v[2], v[3]);
       }
     }
     wg_sync();
@@ -324,8 +308,7 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
     // the accumulators start at x1 + b2, so the MMA adds the residual and the bias and x1 is dead once it is issued
 #pragma unroll
     for (int j = 0; j < 16; j++) {
-      const int c = 8 * j + cq;
-      const float2 b = __ldg(reinterpret_cast<const float2*>(g.b2 + c));
+      const float2 b = ldg2(g.b2 + cq, j);
       acc[4 * j] = x1[4 * j] + b.x;
       acc[4 * j + 1] = x1[4 * j + 1] + b.y;
       acc[4 * j + 2] = x1[4 * j + 2] + b.x;
@@ -339,44 +322,72 @@ __global__ void __launch_bounds__(NTHR, 1) sra_chain2_kernel(const __grid_consta
       release(2);
     }
     row_norm(acc, g.g2, g.be2, g.eps, g.affine);
-#pragma unroll
-    for (int grp = 0; grp < 4; grp++) {
-      const float* posA = TAIL ? pos_row(g, codeA, grp) : nullptr;
-      const float* posB = TAIL ? pos_row(g, codeB, grp) : nullptr;
-#pragma unroll
-      for (int j = 4 * grp; j < 4 * grp + 4; j++) {
-        const int c = 8 * j + cq;
-        if (okA) *reinterpret_cast<float2*>(g.y + (size_t)rowA * D + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        if (okB) *reinterpret_cast<float2*>(g.y + (size_t)rowB * D + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        if (TAIL) {
-          st_op(sX, rl, c, pack_f16(acc[4 * j], acc[4 * j + 1]));
-          st_op(sX, rl + 8, c, pack_f16(acc[4 * j + 2], acc[4 * j + 3]));
-          const float2 pa = posA ? __ldg(reinterpret_cast<const float2*>(posA + c)) : make_float2(0.f, 0.f);
-          const float2 pb = posB ? __ldg(reinterpret_cast<const float2*>(posB + c)) : make_float2(0.f, 0.f);
-          st_op(sH, rl, c, pack_f16(acc[4 * j] + pa.x, acc[4 * j + 1] + pa.y));
-          st_op(sH, rl + 8, c, pack_f16(acc[4 * j + 2] + pb.x, acc[4 * j + 3] + pb.y));
-        }
-      }
-    }
-    if (!TAIL) continue;
-    wg_sync();
-
-    // ---- GEMM4: next layer's q|k (from y + pos) and v (from y) + bias -> fp16 rows ------------------------------------------------
-#pragma unroll 1
-    for (int q = 0; q < 3; q++) {
-      wg_tile_mma<128, false, 8>(acc, q < 2 ? sH : sX, OPH, acquire(0), OPB, false);
-      wgmma_wait<0>();
-      release(1);
-      uint32_t pa[16], pb[16];
+    {
+      float* yA = g.y + (size_t)rowA * D + cq;   // row rb is 8 rows further
 #pragma unroll
       for (int j = 0; j < 16; j++) {
-        const int c = 8 * j + cq;
-        const float2 b = __ldg(reinterpret_cast<const float2*>(g.bqkv + 128 * q + c));
-        pa[j] = pack_f16(acc[4 * j] + b.x, acc[4 * j + 1] + b.y);
-        pb[j] = pack_f16(acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y);
+        if (okA) *reinterpret_cast<float2*>(yA + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        if (okB) *reinterpret_cast<float2*>(yA + 8 * D + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
-      st_row_f16(g.qkv + (size_t)rowA * 3 * D + 128 * q, pa, okA);
-      st_row_f16(g.qkv + (size_t)rowB * 3 * D + 128 * q, pb, okB);
+    }
+    if constexpr (TAIL) {   // y -> X, y + pos -> H, then GEMM4
+#pragma unroll
+      for (int p = 0; p < 8; p++) st_op16(oX, p, acc);
+#pragma unroll
+      for (int grp = 0; grp < 4; grp++) {
+        const bool has = g.pos_grp[grp] != nullptr;   // uniform
+        const float* posA = pos_row(g, codeA, grp, cq);
+        const float* posB = pos_row(g, codeB, grp, cq);
+#pragma unroll
+        for (int p = 2 * grp; p < 2 * grp + 2; p++) {
+          uint32_t v[4];
+#pragma unroll
+          for (int i = 0; i < 2; i++) {
+            const int j = 2 * p + i;
+            const float2 pa = has ? ldg2(posA, j) : make_float2(0.f, 0.f);
+            const float2 pb = has ? ldg2(posB, j) : make_float2(0.f, 0.f);
+            v[2 * i] = pack_f16(acc[4 * j] + pa.x, acc[4 * j + 1] + pa.y);
+            v[2 * i + 1] = pack_f16(acc[4 * j + 2] + pb.x, acc[4 * j + 3] + pb.y);
+          }
+          stsm_x4(oH, p, OPH, v[0], v[1], v[2], v[3]);
+        }
+      }
+      wg_sync();
+
+      // ---- GEMM4: next layer's q|k (from y + pos) and v (from y) + bias -> fp16 rows ----------------------------------------------
+      // Each warp stages its 16 rows of a chunk in H's upper 16 KB (free: y + pos fills the lower half) and copies them out itself:
+      // per step, lanes 0-15 and 16-31 each store one row's 256 contiguous bytes.  Lane piece (lane & 15) of rows rq + 2 i.
+      const int rw = 16 * ((tid >> 5) & 3) + (lane >> 4), rq = tile * TM + wg * HM + rw;
+      __half* gq = g.qkv + (size_t)rq * 3 * D + 8 * (lane & 15);
+      const uint32_t sq = sH + 2 * OPH + ((lane >> 3) & 1) * OPH + rw * 128 + (((lane & 7) ^ (lane >> 4)) << 4);
+#pragma unroll 1
+      for (int q = 0; q < 3; q++) {
+        wg_tile_mma<128, false, 8>(acc, q < 2 ? sH : sX, OPH, acquire(0), OPB, false);
+        wgmma_wait<0>();
+        release(1);
+#pragma unroll
+        for (int p = 0; p < 8; p++) {
+          uint32_t v[4];
+#pragma unroll
+          for (int i = 0; i < 2; i++) {
+            const int j = 2 * p + i;
+            const float2 b = ldg2(g.bqkv + 128 * q + cq, j);
+            v[2 * i] = pack_f16(acc[4 * j] + b.x, acc[4 * j + 1] + b.y);
+            v[2 * i + 1] = pack_f16(acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y);
+          }
+          stsm_x4(oH + 2 * OPH, p, OPH, v[0], v[1], v[2], v[3]);
+        }
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < 8; i++) {   // row rq + 2 i sits at row & 7 = (2 i + (lane >> 4)) & 7 of its swizzle atom
+          uint4 v;
+          asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];\n"
+                       : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+                       : "r"((sq ^ ((uint32_t)(2 * i & 7) << 4)) + 256 * i)
+                       : "memory");
+          if (rq + 2 * i < M) *reinterpret_cast<uint4*>(gq + (size_t)2 * i * 3 * D + 128 * q) = v;
+        }
+      }
     }
   }
 }
@@ -437,12 +448,14 @@ int sstb_sra_chain2(sstb200_ctx* c, const sstb200_sra_layer* L, const __half* at
     rc |= tmap_2d_sw128(&maps.wqkv, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, next->in_proj_w_f16, 128, 384, 256, 64, 128);
     g.qkv = reinterpret_cast<__half*>(next_qkv);
     g.bqkv = next->in_proj_b;
-    g.pos_tab = next_plan->pos_table;
     g.pos_code = next_plan->pos_code;
     g.posL = next_plan->pos_L;
-    g.pos_maxw = next_plan->pos_maxw;
-    g.pos_ndim = next_plan->pos_ndim;
-    for (int grp = 0; grp < 4; grp++) g.pos_axes |= (32 * grp / g.posL) << (8 * grp);
+    for (int grp = 0; grp < 4; grp++) {   // table [ndim][maxw][posL]: row (axis, cv) at (axis maxw + cv) posL, its columns from axis posL on
+      const int axis = 32 * grp / g.posL;
+      if (axis >= next_plan->pos_ndim) continue;
+      g.pos_grp[grp] = next_plan->pos_table + (size_t)axis * (next_plan->pos_maxw - 1) * g.posL;
+      g.pos_shift |= (8 * axis) << (8 * grp);
+    }
   }
   if (rc) return sstb_fail(c, SSTB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d): operands must be 16-byte aligned", rc);
   g.x = x;

@@ -20,6 +20,22 @@ __device__ __forceinline__ size_t sw128_off(int rows, int r, int j) {
   return (size_t)(j >> 3) * rows * 128 + r * 128 + (((j & 7) ^ (r & 7)) << 4);
 }
 
+// Accumulator fragment (m64nN layout, wg_frag_pairs below) -> 16-bit operand of a warpgroup's 64 rows, by stmatrix: one .x4 stores
+// 16 columns of the warp's 16 rows, its four 8 x 8 matrices being rows 0-7 and 8-15 of columns 0-7, then of columns 8-15 (each
+// lane's register holds the pair its fragment holds).  Lane l names row l & 7 of matrix l >> 3.  stsm_base gives that row's address
+// for columns 0-15 of the operand at `buf` (128-B aligned); columns 16 p .. 16 p + 15 are pieces 2p & 7 and its neighbour of K
+// block p >> 2, so only the swizzled piece bits (4-6) change, by an XOR with 2p & 7, and the block adds its pitch.
+__device__ __forceinline__ uint32_t stsm_base(uint32_t buf) {
+  const int l = threadIdx.x & 31;
+  const int r = 16 * ((threadIdx.x >> 5) & 3) + (l & 15);
+  return buf + r * 128 + ((((l >> 4) & 1) ^ (l & 7)) << 4);
+}
+__device__ __forceinline__ void stsm_x4(uint32_t base, int p, uint32_t block_pitch, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"((base ^ ((uint32_t)(2 * p & 7) << 4)) + (uint32_t)(p >> 2) * block_pitch),
+               "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+               : "memory");
+}
+
 // One 16-byte piece of an operand: cp.async from `src` when `valid` (completed by the caller's cp.async.wait_all), zeros otherwise
 __device__ __forceinline__ void cp_async_piece_or_zero(uint8_t* dst, const void* src, bool valid) {
   if (valid)
@@ -106,13 +122,16 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 // One warpgroup: rows of A starting at `a` (already offset to the warpgroup's 64 rows), rows of B starting at `b`; KSTEPS
 // steps of K = 16; a_cp / b_cp = byte pitch of one 64-wide K chunk of each operand.  Issues and commits one wgmma group;
 // the caller waits with wgmma_wait.  accumulate = false starts from zero.
+// Each step's descriptor is the first one plus its byte offset >> 4: shared addresses lie below 2^18, so the 14-bit start field
+// of every operand address never carries into the next field, and the descriptors equal wg_desc_sw128 of each address.
 template <int N, bool BF16, int KSTEPS>
 __device__ __forceinline__ void wg_tile_mma(float (&d)[N / 2], uint32_t a, uint32_t a_cp, uint32_t b, uint32_t b_cp, bool accumulate) {
+  const uint64_t da = wg_desc_sw128(a), db = wg_desc_sw128(b);
   wgmma_fence();
 #pragma unroll
   for (int k = 0; k < KSTEPS; k++) {
     const uint32_t off = (uint32_t)(k >> 2), s = (uint32_t)(k & 3) * 32u;
-    wgmma_ss<N, BF16>(d, wg_desc_sw128(a + off * a_cp + s), wg_desc_sw128(b + off * b_cp + s), (accumulate || k) ? 1 : 0);
+    wgmma_ss<N, BF16>(d, da + ((off * a_cp + s) >> 4), db + ((off * b_cp + s) >> 4), (accumulate || k) ? 1 : 0);
   }
   wgmma_commit();
 }

@@ -41,10 +41,10 @@ CLASSES = [
     ("convert", ("F2FP", "F2F", "F2I", "I2F", "I2FP", "F2IP")),
     ("shuffle", ("SHFL",)),
     ("global", ("LDG", "STG", "LD", "ST", "RED", "ATOM")),
-    ("shared", ("LDS", "STS", "LDSM", "ATOMS")),
+    ("shared", ("LDS", "STS", "LDSM", "STSM", "ATOMS")),
     ("const", ("LDC", "ULDC")),
-    ("sync/tma", ("BAR", "SYNCS", "UTMALDG", "UBLKCP", "FENCE", "MEMBAR", "DEPBAR", "WARPSYNC", "ACQBULK", "PREEXIT", "ELECT",
-                  "UTMAPF", "CCTL", "ERRBAR")),
+    ("sync/tma", ("BAR", "SYNCS", "UTMALDG", "UTMASTG", "UBLKCP", "UTMACMDFLUSH", "FENCE", "MEMBAR", "DEPBAR", "WARPSYNC", "ACQBULK",
+                  "PREEXIT", "ELECT", "UTMAPF", "CCTL", "ERRBAR")),
     ("control", ("BRA", "BSSY", "BSYNC", "EXIT", "RET", "CALL", "YIELD", "BPT", "NANOSLEEP", "VOTE", "VOTEU", "PLOP3")),
 ]
 
