@@ -338,7 +338,11 @@ __device__ __forceinline__ uint32_t sp_pack_f16(float a, float b) {
 constexpr int SPU_EXP_TOP = 14;    // a scaled row's largest |element| lies in [2^13, 2^14): below fp16's 65504 with room for rounding
 constexpr int SPU_EXP_LIM = 100;   // |exponent| bound: 2^+-100 and every product with an fp16-range value are exact fp32
 
-// rexp[i] = the power of two that lifts row i's largest |element| into [2^(SPU_EXP_TOP - 1), 2^SPU_EXP_TOP); one warp per row
+// the power of two that lifts a largest |element| of bits m into [2^(SPU_EXP_TOP - 1), 2^SPU_EXP_TOP): amax = f * 2^(field - 126),
+// f in [0.5, 1); an all-zero (or subnormal) row takes the largest exponent and never decides a minimum
+__device__ __forceinline__ int sp_exp_of(uint32_t m) { return max(-SPU_EXP_LIM, min(SPU_EXP_LIM, SPU_EXP_TOP - ((int)(m >> 23) - 126))); }
+
+// rexp[i] = sp_exp_of(row i's largest |element|); one warp per row
 __global__ void __launch_bounds__(256) sp_row_exp_kernel(const float* __restrict__ feats, int lda, int C, int n, const int32_t* __restrict__ n_dev,
                                                         int32_t* __restrict__ rexp) {
   pdl_wait();
@@ -355,8 +359,7 @@ __global__ void __launch_bounds__(256) sp_row_exp_kernel(const float* __restrict
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-  // amax = f * 2^(field - 126), f in [0.5, 1); an all-zero (or subnormal) row takes the largest exponent and never decides a minimum
-  if (lane == 0) rexp[row] = max(-SPU_EXP_LIM, min(SPU_EXP_LIM, SPU_EXP_TOP - ((int)(m >> 23) - 126)));
+  if (lane == 0) rexp[row] = sp_exp_of(m);
 }
 
 __device__ __forceinline__ float sp_exp2i(int e) { return __int_as_float((e + 127) << 23); }   // 2^e, |e| <= SPU_EXP_LIM
@@ -364,6 +367,7 @@ __device__ __forceinline__ float sp_exp2i(int e) { return __int_as_float((e + 12
 struct SpArgs {
   const float* feats;      // [*, lda] fp32 rows (gathered through nbr, or row o itself when nbr == nullptr)
   const int32_t* rexp;     // per-row power-of-two exponents of feats (sp_row_exp_kernel), or nullptr: operands converted as they are
+  int self_exp;            // SPLIT, nbr == nullptr only: each CTA takes its rows' exponents from the rows themselves (rexp unused)
   const float* wun;        // [Cout] 2^-e of the exponent the 16-bit weight copy carries per output channel, or nullptr (1)
   int lda, Cin;
   const int32_t* nbr;      // [n_out, KV] or nullptr (KV must be 1: a plain row GEMM)
@@ -430,7 +434,7 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_wgmm
     if (lane == 0 && m) atomicOr(&used_mask, m);
   }
   __syncthreads();
-  if (tid < SPU_TM) {
+  if (!(SPLIT && g.self_exp) && tid < SPU_TM) {   // (GEMM mode: below, behind the first two stages' loads)
     int e = g.rexp ? SPU_EXP_LIM : 0;
     if (g.rexp)
       for (int k = 0; k < KV; k++) {
@@ -538,6 +542,27 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_wgmm
   R0.valid = R1.valid = 0u;
   load_next(R0);
   load_next(R1);
+  if (SPLIT && g.self_exp) {   // GEMM mode (sstb_gemm_rows_x3), while the first two stages load: eight threads per row, 128
+    // contiguous bytes per row and load
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const int r = (tid >> 3) + 32 * u, o = row0 + r;
+      uint32_t m = 0u;
+      if (o < n_out) {
+        const float4* p = reinterpret_cast<const float4*>(g.feats + (size_t)o * g.lda);
+#pragma unroll 4
+        for (int q = tid & 7; q < (Cin >> 2); q += 8) {   // Cin is a multiple of 64: 2 or more loads per thread, several in flight
+          const float4 v = p[q];
+          m = max(max(m, __float_as_uint(v.x) & 0x7fffffffu), max(__float_as_uint(v.y) & 0x7fffffffu, __float_as_uint(v.z) & 0x7fffffffu));
+          m = max(m, __float_as_uint(v.w) & 0x7fffffffu);
+        }
+      }
+#pragma unroll
+      for (int x = 4; x > 0; x >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, x));
+      if ((tid & 7) == 0) sExp[r] = sp_exp_of(m);
+    }
+    __syncthreads();
+  }
   for (int s = 0; s < nst; s += 2) {
     run_stage(s, R0);
     if (s + 1 < nst) run_stage(s + 1, R1);
@@ -593,16 +618,32 @@ static int dispatch_spconv_wgmma(sstb200_ctx* c, const SpArgs& g, bool split) {
   return launch_spconv_wgmma<64, 3, false>(c, g);
 }
 
-// W fp32 -> (hi, lo) fp16, elementwise
-__global__ void split_f16_kernel(const float* __restrict__ w, size_t n, __half* __restrict__ hi, __half* __restrict__ lo) {
+// W [N, K] fp32 -> (hi, lo) fp16, one block per output channel: the channel is lifted by the power of two sp_exp_of gives its
+// largest |w| before it is split (exact), and wun[n] = the inverse power, which the epilogue applies
+__global__ void __launch_bounds__(256) split_f16_rows_kernel(const float* __restrict__ w, int K, __half* __restrict__ hi,
+                                                            __half* __restrict__ lo, float* __restrict__ wun) {
   pdl_wait();
   pdl_launch();
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float x = w[i];
-  const __half h = __float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f));
-  hi[i] = h;
-  lo[i] = __float2half_rn(x - __half2float(h));
+  __shared__ uint32_t amax;
+  const int n = blockIdx.x;
+  const float* p = w + (size_t)n * K;
+  if (threadIdx.x == 0) amax = 0u;
+  __syncthreads();
+  uint32_t m = 0u;   // |w| as bits, as in sp_row_exp_kernel
+  for (int k = threadIdx.x; k < K; k += 256) m = max(m, __float_as_uint(p[k]) & 0x7fffffffu);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) atomicMax(&amax, m);
+  __syncthreads();
+  const int e = sp_exp_of(amax);
+  const float s = sp_exp2i(e);
+  for (int k = threadIdx.x; k < K; k += 256) {
+    const float x = p[k] * s;
+    const __half h = __float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f));
+    hi[(size_t)n * K + k] = h;
+    lo[(size_t)n * K + k] = __float2half_rn(x - __half2float(h));
+  }
+  if (threadIdx.x == 0) wun[n] = sp_exp2i(-e);
 }
 
 }  // namespace
@@ -762,7 +803,7 @@ extern "C" int sstb200_spconv_forward(sstb200_ctx* c, const float* feats, int n_
   if (!rexp) return sstb_fail(c, SSTB_ERR_WORKSPACE, "spconv_forward: arena too small");
   if (n_in) launch_pdl(sp_row_exp_kernel, dim3((n_in + 7) / 8), dim3(256), (size_t)0, c->stream, feats, c_in, c_in, n_in, (const int32_t*)nullptr, rexp);
   SpArgs g;
-  g.feats = feats, g.rexp = rexp, g.wun = weight_h16_unscale;
+  g.feats = feats, g.rexp = rexp, g.self_exp = 0, g.wun = weight_h16_unscale;
   g.lda = c_in, g.Cin = c_in, g.nbr = nbr, g.n_out = n_out, g.n_dev = nullptr, g.KV = kernel_volume;
   g.Whi = (const __half*)weight_h16;
   g.Wlo = g.Whi + (size_t)kernel_volume * c_out * c_in;   // FP32_TC: the residue copy follows the hi copy
@@ -771,18 +812,20 @@ extern "C" int sstb200_spconv_forward(sstb200_ctx* c, const float* feats, int n_
 }
 
 // fp32-tolerance row GEMM on the tensor core (used by the fp32 mode of the SRA encoder, csrc/sra_fp32.cu):
-//   out[r, :N] = act(A[r, :K] . W[N, K]^T + bias) + res[r]      with every operand split into two fp16 numbers (see SPLIT above)
+//   out[r, :N] = act(A[r, :K] . W[N, K]^T + bias) + res[r]      with every operand split into two fp16 numbers (see SPLIT above),
+// each row of A and each output channel of W first lifted to the top of fp16's range by its own power of two, as in
+// sstb200_spconv_forward: the result is homogeneous in the scale of either operand
 int sstb_gemm_rows_x3(sstb200_ctx* c, const float* A, int lda, const float* W, const float* bias, const float* res, int ldr, float* out,
                       int ldo, int M_cap, const int32_t* M_dev, int N, int K, int act) {
   if (M_cap <= 0) return SSTB_OK;
   if ((K & 63) || (N & 63) || (lda & 3) || (ldo & 3) || (ldr & 3) || (act == 1 && res)) return SSTB_ERR_UNSUPPORTED;
   __half* hi = arena_alloc<__half>(c, (size_t)N * K);
   __half* lo = arena_alloc<__half>(c, (size_t)N * K);
-  if (!hi || !lo) return sstb_fail(c, SSTB_ERR_WORKSPACE, "gemm_rows_x3: arena too small");
-  const size_t n = (size_t)N * K;
-  launch_pdl(split_f16_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), (size_t)0, c->stream, W, n, hi, lo);
+  float* wun = arena_alloc<float>(c, (size_t)N);
+  if (!hi || !lo || !wun) return sstb_fail(c, SSTB_ERR_WORKSPACE, "gemm_rows_x3: arena too small");
+  launch_pdl(split_f16_rows_kernel, dim3((unsigned)N), dim3(256), (size_t)0, c->stream, W, K, hi, lo, wun);
   SpArgs g;
-  g.rexp = nullptr, g.wun = nullptr;   // operands converted as they are: see sra.cuh for the range this leaves the caller
+  g.rexp = nullptr, g.self_exp = 1, g.wun = wun;
   g.feats = A, g.lda = lda, g.Cin = K, g.nbr = nullptr, g.n_out = M_cap, g.n_dev = M_dev, g.KV = 1, g.Whi = hi, g.Wlo = lo, g.Cout = N;
   g.scale = nullptr, g.shift = bias, g.residual = res, g.ldr = ldr, g.act = act, g.out = out, g.ldo = ldo;
   return dispatch_spconv_wgmma(c, g, true);

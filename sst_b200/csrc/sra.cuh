@@ -11,9 +11,12 @@ void sstb_gemm_rows_ex(cudaStream_t st, const float* A, int lda, const float* W,
                        int act, const float* pos_tab, const int32_t* pos_code, int posL, int pos_maxw, int pos_ndim, int pos_ncols);
 // fp32-tolerance row GEMM on the tensor core (csrc/spconv.cu, split-fp16 operands): out = act(A . W^T + bias) + res.  Returns
 // SSTB_ERR_UNSUPPORTED (nothing launched) when the shape does not fit (K, N multiples of 64) - callers then use sstb_gemm_rows.
-// Operands are rounded to fp16 pairs as they are (no per-row / per-channel exponents, unlike sstb200_spconv_forward): the 2^-22
-// tolerance holds for |A|, |W| in about [2^-3, 65504] and degrades to an absolute 2^-25 per element below.  Its callers feed it
-// LayerNorm outputs, attention outputs and trained Linear weights, which sit in that range.
+// Each row of A and each output channel of W is lifted by a power of two to the top of fp16's range before it is split into an
+// fp16 pair (as in sstb200_spconv_forward), so the result is homogeneous in the scale of either operand: an element within 2^-16
+// of its row's (channel's) largest |value| keeps 22 significant bits, a smaller one an absolute error of 2^-38 of that largest,
+// at any magnitude fp32 holds.  Unscaled, the pair loses bits for every |x| below about 2^-3 - which is where nn.Linear's default
+// init (|w| <= 1 / sqrt(K)) and xavier's (|w| <= sqrt(6 / (K + N))) put the weights of an encoder layer, and where small
+// activation rows lie.
 int sstb_gemm_rows_x3(sstb200_ctx* c, const float* A, int lda, const float* W, const float* bias, const float* res, int ldr, float* out,
                       int ldo, int M_cap, const int32_t* M_dev, int N, int K, int act);
 void sstb_add_norm_act(cudaStream_t st, const float* a, const float* b, const float* gamma, const float* beta,

@@ -192,7 +192,8 @@ void sstb_add_norm(cudaStream_t st, const float* a, const float* b, const float*
 
 // ------------------------------------------------------------------------------------------------
 // fp32-tolerance GEMMs on the tensor core: every Linear of the layer runs through sstb_gemm_rows_x3 (split-fp16 operands:
-// hi.hi + lo.hi + hi.lo in one set of fp32 accumulators, ~2^-22 relative) instead of the FFMA kernel above; the positional term of
+// hi.hi + lo.hi + hi.lo in one set of fp32 accumulators, ~2^-22 relative at any operand scale, see sra.cuh) instead of the FFMA
+// kernel above; the positional term of
 // q|k is added to a copy of the input first.  Shapes sstb_gemm_rows_x3 does not take (d_model or dim_ff not a multiple of 64) run
 // on the FFMA kernel.
 // ------------------------------------------------------------------------------------------------
