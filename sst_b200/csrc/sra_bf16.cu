@@ -7,6 +7,10 @@
 // post-attention chain of csrc/sra_chain2.cu (out-projection + LN1 + FFN + LN2, in the encoder stack also the next layer's
 // QKV), so the stack takes 2 launches per layer.  fp32 stays the type of the residual stream, softmax, LayerNorm and all
 // accumulation.
+//
+// Range: every 16-bit operand is IEEE fp16, largest finite value 65504.  A q|k operand x + pos, a v operand x, or an
+// activation x1, h, y beyond it rounds to inf and the layer's output is no longer finite; inputs stay well inside it in the
+// models this path serves (normalised residual streams), and nothing here rescales them.
 #include <stdarg.h>
 #include <cuda_fp16.h>
 #include "sra.cuh"
@@ -48,7 +52,10 @@ int sstb_sra_layer_bf16(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb20
   const int d = L->d_model, ff = L->dim_ff;
   if (d != 128 || ff != 256 || !L->post_norm || L->norm1_mean || L->act != 2)
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED,
-                     "bf16 tensor-core path is built for d_model=128, dim_ff=256, post-norm LayerNorm, gelu (got d=%d ff=%d)", d, ff);
+                     "bf16 tensor-core path is built for d_model=128, dim_ff=256, post-norm LayerNorm, gelu (got d=%d ff=%d, %s, %s; "
+                     "BatchNorm runs in the fused stack only)",
+                     d, ff, !L->post_norm ? "pre-norm" : L->norm1_mean ? "post-norm BatchNorm" : "post-norm LayerNorm",
+                     L->act == 2 ? "gelu" : "relu");
   if (!L->in_proj_w_f16 || !L->out_proj_w_f16 || !L->lin1_w_f16 || !L->lin2_w_f16)
     return sstb_fail(c, SSTB_ERR_ARG, "the tensor-core path needs the *_w_f16 weight copies");
   if (P->pos_table && P->pos_L % 8 != 0)
@@ -59,8 +66,8 @@ int sstb_sra_layer_bf16(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb20
   // tensor-core attention path: plain scaled-dot-product, 8 heads x 16, windows <= 144 tokens
   const bool tc_attn = L->nhead == 8 && (!L->tau || L->tau_n == 1 || L->tau_n == 8) && P->max_window_tokens > 0 && P->max_window_tokens <= ATT_MAXT &&
                        P->num_windows_dev && P->win_batch;
-  // 1. QKV projection.  q/k/v for the tensor-core attention are written as fp16 (softmax logits need the mantissa: with bf16
-  // q,k the logit error dominates the layer's error budget); the SIMT fallback reads bf16.
+  // 1. QKV projection, fp16 q/k/v for either attention kernel (softmax logits need the mantissa: with bf16 q,k the logit error
+  // would dominate the layer's error budget).
   int rc = qkv_gemm(c, L, P, x, qkv, n_cap, n_dev, tc_attn);
   if (rc) return rc;
   // 2. ragged window attention (fp32 math on bf16 q/k/v)
