@@ -15,8 +15,8 @@
 // takes each group max with its arg-max row (launch_segment_reduce) - the backward is in sir_train.cu.
 #include <stdarg.h>
 #include "index.cuh"
+#include "rows.cuh"
 #include "sir.cuh"
-#include "sra.cuh"
 
 // ---- relation MLP + gating: one warp per point -----------------------------------------------------
 __global__ void __launch_bounds__(256) sir_rel_gate_kernel(RelDev r, const float* __restrict__ feats /*[N,cin]*/,
@@ -283,7 +283,9 @@ static int sir_forward_fp32(sstb200_ctx* c, const sstb200_sir_layer* L, const fl
   if (rc) return rc;
   // 2. layer 0: p0 = act(LN(W0 x0)); g0 = segmax(p0)
   CHECK_ARG(c, L->vfe_w[0] && L->vfe_ln_w[0] && L->vfe_ln_b[0]);
-  sstb_gemm_rows_ex(st, x0, cin, L->vfe_w[0], cin, nullptr, nullptr, 0, nullptr, t0, C0, N, nullptr, C0, cin, 0, nullptr, nullptr, 0, 0, 0, 0);
+  RowGemm g0{};
+  g0.A = x0, g0.lda = cin, g0.W = L->vfe_w[0], g0.out = t0, g0.ldo = C0, g0.M_cap = N, g0.N = C0, g0.K = cin;
+  sstb_row_gemm(st, g0);
   float* p0out = (C1 == 0) ? out_point : p0;
   sstb_add_norm_act(st, t0, nullptr, L->vfe_ln_w[0], L->vfe_ln_b[0], nullptr, nullptr, L->norm_eps, p0out, N, nullptr, C0, L->act);
   const int Cg = C0 + C1;
@@ -291,10 +293,12 @@ static int sir_forward_fp32(sstb200_ctx* c, const sstb200_sir_layer* L, const fl
   if (C1) {
     CHECK_ARG(c, L->vfe_w[1] && L->vfe_ln_w[1] && L->vfe_ln_b[1]);
     // 3. layer 1 on [p0 || g0[group]]:  W1a p0 + (W1b g0)[group]
-    sstb_gemm_rows_ex(st, out_group, Cg, L->vfe_w[1] + C0, 2 * C0, nullptr, nullptr, 0, nullptr, gterm, C1, G, nullptr, C1, C0, 0, nullptr,
-                      nullptr, 0, 0, 0, 0);
-    sstb_gemm_rows_ex(st, p0, C0, L->vfe_w[1], 2 * C0, nullptr, gterm, C1, inv, t1, C1, N, nullptr, C1, C0, 0, nullptr,
-                      nullptr, 0, 0, 0, 0);
+    RowGemm gw{}, pw{};
+    gw.A = out_group, gw.lda = Cg, gw.W = L->vfe_w[1] + C0, gw.ldw = 2 * C0, gw.out = gterm, gw.ldo = C1, gw.M_cap = G, gw.N = C1, gw.K = C0;
+    sstb_row_gemm(st, gw);
+    pw.A = p0, pw.lda = C0, pw.W = L->vfe_w[1], pw.ldw = 2 * C0, pw.res = gterm, pw.ldr = C1, pw.res_index = inv, pw.out = t1, pw.ldo = C1;
+    pw.M_cap = N, pw.N = C1, pw.K = C0;
+    sstb_row_gemm(st, pw);
     sstb_add_norm_act(st, t1, nullptr, L->vfe_ln_w[1], L->vfe_ln_b[1], nullptr, nullptr, L->norm_eps, out_point, N, nullptr, C1, L->act);
     sir_group_max(c, out_point, C1, off, order, inv, N, G, gord, gterm, s ? s->am1 : nullptr, out_group, Cg, C0);
   }

@@ -43,3 +43,5 @@ int sstb_sir_rel_gate(sstb200_ctx* c, const sstb200_sir_layer* L, const float* i
 int sstb_sir_group_csr(sstb200_ctx* c, const long long* inv, int N, int G, int32_t* offsets, int32_t* order);
 // the range the fp32 training path covers (SSTB_ERR_UNSUPPORTED / SSTB_ERR_ARG with a message otherwise)
 int sstb_sir_train_check(sstb200_ctx* c, const sstb200_sir_layer* L);
+// out[g, col0 + c] = the group max that ord[g, c] holds in order-preserving form (0, an empty group, gives 0)
+void sstb_sir_segmax_finalize(cudaStream_t st, const uint32_t* ord, int G, int C, float* out, int ldo, int col0);

@@ -13,7 +13,7 @@
 // The [N, 2*C0] concat of the reference is never formed; weights are converted to bf16 operands once per CTA.
 #include <stdarg.h>
 #include "index.cuh"
-#include "sra.cuh"
+#include "sir.cuh"
 #include "wgmma.cuh"
 
 namespace {

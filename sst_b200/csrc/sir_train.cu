@@ -14,8 +14,8 @@
 // once (a row belongs to one group).  Two calls on the same inputs give the same bits.
 #include <stdarg.h>
 #include "index.cuh"
+#include "rows.cuh"
 #include "sir.cuh"
-#include "sra.cuh"
 
 // ---- small helpers ---------------------------------------------------------------------------------
 // out[c, r] = W[r, c]   (W [rows, >= cols] with row pitch ldw)
@@ -524,8 +524,11 @@ extern "C" int sstb200_sir_layer_backward(sstb200_ctx* c, const sstb200_sir_laye
     sir_dw(c, dt1, C1, p0, C0, N, C1, C0, part, grads->vfe_w[1], 2 * C0);
     sir_dw(c, S1, C1, g0, C0, G, C1, C0, part, grads->vfe_w[1] + C0, 2 * C0);
     // into layer 0: dp0 = dt1 W1a, dg0 = S1 W1b + grad_group[:, :C0] at the arg-max rows
-    sstb_gemm_rows_ex(st, S1, C1, W1bt, C1, nullptr, grad_group, Cg, nullptr, dg0, C0, G, nullptr, C0, C1, 0, nullptr, nullptr, 0, 0, 0, 0);
-    sstb_gemm_rows_ex(st, dt1, C1, W1at, C1, nullptr, nullptr, 0, nullptr, dP0, C0, N, nullptr, C0, C1, 0, nullptr, nullptr, 0, 0, 0, 0);
+    RowGemm dg{}, dp{};
+    dg.A = S1, dg.lda = C1, dg.W = W1bt, dg.res = grad_group, dg.ldr = Cg, dg.out = dg0, dg.ldo = C0, dg.M_cap = G, dg.N = C0, dg.K = C1;
+    sstb_row_gemm(st, dg);
+    dp.A = dt1, dp.lda = C1, dp.W = W1at, dp.out = dP0, dp.ldo = C0, dp.M_cap = N, dp.N = C0, dp.K = C1;
+    sstb_row_gemm(st, dp);
     launch_pdl(sirb_scatter_max_kernel, blocks((size_t)G * C0), dim3(256), (size_t)0, st, (const long long*)s.am0, G, C0, (const float*)dg0, C0, 0, dP0, N);
   } else {
     if (grad_point) CUDA_TRY(c, cudaMemcpyAsync(dP0, grad_point, Nf * C0 * 4, cudaMemcpyDeviceToDevice, st));
@@ -536,7 +539,9 @@ extern "C" int sstb200_sir_layer_backward(sstb200_ctx* c, const sstb200_sir_laye
   // layer 0
   ln_bwd(s.t0, dP0, C0, 0, dt0);
   sir_dw(c, dt0, C0, x0, cin, N, C0, cin, part, grads->vfe_w[0], cin);
-  sstb_gemm_rows_ex(st, dt0, C0, W0t, C0, nullptr, nullptr, 0, nullptr, dx0, cin, N, nullptr, cin, C0, 0, nullptr, nullptr, 0, 0, 0, 0);
+  RowGemm dx{};
+  dx.A = dt0, dx.lda = C0, dx.W = W0t, dx.out = dx0, dx.ldo = cin, dx.M_cap = N, dx.N = cin, dx.K = C0;
+  sstb_row_gemm(st, dx);
 
   // gating + rel-MLP
   {

@@ -13,7 +13,7 @@
 #include <cuda_fp16.h>
 #include "index.cuh"
 #include "wgmma.cuh"
-#include "sra.cuh"
+#include "rows.cuh"
 
 namespace {
 
@@ -542,7 +542,7 @@ __global__ void __launch_bounds__(256, (NT == 64 && !SPLIT) ? 2 : 1) spconv_wgmm
   R0.valid = R1.valid = 0u;
   load_next(R0);
   load_next(R1);
-  if (SPLIT && g.self_exp) {   // GEMM mode (sstb_gemm_rows_x3), while the first two stages load: eight threads per row, 128
+  if (SPLIT && g.self_exp) {   // GEMM mode (sstb_row_gemm_x3), while the first two stages load: eight threads per row, 128
     // contiguous bytes per row and load
 #pragma unroll
     for (int u = 0; u < 4; u++) {
@@ -811,23 +811,24 @@ extern "C" int sstb200_spconv_forward(sstb200_ctx* c, const float* feats, int n_
   return dispatch_spconv_wgmma(c, g, precision == SSTB200_PREC_FP32_TC);
 }
 
-// fp32-tolerance row GEMM on the tensor core (used by the fp32 mode of the SRA encoder, csrc/sra_fp32.cu):
+// fp32-tolerance row GEMM on the tensor core (rows.cuh; the fp32 mode of the SRA encoder, csrc/sra_fp32.cu, runs on it):
 //   out[r, :N] = act(A[r, :K] . W[N, K]^T + bias) + res[r]      with every operand split into two fp16 numbers (see SPLIT above),
 // each row of A and each output channel of W first lifted to the top of fp16's range by its own power of two, as in
 // sstb200_spconv_forward: the result is homogeneous in the scale of either operand
-int sstb_gemm_rows_x3(sstb200_ctx* c, const float* A, int lda, const float* W, const float* bias, const float* res, int ldr, float* out,
-                      int ldo, int M_cap, const int32_t* M_dev, int N, int K, int act) {
-  if (M_cap <= 0) return SSTB_OK;
-  if ((K & 63) || (N & 63) || (lda & 3) || (ldo & 3) || (ldr & 3) || (act == 1 && res)) return SSTB_ERR_UNSUPPORTED;
+int sstb_row_gemm_x3(sstb200_ctx* c, const RowGemm& r) {
+  if (r.M_cap <= 0) return SSTB_OK;
+  const int N = r.N, K = r.K;
+  if ((K & 63) || (N & 63) || (r.lda & 3) || (r.ldo & 3) || (r.ldr & 3) || (r.act == 1 && r.res)) return SSTB_ERR_UNSUPPORTED;
+  if ((r.ldw && r.ldw != K) || r.res_index || r.pos.tab) return SSTB_ERR_UNSUPPORTED;   // forms only the FFMA row GEMM takes
   __half* hi = arena_alloc<__half>(c, (size_t)N * K);
   __half* lo = arena_alloc<__half>(c, (size_t)N * K);
   float* wun = arena_alloc<float>(c, (size_t)N);
-  if (!hi || !lo || !wun) return sstb_fail(c, SSTB_ERR_WORKSPACE, "gemm_rows_x3: arena too small");
-  launch_pdl(split_f16_rows_kernel, dim3((unsigned)N), dim3(256), (size_t)0, c->stream, W, K, hi, lo, wun);
+  if (!hi || !lo || !wun) return sstb_fail(c, SSTB_ERR_WORKSPACE, "row_gemm_x3: arena too small");
+  launch_pdl(split_f16_rows_kernel, dim3((unsigned)N), dim3(256), (size_t)0, c->stream, r.W, K, hi, lo, wun);
   SpArgs g;
   g.rexp = nullptr, g.self_exp = 1, g.wun = wun;
-  g.feats = A, g.lda = lda, g.Cin = K, g.nbr = nullptr, g.n_out = M_cap, g.n_dev = M_dev, g.KV = 1, g.Whi = hi, g.Wlo = lo, g.Cout = N;
-  g.scale = nullptr, g.shift = bias, g.residual = res, g.ldr = ldr, g.act = act, g.out = out, g.ldo = ldo;
+  g.feats = r.A, g.lda = r.lda, g.Cin = K, g.nbr = nullptr, g.n_out = r.M_cap, g.n_dev = r.M_dev, g.KV = 1, g.Whi = hi, g.Wlo = lo, g.Cout = N;
+  g.scale = nullptr, g.shift = r.bias, g.residual = r.res, g.ldr = r.ldr, g.act = r.act, g.out = r.out, g.ldo = r.ldo;
   return dispatch_spconv_wgmma(c, g, true);
 }
 

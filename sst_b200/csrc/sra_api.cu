@@ -1,5 +1,6 @@
 // C-ABI entry for the SRA encoder layer; dispatches on precision.
 #include <stdarg.h>
+#include "rows.cuh"
 #include "sra.cuh"
 
 extern "C" int sstb200_sra_layer_forward(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb200_sra_plan* P, const float* x,
@@ -25,7 +26,9 @@ extern "C" int sstb200_linear(sstb200_ctx* c, const float* A, const float* W, co
   CHECK_ARG(c, c && M >= 0 && N > 0 && K > 0 && act >= 0 && act <= 2);
   if (M == 0) return SSTB_OK;
   CHECK_ARG(c, A && W && out);
-  sstb_gemm_rows(c->stream, A, K, W, bias, nullptr, 0, out, N, M, nullptr, N, K, act, nullptr, nullptr, 0, 0, 0, 0);
+  RowGemm g{};
+  g.A = A, g.lda = K, g.W = W, g.bias = bias, g.out = out, g.ldo = N, g.M_cap = M, g.N = N, g.K = K, g.act = act;
+  sstb_row_gemm(c->stream, g);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }

@@ -7,7 +7,7 @@
 // registers - the per-point feature tensors are never materialised.
 #include <stdarg.h>
 #include "index.cuh"
-#include "sra.cuh"
+#include "rows.cuh"
 #include "wgmma.cuh"
 
 struct VfeDev {
@@ -727,14 +727,19 @@ static int vfe_wide_path(sstb200_ctx* c, const sstb200_vfe_cfg* cfg, const VfeDe
              vmean);
   launch_pdl(vfe_decorate_wide_kernel<TC, TM>, dim3((unsigned)(((size_t)P * 32 + 255) / 256)), dim3(256), (size_t)0, st, v, pts, coors, map,
              (const float*)vmean, P, X, row64);
-  sstb_gemm_rows_ex(st, X, D0, cfg->weight[0], D0, nullptr, nullptr, 0, nullptr, Y0, C0, P, nullptr, C0, D0, 0, nullptr, nullptr, 0, 0, 0, 0);
+  RowGemm g0{};
+  g0.A = X, g0.lda = D0, g0.W = cfg->weight[0], g0.out = Y0, g0.ldo = C0, g0.M_cap = P, g0.N = C0, g0.K = D0;
+  sstb_row_gemm(st, g0);
   sstb_add_norm_act(st, Y0, nullptr, cfg->bn_weight[0], cfg->bn_bias[0], cfg->bn_mean[0], cfg->bn_var[0], cfg->bn_eps, Y0, P, nullptr, C0, 1);
   launch_segment_reduce(c, Y0, C0, r.offsets, r.order, P, num_dev, mode, 0.f, C1 ? V0 : out_feats, nullptr, P);
   if (C1) {
-    sstb_gemm_rows_ex(st, V0, C0, cfg->weight[1] + C0, 2 * C0, nullptr, nullptr, 0, nullptr, G, C1, P, num_dev, C1, C0, 0, nullptr, nullptr, 0, 0,
-                      0, 0);
-    sstb_gemm_rows_ex(st, Y0, C0, cfg->weight[1], 2 * C0, nullptr, G, C1, (const long long*)row64, T1, C1, P, nullptr, C1, C0, 0, nullptr, nullptr,
-                      0, 0, 0, 0);
+    RowGemm gv{}, gy{};
+    gv.A = V0, gv.lda = C0, gv.W = cfg->weight[1] + C0, gv.ldw = 2 * C0, gv.out = G, gv.ldo = C1, gv.M_cap = P, gv.M_dev = num_dev;
+    gv.N = C1, gv.K = C0;
+    sstb_row_gemm(st, gv);
+    gy.A = Y0, gy.lda = C0, gy.W = cfg->weight[1], gy.ldw = 2 * C0, gy.res = G, gy.ldr = C1, gy.res_index = row64, gy.out = T1, gy.ldo = C1;
+    gy.M_cap = P, gy.N = C1, gy.K = C0;
+    sstb_row_gemm(st, gy);
     sstb_add_norm_act(st, T1, nullptr, cfg->bn_weight[1], cfg->bn_bias[1], cfg->bn_mean[1], cfg->bn_var[1], cfg->bn_eps, T1, P, nullptr, C1, 1);
     launch_segment_reduce(c, T1, C1, r.offsets, r.order, P, num_dev, mode, 0.f, out_feats, nullptr, P);
   }

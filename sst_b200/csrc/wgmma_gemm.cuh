@@ -11,7 +11,7 @@
 // exponent range, and forward + backward then share one set of saved activations).
 #pragma once
 #include <stdarg.h>
-#include "sra.cuh"
+#include "common.cuh"
 #include "wgmma.cuh"
 
 namespace {

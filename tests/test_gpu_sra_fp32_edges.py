@@ -3,12 +3,13 @@ count and operand scale.
 
 Each of the layer's five Linears (q|k, v or q|k|v, out_proj, linear1, linear2) runs on one of two GEMMs:
 
-    x3     sstb_gemm_rows_x3 (csrc/spconv.cu)   split-fp16 wgmma, K and N multiples of 64; NT 128 when N % 128 == 0, else NT 64;
-                                                 K / 64 stages; q|k gets its positional term from add_pos_kernel first
-    ffma   gemm_rows_kernel (csrc/sra_fp32.cu)   fp32 FFMA, any K and N; the q|k|v GEMM takes it whenever d_model or dim_ff is not a
-                                                 multiple of 64, with the positional term fused into its A loads (pos_ncols = 2 d)
+    x3     sstb_row_gemm_x3 (csrc/spconv.cu)   split-fp16 wgmma, K and N multiples of 64; NT 128 when N % 128 == 0, else NT 64;
+                                                K / 64 stages; q|k gets its positional term from add_pos_kernel first
+    ffma   gemm_rows_kernel (csrc/rows.cu)      fp32 FFMA, any K and N; the q|k|v GEMM takes it whenever d_model or dim_ff is not a
+                                                multiple of 64, with the positional term fused into its A loads (pos_ncols = 2 d)
 
-and the norms run on add_norm_kernel (post- or pre-norm, LayerNorm or eval BatchNorm, at most 8 values per lane: d_model <= 256).
+and the norms run on add_norm_kernel (csrc/rows.cu: post- or pre-norm, LayerNorm or eval BatchNorm, at most 8 values per lane:
+d_model <= 256).
 Every comparison is held to two bounds against the float64 oracle: the fp32 contract (max-norm, 1e-3 of the output's max-abs) and,
 per row, TIGHT of that row's max-abs (or 1e-3 of the output's max-abs, whichever is larger), so that an error confined to a few
 rows, columns or tile edges cannot hide in a max-norm over the frame.
@@ -71,7 +72,7 @@ VARIANTS = {
 # routes, mirrored from the dispatch of csrc/sra_fp32.cu and csrc/spconv.cu
 # ------------------------------------------------------------------------------------------------------------------------------
 def _x3(N, K):
-    """sstb_gemm_rows_x3's route for an [N, K] weight, or None when it refuses the shape (the FFMA kernel runs)."""
+    """sstb_row_gemm_x3's route for an [N, K] weight, or None when it refuses the shape (the FFMA kernel runs)."""
     if N % 64 or K % 64:
         return None
     return ("x3", 128 if N % 128 == 0 else 64, K // 64)
@@ -92,17 +93,24 @@ def family(d, ff):
     return "x3" if kinds == {"x3"} else "ffma" if "x3" not in kinds else "mixed"
 
 
-def test_route_matrix():
+def test_row_gemm_route_matrix():
     """CPU: the dispatch rules the route mirror restates are still the ones in the sources, and the shape matrix reaches every
     route the issue of each shape claims: both x3 tile widths, 1 / 2 / 3 / 4 / 5 / 8 stages, the fused-pos FFMA q|k|v beside x3
     GEMMs in one layer, FFMA with N and K tails, and d_model 256 (v[8] full)."""
     fp32 = open(os.path.join(ROOT, "sst_b200", "csrc", "sra_fp32.cu")).read()
     spc = open(os.path.join(ROOT, "sst_b200", "csrc", "spconv.cu")).read()
     assert "if (d % 64 == 0 && ff % 64 == 0) {" in fp32
-    assert "2 * d);" in fp32[fp32.index("sstb_gemm_rows(st, xin, d, L->in_proj_w"):][:260], "q|k|v FFMA: pos_ncols = 2 d"
+    qkv = fp32[fp32.index("} else {  // q|k|v in one FFMA GEMM"):]
+    qkv = qkv[:qkv.index("sstb_row_gemm(st, g);")]
+    assert "g.A = xin, g.lda = d, g.W = L->in_proj_w," in qkv and "g.N = 3 * d, g.K = d;" in qkv, "q|k|v in one FFMA GEMM"
+    assert "g.pos = pt, g.pos_ncols = 2 * d;" in qkv, "q|k|v FFMA: pos_ncols = 2 d"
+    assert "static int linear_fp32(sstb200_ctx* c, const RowGemm& g) {\n  const int rc = sstb_row_gemm_x3(c, g);" in fp32
     assert "if (d > 256 || d % 32)" in fp32
-    x3 = spc[spc.index("int sstb_gemm_rows_x3("):]
-    assert "if ((K & 63) || (N & 63)" in x3 and "dispatch_spconv_wgmma(c, g, true)" in x3
+    x3 = spc[spc.index("int sstb_row_gemm_x3("):]
+    x3 = x3[:x3.index("\n}\n")]
+    assert "if ((K & 63) || (N & 63) || (r.lda & 3) || (r.ldo & 3) || (r.ldr & 3) || (r.act == 1 && r.res))" in x3
+    assert "if ((r.ldw && r.ldw != K) || r.res_index || r.pos.tab) return SSTB_ERR_UNSUPPORTED;" in x3
+    assert "dispatch_spconv_wgmma(c, g, true)" in x3
     assert "if (g.Cout % 128 == 0) return launch_spconv_wgmma<128, 2, true>(c, g);" in spc
     for shape, fam in SHAPES.items():
         assert family(shape[0], shape[2]) == fam, shape
@@ -148,7 +156,7 @@ def _pow2_top(amax):
 
 
 def x3_emulated(a, w, scaled):
-    """out = a . w^T as sstb_gemm_rows_x3 forms it: each operand element split into hi = fp16(x), lo = fp16(x - hi) (after the
+    """out = a . w^T as sstb_row_gemm_x3 forms it: each operand element split into hi = fp16(x), lo = fp16(x - hi) (after the
     row's / output channel's power of two when `scaled`), the three products hi.hi + lo.hi + hi.lo summed exactly (float64)."""
     a, w = a.astype(np.float32), w.astype(np.float32)
     ea = _pow2_top(np.abs(a).max(1)) if scaled else np.zeros(a.shape[0])
@@ -171,7 +179,7 @@ def _row_err(got, ref):
 
 def test_x3_split_operand_scale_emulated():
     """CPU: the rounding of the x3 GEMM's operands on the scale cases of test_operand_scale.  With each row of A and each output
-    channel of W lifted to the top of fp16's range (what sstb_gemm_rows_x3 does), the split keeps every row of A . W^T within
+    channel of W lifted to the top of fp16's range (what sstb_row_gemm_x3 does), the split keeps every row of A . W^T within
     2^-20 of its max-abs at every scale - 22 bits per element, accumulated over K.  Converted as they are, the pair has no
     normal fp16 residue below about 2^-3, where the weights of an encoder layer lie (xavier: |w| <= 0.18 for these shapes):
     activations x 2^-8 and below and any weight matrix x 2^-6 leave that bound, and from 2^-12 on (or w x 2^-6) the layer's
