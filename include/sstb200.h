@@ -626,6 +626,59 @@ int sstb200_dcn_backward(sstb200_ctx* ctx, const int32_t geom[15], const float* 
                          const float* grad_y, void* workspace, int64_t workspace_bytes, float* grad_x, float* grad_offset,
                          float* grad_weight);
 
+/* ---- CenterHead training (mmdet3d/models/dense_heads/centerpoint_head.py:421-610), fp32, stream-ordered, no sync.
+ *
+ * sstb200_centerpoint_targets: CenterHead.get_targets for the whole batch and every task in three launches.
+ *   boxes [N, box_dim] gravity-centred (x, y, z, dx, dy, dz, yaw[, vx, vy]), box_dim 7 or 9, labels int64 [N], the samples' boxes
+ *   concatenated: sample b owns rows [sample_offsets[b], sample_offsets[b + 1]) (host, batch + 1 entries, sample_offsets[0] = 0).
+ *   Task t owns the labels [task_label_offsets[t], task_label_offsets[t + 1]) (host, num_tasks + 1 entries, each range non-empty);
+ *   other labels are ignored.  Geometry: pc_min (x, y), voxel_size (x, y), out_size_factor, the feature map width x height,
+ *   gaussian_overlap, min_radius, max_objs, norm_bbox.  Outputs per task t (host arrays of num_tasks device pointers), fully written:
+ *     heatmaps[t] f32 [batch, ncls_t, height, width], anno_boxes[t] f32 [batch, max_objs, 10], inds[t] int64 [batch, max_objs],
+ *     masks[t] uint8 [batch, max_objs].
+ *   A task's boxes take slots ordered by class within the task, then by input row; only the first max_objs are considered.  A box is
+ *   skipped (its slot keeps ind 0, mask 0, anno_box 0) when dx / vx / osf <= 0 or dy / vy / osf <= 0 or trunc((x - pc_min) / voxel /
+ *   osf) lies outside the map; every quantity is the reference's sequence of correctly rounded fp32 operations (gaussian_radius with
+ *   the Python scalars 1 - o, 1 + o, -2 o, o - 1 and 4 (4 o) rounded to fp32), radius = max(min_radius, trunc(min(r1, r2, r3))).
+ *   ind = cy * width + cx, anno_box = (x_map - cx, y_map - cy, z, log(dims) or dims, sin(yaw), cos(yaw), vx, vy), zeros for 7-dim boxes.
+ *   The heatmap is the max over the drawn boxes of fp32(exp(-(dx^2 + dy^2) / (2 sigma^2))) in double, sigma = (2 r + 1) / 6, over the
+ *   window clipped to the map; two calls give bit-identical results.  Temporaries (16 bytes per slot) from the context arena.
+ *   Errors: box_dim not 7 or 9, a size < 1, non-monotone offsets, an empty task range, a NULL pointer (SSTB_ERR_ARG); more than 256
+ *   samples or 16 tasks, height * width or batch * num_tasks * max_objs reaching 2^31 (SSTB_ERR_UNSUPPORTED).
+ *
+ * sstb200_gaussian_focal_loss_forward: mmdet 2.14 GaussianFocalLoss (alpha 2, gamma 4, reduction 'mean') on p = clamp(sigmoid(logits),
+ *   1e-4, 1 - 1e-4) against target, both [n]: *loss = loss_weight * sum / max(num_pos, 1), *num_pos = the number of targets equal to 1
+ *   (both device f32 scalars).  Block partials in double, then one block sums them in a fixed order: deterministic.  Two launches,
+ *   partials from the context arena.
+ * sstb200_gaussian_focal_loss_backward: grad_logits [n] = grad_loss[0] * loss_weight / max(num_pos[0], 1) * d loss / d logit, recomputed
+ *   from (logits, target); the clamp passes the gradient where the sigmoid lies within its bounds inclusive (as torch.clamp).  One launch.
+ *   Errors (both): n < 1 or a NULL pointer (SSTB_ERR_ARG).
+ *
+ * sstb200_centerpoint_l1_loss_forward: mmdet 2.14 L1Loss (reduction 'mean') of CenterHead.loss: heads = (reg [B, 2, H, W], height
+ *   [B, 1, H, W], dim [B, 3, H, W], rot [B, 2, H, W], vel [B, 2, H, W]) read in place at ind, against anno_box [B, max_objs, 10], weight
+ *   mask * (target not NaN) * code_weights[c]; *loss = loss_weight * sum(|pred - target| weight) / (sum(mask) + 1e-4) (device f32,
+ *   avg factor in fp32 on the device).  An ind outside [0, H W) of a masked slot makes the loss NaN.  One launch.
+ * sstb200_centerpoint_l1_loss_backward: grad_heads (same shapes as heads) fully written: zero, except at each masked cell the sum over
+ *   the slots gathering it, in slot order, of grad_loss[0] * loss_weight / avg * weight * sign(pred - target).  No float atomics, two
+ *   calls give bit-identical results.  Two launches.
+ *   Errors (both): a size < 1 or a NULL pointer (SSTB_ERR_ARG); max_objs above 4096 (SSTB_ERR_UNSUPPORTED). */
+int sstb200_centerpoint_targets(sstb200_ctx* ctx, const float* boxes, const int64_t* labels, int box_dim, const int32_t* sample_offsets,
+                                int batch, const int32_t* task_label_offsets, int num_tasks, const float pc_min[2],
+                                const float voxel_size[2], int out_size_factor, int width, int height, double gaussian_overlap,
+                                int min_radius, int max_objs, int norm_bbox, float* const* heatmaps, float* const* anno_boxes,
+                                int64_t* const* inds, uint8_t* const* masks);
+int sstb200_gaussian_focal_loss_forward(sstb200_ctx* ctx, const float* logits, const float* target, int64_t n, float loss_weight,
+                                        float* loss, float* num_pos);
+int sstb200_gaussian_focal_loss_backward(sstb200_ctx* ctx, const float* logits, const float* target, int64_t n, float loss_weight,
+                                         const float* num_pos, const float* grad_loss, float* grad_logits);
+int sstb200_centerpoint_l1_loss_forward(sstb200_ctx* ctx, const float* const heads[5], int batch, int height, int width,
+                                        const float* anno_box, const int64_t* ind, const uint8_t* mask, int max_objs,
+                                        const float code_weights[10], float loss_weight, float* loss);
+int sstb200_centerpoint_l1_loss_backward(sstb200_ctx* ctx, const float* const heads[5], int batch, int height, int width,
+                                         const float* anno_box, const int64_t* ind, const uint8_t* mask, int max_objs,
+                                         const float code_weights[10], float loss_weight, const float* grad_loss,
+                                         float* const grad_heads[5]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1046,3 +1046,166 @@ def deform_conv2d(input, offset, weight, stride=1, padding=0, dilation=1, groups
     """mmcv.ops.deform_conv2d: fp32 NCHW input [N, Cin, H, W], offset [N, 2 dg kh kw, Ho, Wo], weight [Cout, Cin / groups, kh, kw] ->
     [N, Cout, Ho, Wo].  im2col_step is accepted and ignored (one launch covers the batch)."""
     return DeformConv2dFunction.apply(input, offset, weight, stride, padding, dilation, groups, deform_groups, bias, im2col_step)
+
+
+# ----------------------------------------------------------------------------------------------
+# CenterHead training (mmdet3d/models/dense_heads/centerpoint_head.py:421-610)
+# ----------------------------------------------------------------------------------------------
+_PP = C.POINTER(C.c_void_p)
+L.SIGNATURES["sstb200_centerpoint_targets"] = (C.c_int, [L.vp, L.vp, L.vp, C.c_int, L.P_i32, C.c_int, L.P_i32, C.c_int, L.P_f32, L.P_f32,
+                                                         C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.c_int, _PP, _PP, _PP,
+                                                         _PP])
+L.SIGNATURES["sstb200_gaussian_focal_loss_forward"] = (C.c_int, [L.vp, L.vp, L.vp, C.c_int64, C.c_float, L.vp, L.vp])
+L.SIGNATURES["sstb200_gaussian_focal_loss_backward"] = (C.c_int, [L.vp, L.vp, L.vp, C.c_int64, C.c_float, L.vp, L.vp, L.vp])
+L.SIGNATURES["sstb200_centerpoint_l1_loss_forward"] = (C.c_int, [L.vp, _PP, C.c_int, C.c_int, C.c_int, L.vp, L.vp, L.vp, C.c_int, L.P_f32,
+                                                                 C.c_float, L.vp])
+L.SIGNATURES["sstb200_centerpoint_l1_loss_backward"] = (C.c_int, [L.vp, _PP, C.c_int, C.c_int, C.c_int, L.vp, L.vp, L.vp, C.c_int, L.P_f32,
+                                                                  C.c_float, L.vp, _PP])
+
+CENTERPOINT_HEADS = (("reg", 2), ("height", 1), ("dim", 3), ("rot", 2), ("vel", 2))
+
+
+def _ptrs(ts):
+    return (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+
+def _fp32_cuda(name, t, dim=None):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise L.SSTB200Error(f"{name} must be a CUDA tensor (there is no CPU path)")
+    if t.dtype == torch.float16:                       # @force_fp32 casts half predictions
+        t = t.float()
+    if t.dtype != torch.float32:
+        raise L.SSTB200Error(f"{name} must be float32, got {t.dtype}")
+    if dim is not None and t.dim() != dim:
+        raise L.SSTB200Error(f"{name} must be {dim}-d, got shape {tuple(t.shape)}")
+    return t.contiguous()
+
+
+def centerpoint_targets(boxes, labels, sample_sizes, task_num_classes, pc_min, voxel_size, out_size_factor, feature_map_size,
+                        gaussian_overlap, min_radius, max_objs, norm_bbox=True):
+    """CenterHead.get_targets for the whole batch: boxes [N, 7|9] fp32 gravity-centred, labels int64 [N], the samples' boxes
+    concatenated (sample_sizes: host ints, one per sample); task_num_classes: classes per task (task t owns the labels after those of the
+    tasks before it); feature_map_size = (W, H) = grid_size[:2] // out_size_factor.  Returns four lists over tasks, the reference's
+    shapes and dtypes: heatmap [B, ncls, H, W] f32, anno_box [B, max_objs, 10] f32, ind [B, max_objs] int64, mask [B, max_objs] uint8.
+    No host sync; bit-identical from run to run."""
+    if not isinstance(boxes, torch.Tensor) or not boxes.is_cuda or not isinstance(labels, torch.Tensor) or not labels.is_cuda:
+        raise L.SSTB200Error("centerpoint_targets: boxes and labels must be CUDA tensors (there is no CPU path)")
+    if boxes.dtype != torch.float32:
+        raise L.SSTB200Error(f"centerpoint_targets: boxes must be float32, got {boxes.dtype}")
+    if boxes.dim() != 2 or boxes.shape[1] not in (7, 9):
+        raise L.SSTB200Error(f"centerpoint_targets: boxes must be [N, 7] or [N, 9], got {tuple(boxes.shape)}")
+    if labels.dim() != 1 or labels.shape[0] != boxes.shape[0]:
+        raise L.SSTB200Error(f"centerpoint_targets: labels {tuple(labels.shape)} do not match boxes {tuple(boxes.shape)}")
+    sizes = [int(n) for n in sample_sizes]
+    if sum(sizes) != boxes.shape[0] or min(sizes, default=-1) < 0:
+        raise L.SSTB200Error(f"centerpoint_targets: sample sizes {sizes} do not add up to the {boxes.shape[0]} boxes")
+    W, H = (int(v) for v in feature_map_size)
+    B, dev = len(sizes), boxes.device
+    boxes, labels = boxes.contiguous(), labels.long().contiguous()
+    offsets, task_off = [0], [0]
+    for n in sizes:
+        offsets.append(offsets[-1] + n)
+    for n in task_num_classes:
+        task_off.append(task_off[-1] + int(n))
+    hm = [torch.empty((B, int(n), H, W), dtype=torch.float32, device=dev) for n in task_num_classes]
+    ab = [torch.empty((B, max_objs, 10), dtype=torch.float32, device=dev) for _ in task_num_classes]
+    ind = [torch.empty((B, max_objs), dtype=torch.int64, device=dev) for _ in task_num_classes]
+    mask = [torch.empty((B, max_objs), dtype=torch.uint8, device=dev) for _ in task_num_classes]
+    c = L.ctx(dev)
+    L.check(c, L.lib().sstb200_centerpoint_targets(
+        c, L.ptr(boxes) if boxes.numel() else None, L.ptr(labels) if labels.numel() else None, boxes.shape[1],
+        L.arr(C.c_int32, offsets), B, L.arr(C.c_int32, task_off), len(task_off) - 1, L.arr(C.c_float, [float(v) for v in pc_min[:2]]),
+        L.arr(C.c_float, [float(v) for v in voxel_size[:2]]), int(out_size_factor), W, H, float(gaussian_overlap), int(min_radius),
+        int(max_objs), int(bool(norm_bbox)), _ptrs(hm), _ptrs(ab), _ptrs(ind), _ptrs(mask)))
+    return hm, ab, ind, mask
+
+
+class GaussianFocalLossFunction(Function):
+    """mmdet 2.14 GaussianFocalLoss (alpha 2, gamma 4, reduction 'mean', avg_factor = max(num_pos, 1)) on clip_sigmoid(logits): returns
+    (loss, num_pos), both fp32 device scalars, num_pos = the number of target elements equal to 1.  Saves only the two inputs; the
+    backward recomputes the per-element derivative."""
+
+    @staticmethod
+    def forward(ctx, logits, target, loss_weight=1.0):
+        x, t = _fp32_cuda("logits", logits), _fp32_cuda("target", target)
+        if x.shape != t.shape or x.numel() == 0:
+            raise L.SSTB200Error(f"gaussian_focal_loss: logits {tuple(x.shape)} and target {tuple(t.shape)} must be one non-empty shape")
+        loss = torch.empty((), dtype=torch.float32, device=x.device)
+        num_pos = torch.empty((), dtype=torch.float32, device=x.device)
+        c = L.ctx(x.device)
+        L.check(c, L.lib().sstb200_gaussian_focal_loss_forward(c, L.ptr(x), L.ptr(t), x.numel(), float(loss_weight), L.ptr(loss),
+                                                               L.ptr(num_pos)))
+        ctx.save_for_backward(x, t, num_pos)
+        ctx.loss_weight, ctx.in_dtype = float(loss_weight), logits.dtype
+        ctx.mark_non_differentiable(num_pos)
+        return loss, num_pos
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_num_pos=None):
+        x, t, num_pos = ctx.saved_tensors
+        g = torch.empty_like(x)
+        gl = grad_loss.float().contiguous()
+        c = L.ctx(x.device)
+        L.check(c, L.lib().sstb200_gaussian_focal_loss_backward(c, L.ptr(x), L.ptr(t), x.numel(), ctx.loss_weight, L.ptr(num_pos), L.ptr(gl),
+                                                                L.ptr(g)))
+        return g.to(ctx.in_dtype), None, None
+
+
+def gaussian_focal_loss(logits, target, loss_weight=1.0):
+    """(loss, num_pos) of GaussianFocalLossFunction"""
+    return GaussianFocalLossFunction.apply(logits, target, loss_weight)
+
+
+def _l1_geom(heads, anno_box, ind, mask):
+    if len(heads) != 5:
+        raise L.SSTB200Error("centerpoint_l1_loss: five heads (reg, height, dim, rot, vel) are needed")
+    hs = [_fp32_cuda(name, h, 4) for (name, _), h in zip(CENTERPOINT_HEADS, heads)]
+    B, _, H, W = hs[0].shape
+    for (name, ch), h in zip(CENTERPOINT_HEADS, hs):
+        if tuple(h.shape) != (B, ch, H, W):
+            raise L.SSTB200Error(f"centerpoint_l1_loss: {name} must be {(B, ch, H, W)}, got {tuple(h.shape)}")
+    ab = _fp32_cuda("anno_box", anno_box, 3)
+    M = ab.shape[1]
+    if tuple(ab.shape) != (B, M, 10) or tuple(ind.shape) != (B, M) or tuple(mask.shape) != (B, M):
+        raise L.SSTB200Error(f"centerpoint_l1_loss: anno_box {tuple(ab.shape)}, ind {tuple(ind.shape)} and mask {tuple(mask.shape)} do "
+                             f"not fit [{B}, max_objs, 10] / [{B}, max_objs]")
+    if not ind.is_cuda or not mask.is_cuda or ind.dtype != torch.int64 or mask.dtype not in (torch.uint8, torch.bool):
+        raise L.SSTB200Error("centerpoint_l1_loss: ind must be int64 and mask uint8, on the GPU")
+    return hs, ab, ind.contiguous(), mask.contiguous().view(torch.uint8), (B, H, W, M)
+
+
+class CenterPointL1LossFunction(Function):
+    """CenterHead.loss's regression term: mmdet 2.14 L1Loss (reduction 'mean') of anno_box [B, M, 10] against the five heads gathered
+    at ind, weight mask * (target not NaN) * code_weights, avg_factor = sum(mask) + 1e-4 on the device.  The heads are read in place;
+    the backward writes their dense gradients with each cell's objects summed in slot order (deterministic, no float atomics)."""
+
+    @staticmethod
+    def forward(ctx, anno_box, ind, mask, code_weights, loss_weight, *heads):
+        hs, ab, ind, mask, (B, H, W, M) = _l1_geom(heads, anno_box, ind, mask)
+        cw = L.arr(C.c_float, [float(v) for v in code_weights])
+        if len(cw) != 10:
+            raise L.SSTB200Error(f"centerpoint_l1_loss: 10 code weights are needed, got {len(cw)}")
+        loss = torch.empty((), dtype=torch.float32, device=ab.device)
+        c = L.ctx(ab.device)
+        L.check(c, L.lib().sstb200_centerpoint_l1_loss_forward(c, _ptrs(hs), B, H, W, L.ptr(ab), L.ptr(ind), L.ptr(mask), M, cw,
+                                                               float(loss_weight), L.ptr(loss)))
+        ctx.save_for_backward(ab, ind, mask, *hs)
+        ctx.cfg = (list(code_weights), float(loss_weight), [h.dtype for h in heads])
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        ab, ind, mask, *hs = ctx.saved_tensors
+        code_weights, loss_weight, dtypes = ctx.cfg
+        B, _, H, W = hs[0].shape
+        grads = [torch.empty_like(h) for h in hs]
+        gl = grad_loss.float().contiguous()
+        c = L.ctx(ab.device)
+        L.check(c, L.lib().sstb200_centerpoint_l1_loss_backward(c, _ptrs(hs), B, H, W, L.ptr(ab), L.ptr(ind), L.ptr(mask), ab.shape[1],
+                                                                L.arr(C.c_float, code_weights), loss_weight, L.ptr(gl), _ptrs(grads)))
+        return (None, None, None, None, None) + tuple(g.to(d) for g, d in zip(grads, dtypes))
+
+
+def centerpoint_l1_loss(preds, anno_box, ind, mask, code_weights, loss_weight=1.0):
+    """preds: a dict with 'reg', 'height', 'dim', 'rot', 'vel' [B, C, H, W] -> the loss (fp32 device scalar)"""
+    return CenterPointL1LossFunction.apply(anno_box, ind, mask, code_weights, loss_weight, *[preds[k] for k, _ in CENTERPOINT_HEADS])
