@@ -100,8 +100,10 @@ int sstb200_unique_rows_i64(sstb200_ctx* ctx, const int64_t* coors, int num_rows
                             int32_t* num_unique_host);
 
 /* V5b torch_scatter.scatter(src, index, dim=0, reduce=sum|mean) / scatter_max (sst_ops.py:173-175).
- *     src [P,C] fp32, index [P] int64 in [0,num_segments), out [num_segments,C] (empty segments: 0).
- *     argmax (int64 [num_segments,C], may be NULL): lowest row attaining the max, P if empty. */
+ *     src [P,C] fp32, index [P] int64, out [num_segments,C] (empty segments: 0).
+ *     argmax (int64 [num_segments,C], may be NULL): lowest row attaining the max, P if empty.
+ *     Rows whose index lies outside [0, num_segments) are dropped: they count towards no segment (nor a mean's divisor).  The call
+ *     does not report them (it makes no host sync). */
 int sstb200_segment_reduce(sstb200_ctx* ctx, const float* src, const int64_t* index, int num_rows,
                            int num_feats, int num_segments, int reduce_type, float* out, int64_t* argmax);
 

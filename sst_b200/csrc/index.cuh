@@ -208,17 +208,20 @@ __global__ void map_count_kernel(const long long* __restrict__ keys, int n, cons
 }
 
 // ---- CSR fill (counting sort, order inside a segment unspecified) -----------------------------------------
+// Rows mapped outside [0, nseg) are skipped: offsets[] holds only nseg + 1 scanned entries, so such a row has no slot in `order`.
+// Maps built by the bitmap rank never leave that range; a caller's segment index (sstb200_segment_reduce) can.
 template <typename TM>
-__global__ void csr_fill_kernel(const TM* __restrict__ map, int n, const uint32_t* __restrict__ offsets,
-                                int32_t* __restrict__ cursor, int32_t* __restrict__ order,
+__global__ void csr_fill_kernel(const TM* __restrict__ map, int n, int nseg_host, const int32_t* __restrict__ nseg_dev,
+                                const uint32_t* __restrict__ offsets, int32_t* __restrict__ cursor, int32_t* __restrict__ order,
                                 const int32_t* __restrict__ n_dev = nullptr) {
   pdl_wait();
   pdl_launch();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (n_dev) n = *n_dev;
   if (i >= n) return;
+  const int nseg = nseg_dev ? *nseg_dev : nseg_host;
   long long v = (long long)map[i];
-  if (v < 0) return;
+  if (v < 0 || v >= nseg) return;
   int pos = atomicAdd(&cursor[v], 1);
   order[offsets[v] + pos] = i;
 }
@@ -307,7 +310,8 @@ __global__ void __launch_bounds__(256) segment_reduce_kernel(const float* __rest
         out[(size_t)s * C + c] = m;
         if (argmax) argmax[(size_t)s * C + c] = am;
       } else {
-        // fp64 accumulation: exact for these magnitudes, so the result does not depend on CSR order
+        // fp64 accumulation: exact while a segment's values span less than about 2^29 in magnitude, and only then is the result
+        // independent of the CSR order (a wider span can round a partial sum, and the order of those roundings varies)
         double acc = 0.0;
         for (uint32_t k = b; k < e; k++) acc += (double)src[(size_t)order[k] * ld + c];
         float r = (float)acc;
@@ -321,7 +325,7 @@ __global__ void __launch_bounds__(256) segment_reduce_kernel(const float* __rest
 // Vector variant (C % 4 == 0, 16-B aligned rows): GROUP lanes own one segment, each lane owns float4 channel groups
 // lane, lane+GROUP, ... (NV4 of them, C = 4*GROUP*NV4 at most), and FOUR points are in flight per lane (independent index and row
 // loads) - a 128-channel row is one 512-B warp transaction.  Same arithmetic as the scalar kernel (max with lowest-index tie
-// break for argmax; sum/mean in fp64, so independent of the CSR order).
+// break for argmax; sum/mean in fp64, independent of the CSR order while a segment's values span less than about 2^29).
 template <int GROUP, int NV4, bool ARG>
 __global__ void __launch_bounds__(256) segment_reduce_v4_kernel(const float* __restrict__ src, int C,
                                                                 const uint32_t* __restrict__ offsets,
@@ -397,7 +401,8 @@ __global__ void __launch_bounds__(256) segment_reduce_v4_kernel(const float* __r
             }
           }
         } else {
-          // fp64 accumulation: exact for these magnitudes, so the result does not depend on the CSR order
+          // fp64 accumulation: exact while a segment's values span less than about 2^29 in magnitude, and only then is the
+          // result independent of the CSR order (see segment_reduce_kernel)
 #pragma unroll
           for (int u = 0; u < RIF; u++)
 #pragma unroll
@@ -500,7 +505,8 @@ static int csr_build(sstb200_ctx* c, Csr& r, const TM* map, int n, const int32_t
     launch_pdl(csr_fill_small_kernel<TM>, dim3((n + CSR_SMALL_ITEMS - 1) / CSR_SMALL_ITEMS), dim3(1024), (size_t)small_nseg * 8, c->stream, map, n, small_nseg,
                (const uint32_t*)r.offsets, r.cursor, r.order);
   else if (n > 0)
-    launch_pdl(csr_fill_kernel<TM>, dim3((n + 255) / 256), dim3(256), (size_t)(0), c->stream, map, n, r.offsets, r.cursor, r.order, n_dev);
+    launch_pdl(csr_fill_kernel<TM>, dim3((n + 255) / 256), dim3(256), (size_t)(0), c->stream, map, n, (int)nseg_cap, nseg_dev,
+               (const uint32_t*)r.offsets, r.cursor, r.order, n_dev);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }

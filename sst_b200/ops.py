@@ -289,16 +289,21 @@ class _SegmentReduce(Function):
             gs = g.new_zeros((ctx.P + 1, g.shape[1]))
             gs.scatter_(0, arg, g)
             return gs[:ctx.P], None, None, None, None
-        gv = g[index]
+        # rows the forward dropped (index outside [0, num_segments)) read the appended zero row
+        n = g.shape[0]
+        index = torch.where((index >= 0) & (index < n), index, n)
+        gv = torch.cat([g, g.new_zeros((1, g.shape[1]))])[index]
         if ctx.mode == "mean":
-            cnt = torch.bincount(index, minlength=g.shape[0]).clamp(min=1)
+            cnt = torch.bincount(index, minlength=n + 1).clamp(min=1)
             gv = gv / cnt[index][:, None].to(g.dtype)
         return gv, None, None, None, None
 
 
 def segment_reduce(src, index, mode, num_segments=None, want_argmax=True):
     """torch_scatter.scatter(src, index, dim=0, reduce=mode) / scatter_max -> (out, argmax or None).  `want_argmax=False`
-    skips the argmax output of 'max' (only valid when no gradient is needed): the kernel then runs one FMNMX per element."""
+    skips the argmax output of 'max' (only valid when no gradient is needed): the kernel then runs one FMNMX per element.
+    Rows whose index lies outside [0, num_segments) are dropped, forward and backward (their gradient is 0); nothing reports them,
+    since that would need a host sync."""
     if num_segments is None:
         num_segments = int(index.max()) + 1 if index.numel() else 0
     if mode == "max" and not want_argmax and src.requires_grad and torch.is_grad_enabled():
