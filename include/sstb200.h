@@ -650,19 +650,21 @@ int sstb200_dcn_backward(sstb200_ctx* ctx, const int32_t geom[15], const float* 
  *
  * sstb200_gaussian_focal_loss_forward: mmdet 2.14 GaussianFocalLoss (alpha 2, gamma 4, reduction 'mean') on p = clamp(sigmoid(logits),
  *   1e-4, 1 - 1e-4) against target, both [n]: *loss = loss_weight * sum / max(num_pos, 1), *num_pos = the number of targets equal to 1
- *   (both device f32 scalars).  Block partials in double, then one block sums them in a fixed order: deterministic.  Two launches,
- *   partials from the context arena.
+ *   (both device f32 scalars).  The clamp keeps NaN, as torch.clamp does: a NaN logit makes the loss NaN.  Block partials in double,
+ *   then one block sums them in a fixed order: deterministic.  Two launches, partials from the context arena.
  * sstb200_gaussian_focal_loss_backward: grad_logits [n] = grad_loss[0] * loss_weight / max(num_pos[0], 1) * d loss / d logit, recomputed
- *   from (logits, target); the clamp passes the gradient where the sigmoid lies within its bounds inclusive (as torch.clamp).  One launch.
+ *   from (logits, target); the clamp passes the gradient where the sigmoid lies within its bounds inclusive (as torch.clamp), and a
+ *   NaN logit gets a NaN gradient.  One launch.
  *   Errors (both): n < 1 or a NULL pointer (SSTB_ERR_ARG).
  *
  * sstb200_centerpoint_l1_loss_forward: mmdet 2.14 L1Loss (reduction 'mean') of CenterHead.loss: heads = (reg [B, 2, H, W], height
  *   [B, 1, H, W], dim [B, 3, H, W], rot [B, 2, H, W], vel [B, 2, H, W]) read in place at ind, against anno_box [B, max_objs, 10], weight
  *   mask * (target not NaN) * code_weights[c]; *loss = loss_weight * sum(|pred - target| weight) / (sum(mask) + 1e-4) (device f32,
- *   avg factor in fp32 on the device).  An ind outside [0, H W) of a masked slot makes the loss NaN.  One launch.
+ *   avg factor in fp32 on the device).  Every slot is gathered, as in the reference: a masked-out slot adds |pred - target| * 0, so a
+ *   NaN prediction at its ind, or an ind outside [0, H W) of any slot, makes the loss NaN; a NaN target does too.  One launch.
  * sstb200_centerpoint_l1_loss_backward: grad_heads (same shapes as heads) fully written: zero, except at each masked cell the sum over
- *   the slots gathering it, in slot order, of grad_loss[0] * loss_weight / avg * weight * sign(pred - target).  No float atomics, two
- *   calls give bit-identical results.  Two launches.
+ *   the slots gathering it, in slot order, of grad_loss[0] * loss_weight / avg * weight * sign(pred - target) (0 for a NaN target or
+ *   a NaN difference, as torch.sign).  No float atomics, two calls give bit-identical results.  Two launches.
  *   Errors (both): a size < 1 or a NULL pointer (SSTB_ERR_ARG); max_objs above 4096 (SSTB_ERR_UNSUPPORTED). */
 int sstb200_centerpoint_targets(sstb200_ctx* ctx, const float* boxes, const int64_t* labels, int box_dim, const int32_t* sample_offsets,
                                 int batch, const int32_t* task_label_offsets, int num_tasks, const float pc_min[2],

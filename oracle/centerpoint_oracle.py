@@ -42,9 +42,34 @@ NUSC = dict(tasks=[1, 2, 2, 1, 2, 2], train_cfg=dict(grid_size=[512, 512, 1], po
 GEOMETRIES = {"waymo": WAYMO, "nusc": NUSC}
 
 
+def geometry(width, height, out_size_factor=1, voxel_size=(0.32, 0.32), gaussian_overlap=0.1, min_radius=2, max_objs=500, tasks=(3,),
+             box_dim=7):
+    """a GEOMETRIES-style dict for a width x height feature map (grid_size = map * out_size_factor), the point-cloud range centred on
+    the origin; the rest as WAYMO, with the code weights of NUSC (none zero)"""
+    vx, vy = voxel_size
+    gx, gy = width * out_size_factor, height * out_size_factor
+    pc = [-0.5 * gx * vx, -0.5 * gy * vy, -2.0, 0.5 * gx * vx, 0.5 * gy * vy, 4.0]
+    return dict(tasks=list(tasks), box_dim=box_dim, loss_bbox_weight=2.0,
+                train_cfg=dict(grid_size=[gx, gy, 1], voxel_size=(vx, vy, 6), out_size_factor=out_size_factor, dense_reg=1,
+                               gaussian_overlap=gaussian_overlap, max_objs=max_objs, min_radius=min_radius, point_cloud_range=pc,
+                               code_weights=list(NUSC['train_cfg']['code_weights'])),
+                bbox_coder=dict(type='CenterPointBBoxCoder', post_center_range=[pc[0] - 10, pc[1] - 10, -10.0, pc[3] + 10, pc[4] + 10, 10.0],
+                                max_num=500, score_threshold=0.1, out_size_factor=out_size_factor, voxel_size=(vx, vy), pc_range=pc[:2],
+                                code_size=9),
+                test_cfg=dict(post_center_limit_range=[pc[0] - 10, pc[1] - 10, -10.0, pc[3] + 10, pc[4] + 10, 10.0], max_per_img=500,
+                              max_pool_nms=False, min_radius=[4, 12, 10, 1, 0.85, 0.175], post_max_size=83, score_threshold=0.1,
+                              pc_range=pc[:2], out_size_factor=out_size_factor, voxel_size=(vx, vy), nms_type='rotate', pre_max_size=1000,
+                              nms_thr=0.2))
+
+
+def _geom(geom):
+    return GEOMETRIES[geom] if isinstance(geom, str) else geom
+
+
 def head_cfg(geom, in_channels=16, share_conv_channel=8, dcn=False):
-    """a CenterHead config dict of GEOMETRIES[geom] (the regression heads of both CenterHead configs; SeparateHead unless dcn)"""
-    G = GEOMETRIES[geom]
+    """a CenterHead config dict of GEOMETRIES[geom] or of a geometry() dict (the regression heads of both CenterHead configs;
+    SeparateHead unless dcn)"""
+    G = _geom(geom)
     names = [[f"c{i}_{j}" for j in range(n)] for i, n in enumerate(G['tasks'])]
     sep = dict(type='SeparateHead', init_bias=-2.19, final_kernel=3)
     if dcn:
@@ -328,16 +353,16 @@ def near_integer_sizes(cfg, count):
 
 
 def synth_batch(seed, geom, sizes, edge=True):
-    """raw boxes / labels per sample for GEOMETRIES[geom]; sizes: boxes per sample (0 = an empty sample)"""
-    G = GEOMETRIES[geom]
+    """raw boxes / labels per sample for GEOMETRIES[geom] or a geometry() dict; sizes: boxes per sample (0 = an empty sample)"""
+    G = _geom(geom)
     ncls = sum(G['tasks'])
     out = [synth_sample(seed * 97 + i, G['train_cfg'], n, ncls, G['box_dim'], edge=edge and n > 0) for i, n in enumerate(sizes)]
     return [o[0] for o in out], [o[1] for o in out]
 
 
 def synth_preds(seed, geom, batch, scale=1.0):
-    """random head outputs (heatmap logits per task and the five regression heads) for GEOMETRIES[geom], fp32"""
-    G = GEOMETRIES[geom]
+    """random head outputs (heatmap logits per task and the five regression heads) for GEOMETRIES[geom] or a geometry() dict, fp32"""
+    G = _geom(geom)
     W, H = feature_map_size(G['train_cfg'])
     g = torch.Generator().manual_seed(seed)
     out = []

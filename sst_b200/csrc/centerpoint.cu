@@ -154,7 +154,7 @@ __global__ void __launch_bounds__(CP_THREADS) cp_draw_kernel(const __grid_consta
   const int left = min(x, radius), right = min(a.W - x, radius + 1);
   const int top = min(y, radius), bottom = min(a.H - y, radius + 1);
   const int ww = left + right, hh = top + bottom;
-  const double sigma = (double)(2 * radius + 1) / 6.0;
+  const double sigma = (2.0 * radius + 1.0) / 6.0;  // in double: radius reaches 2^30, where 2 radius + 1 overflows an int
   const double den = 2.0 * sigma * sigma;
   int* hm = (int*)(a.task[task].heatmap + ((size_t)b * a.task[task].ncls + r.x) * a.H * a.W);
   for (int k = lane; k < ww * hh; k += 32) {
@@ -171,18 +171,22 @@ __global__ void __launch_bounds__(CP_THREADS) cp_draw_kernel(const __grid_consta
 
 __device__ __forceinline__ float fl_sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 
+// torch.clamp: a NaN sigmoid stays NaN (fminf / fmaxf would turn it into a bound and hide a NaN logit)
+__device__ __forceinline__ float fl_clip(float s) { return s < FL_CLIP_LO ? FL_CLIP_LO : (s > FL_CLIP_HI ? FL_CLIP_HI : s); }
+
 __device__ __forceinline__ float fl_loss(float x, float t) {
-  const float p = fminf(fmaxf(fl_sigmoid(x), FL_CLIP_LO), FL_CLIP_HI);
+  const float p = fl_clip(fl_sigmoid(x));
   const float q = 1.f - p, u = 1.f - t;
   const float pos = t == 1.f ? -logf(p + FL_EPS) * q * q : 0.f;
   const float neg = -logf(q + FL_EPS) * p * p * (u * u) * (u * u);
   return pos + neg;
 }
 
-// d loss / d x: d/dp of the element's loss times the clamp's pass-through (inclusive at the bounds, as torch.clamp) times s (1 - s)
+// d loss / d x: d/dp of the element's loss times the clamp's pass-through (inclusive at the bounds, as torch.clamp) times s (1 - s);
+// a NaN sigmoid passes the clamp, so a NaN logit gets a NaN gradient
 __device__ __forceinline__ float fl_grad(float x, float t) {
   const float s = fl_sigmoid(x);
-  if (!(s >= FL_CLIP_LO && s <= FL_CLIP_HI)) return 0.f;
+  if (s < FL_CLIP_LO || s > FL_CLIP_HI) return 0.f;
   const float p = s, q = 1.f - p, u = 1.f - t;
   float d = (p * p / (q + FL_EPS) - 2.f * p * logf(q + FL_EPS)) * ((u * u) * (u * u));
   if (t == 1.f) d += -q * q / (p + FL_EPS) + 2.f * q * logf(p + FL_EPS);
@@ -300,9 +304,10 @@ __global__ void __launch_bounds__(CP_THREADS) l1_forward_kernel(const __grid_con
   for (long long e = threadIdx.x; e < (long long)a.B * a.M * 10; e += blockDim.x) {
     const long long bm = e / 10;
     const int c = (int)(e - bm * 10), b = (int)(bm / a.M);
-    if (!a.mask[bm]) continue;
+    // a masked-out slot adds |pred - target| * 0, as the reference's gather at every slot does: a NaN or an off-map ind there makes
+    // the loss NaN
     const float tv = a.anno_box[e];
-    acc += (double)(fabsf(l1_pred(a, b, a.ind[bm], c) - tv) * l1_weight(a, tv, c));
+    acc += (double)(fabsf(l1_pred(a, b, a.ind[bm], c) - tv) * (a.mask[bm] ? l1_weight(a, tv, c) : 0.f));
   }
   acc = block_sum_double(acc, shd);
   if (threadIdx.x == 0) *loss = (float)((double)a.loss_weight * (acc / (double)avg));

@@ -1128,7 +1128,8 @@ def centerpoint_targets(boxes, labels, sample_sizes, task_num_classes, pc_min, v
 class GaussianFocalLossFunction(Function):
     """mmdet 2.14 GaussianFocalLoss (alpha 2, gamma 4, reduction 'mean', avg_factor = max(num_pos, 1)) on clip_sigmoid(logits): returns
     (loss, num_pos), both fp32 device scalars, num_pos = the number of target elements equal to 1.  Saves only the two inputs; the
-    backward recomputes the per-element derivative."""
+    backward recomputes the per-element derivative.  As torch.clamp, the clamp keeps NaN: a NaN logit makes the loss NaN and its own
+    gradient NaN."""
 
     @staticmethod
     def forward(ctx, logits, target, loss_weight=1.0):
@@ -1182,7 +1183,9 @@ def _l1_geom(heads, anno_box, ind, mask):
 class CenterPointL1LossFunction(Function):
     """CenterHead.loss's regression term: mmdet 2.14 L1Loss (reduction 'mean') of anno_box [B, M, 10] against the five heads gathered
     at ind, weight mask * (target not NaN) * code_weights, avg_factor = sum(mask) + 1e-4 on the device.  The heads are read in place;
-    the backward writes their dense gradients with each cell's objects summed in slot order (deterministic, no float atomics)."""
+    the backward writes their dense gradients with each cell's objects summed in slot order (deterministic, no float atomics).  As in
+    the reference, every slot is gathered, masked or not: a NaN target, or a NaN prediction at any slot's ind, makes the loss NaN, while
+    the gradient there stays 0 (torch.sign(NaN) = 0)."""
 
     @staticmethod
     def forward(ctx, anno_box, ind, mask, code_weights, loss_weight, *heads):

@@ -34,6 +34,27 @@ def test_oracle_targets_bit_identical_to_reference(geom, sizes):
             assert torch.equal(a, b), f"{name} of task {t} differs in {int((a != b).sum())} elements"
 
 
+# non-square maps, and an out_size_factor of 2 with 9-dim boxes and two tasks: the shapes tests/test_gpu_centerpoint_edges.py builds on
+NONSQUARE = {"200x136": dict(width=200, height=136),
+             "osf2_256x176": dict(width=256, height=176, out_size_factor=2, voxel_size=(0.2, 0.2), tasks=(1, 2), box_dim=9)}
+
+
+@pytest.mark.parametrize("name", list(NONSQUARE))
+def test_oracle_targets_bit_identical_to_reference_nonsquare(name):
+    R = _ref()
+    G = CO.geometry(**NONSQUARE[name])
+    W, H = CO.feature_map_size(G['train_cfg'])
+    assert W != H
+    boxes, labels = CO.synth_batch(17, G, [400, 0, 50])
+    ref = CR.build_center_head(CO.head_cfg(G)).get_targets([R.Boxes(b) for b in boxes], labels)
+    got = CO.targets([CO.gravity(b) for b in boxes], labels, G['tasks'], G['train_cfg'])
+    for i, name in enumerate(("heatmap", "anno_box", "ind", "mask")):
+        for t, (a, b) in enumerate(zip(ref[i], got[i])):
+            assert a.dtype == b.dtype and a.shape == b.shape, (name, t)
+            assert torch.equal(a, b), f"{name} of task {t} differs in {int((a != b).sum())} elements"
+    assert ref[0][0].shape[-2:] == (H, W)
+
+
 def test_edge_cases_are_exercised():
     """the synthetic batches hold what the targets' semantics hinge on"""
     G = CO.GEOMETRIES["waymo"]
