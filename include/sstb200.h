@@ -683,6 +683,77 @@ int sstb200_centerpoint_l1_loss_backward(sstb200_ctx* ctx, const float* const he
                                          const float code_weights[10], float loss_weight, const float* grad_loss,
                                          float* const grad_heads[5]);
 
+/* ---- Anchor3DHead training (mmdet3d/models/dense_heads/anchor3d_head.py:197-379, train_mixins.py), fp32, stream-ordered, no sync.
+ *
+ * sstb200_anchor3d_targets: anchor_target_3d of one level with one MaxIoUAssigner per anchor size (BboxOverlapsNearest3D,
+ *   ignore_iof_thr -1, match_low_quality), PseudoSampler, DeltaXYZWLHRBBoxCoder (code_size 7) and get_direction_target, for every
+ *   sample and size in a fixed number of launches (seven).
+ *   Anchors (AlignedAnchor3DRangeGenerator, never materialised): anchor ((y W + x) S + s) R + r = (x_centers[x], y_centers[y],
+ *   size_z[s], size_wlh[s][0..2], rotations[r]), device arrays [W], [H], [S], [S, 3], [R].  GT boxes [N, 7] bottom-centre (x, y, z, w,
+ *   l, h, yaw) and labels int64 [N], the samples concatenated: sample b owns rows [sample_offsets[b], sample_offsets[b + 1]) (host,
+ *   batch + 1 entries).  Per size s (host arrays): pos_iou_thr, neg_iou_thr, min_pos_iou (compared as fp32), gt_max_assign_all.
+ *   assign_per_class: size s sees only the GTs labelled s.
+ *   Assignment (mmdet 2.14 MaxIoUAssigner.assign_wrt_overlaps, IoU(gt, anchor)), per sample and size:
+ *     - an anchor with max IoU >= 0 and < neg_iou_thr gets 0 (negative); every other anchor starts at -1 (ignored);
+ *     - an anchor with max IoU >= pos_iou_thr gets argmax + 1, the argmax being the first GT on ties;
+ *     - then for each GT i in order whose max IoU over the anchors is >= min_pos_iou, every anchor whose IoU with i equals that max gets
+ *       i + 1 (only the first such anchor when gt_max_assign_all is 0).  Later GTs overwrite earlier ones; this overrides the first two
+ *       rules.
+ *     - with no GT (of its class, under assign_per_class) every anchor of the size is negative.
+ *   IoU = mmdet bbox_overlaps of the nearest BEV boxes (lidar_box3d.py nearest_bev: w and l swapped when |limit_period(yaw, 0.5, pi)|
+ *   > pi / 4), every operation a correctly rounded fp32 one with pi and pi / 4 rounded to fp32, no FMA contraction:
+ *   overlap / max(area_gt + area_anchor - overlap, 1e-6).  Per-GT maxima combine by an integer max on the fp32 bits, so two calls give
+ *   bit-identical results.  Boxes must be finite.
+ *   Outputs [batch, A] in the anchor order above (A = H W S R), fully written:
+ *     labels int64 (the GT's label for positives, num_classes otherwise), label_weights f32 (1 for positive and negative, 0 for
+ *     ignored), bbox_targets / bbox_weights f32 [batch, A, 7] (encode(anchor, gt) and 1 for positives, else 0), dir_targets int64 /
+ *     dir_weights f32 (clamp(floor(limit_period(rt + ra - dir_offset, 0, 2 pi) / pi), 0, 1) and 1 for positives, else 0), and the
+ *     device scalar num_total_pos int64 = sum over samples of max(positives, 1).  Temporaries (12 bytes per anchor and sample, 8 per GT
+ *     and size) from the context arena.
+ *   Errors: a NULL pointer, a size < 1, non-monotone offsets (SSTB_ERR_ARG); more than 256 samples, 8 sizes or 8 rotations, more than
+ *   4096 GTs in a sample, batch A reaching 2^28 (SSTB_ERR_UNSUPPORTED).
+ *
+ * sstb200_anchor_focal_loss_forward: mmdet 2.14 FocalLoss(use_sigmoid, gamma 2, alpha 0.25) of cls_score [B, A_loc C, H, W] (read in
+ *   place; element (b, y, x, a, c) is channel a C + c, anchor (y W + x) A_loc + a) against one-hot(labels) [B, A] with background
+ *   num_classes, weighted by label_weights [B, A]: *loss = loss_weight * sum / num_total_pos (device int64).  Log-sigmoid is the stable
+ *   softplus form of mmdet's py_sigmoid_focal_loss: it stays exact for logits of any size, where mmcv's CUDA kernel clamps
+ *   log(max(1 - p, FLT_MIN)) and so saturates near 87 for logits beyond about +-17.  A NaN logit makes the loss NaN.  Block partials in
+ *   double summed in a fixed order: deterministic.  Two launches, partials from the context arena.
+ * sstb200_anchor_focal_loss_backward: grad_cls_score (same shape) = grad_loss[0] * loss_weight / num_total_pos * label_weight * d loss /
+ *   d logit, recomputed from the logits in one elementwise pass; NaN only at a NaN logit.
+ *
+ * sstb200_anchor_reg_dir_loss_forward: over the positives (0 <= label < num_classes) only.  bbox_pred [B, A_loc 7, H, W] and
+ *   dir_cls_preds [B, A_loc 2, H, W] read in place.  loss_bbox = loss_weight_bbox * sum |pred - target| * bbox_weight * code_weight /
+ *   num_total_pos, channel 6 compared as sin(p) cos(t) against cos(p) sin(t) (add_sin_difference); loss_dir = loss_weight_dir *
+ *   sum dir_weight * (logsumexp(z) - z[dir_target]) / num_total_pos.  No positives: both 0.  Two launches.
+ * sstb200_anchor_reg_dir_loss_backward: grad_losses = (d / d loss_bbox, d / d loss_dir) on the device; grad_bbox_pred / grad_dir_cls_preds
+ *   fully written, zero off the positives: each positive owns its cells' channels, so there are no atomics.  sign(0) = 0, as torch.abs'
+ *   gradient; the yaw channel's derivative goes through both sin(p) cos(t) and cos(p) sin(t).  One launch.
+ *   Errors (all four): a NULL pointer or a size < 1 (SSTB_ERR_ARG). */
+int sstb200_anchor3d_targets(sstb200_ctx* ctx, const float* x_centers, int width, const float* y_centers, int height, const float* size_z,
+                             const float* size_wlh, int num_sizes, const float* rotations, int num_rots, const float* gt_boxes,
+                             const int64_t* gt_labels, const int32_t* sample_offsets, int batch, const float* pos_iou_thr,
+                             const float* neg_iou_thr, const float* min_pos_iou, const int32_t* gt_max_assign_all, int assign_per_class,
+                             int num_classes, float dir_offset, int64_t* labels, float* label_weights, float* bbox_targets,
+                             float* bbox_weights, int64_t* dir_targets, float* dir_weights, int64_t* num_total_pos);
+int sstb200_anchor_focal_loss_forward(sstb200_ctx* ctx, const float* cls_score, int batch, int num_anchors, int num_classes, int height,
+                                      int width, const int64_t* labels, const float* label_weights, const int64_t* num_total_pos,
+                                      float loss_weight, float* loss);
+int sstb200_anchor_focal_loss_backward(sstb200_ctx* ctx, const float* cls_score, int batch, int num_anchors, int num_classes, int height,
+                                       int width, const int64_t* labels, const float* label_weights, const int64_t* num_total_pos,
+                                       float loss_weight, const float* grad_loss, float* grad_cls_score);
+int sstb200_anchor_reg_dir_loss_forward(sstb200_ctx* ctx, const float* bbox_pred, const float* dir_cls_preds, int batch, int num_anchors,
+                                        int num_classes, int height, int width, const int64_t* labels, const float* bbox_targets,
+                                        const float* bbox_weights, const int64_t* dir_targets, const float* dir_weights,
+                                        const float code_weight[7], const int64_t* num_total_pos, float loss_weight_bbox,
+                                        float loss_weight_dir, float* loss_bbox, float* loss_dir);
+int sstb200_anchor_reg_dir_loss_backward(sstb200_ctx* ctx, const float* bbox_pred, const float* dir_cls_preds, int batch, int num_anchors,
+                                         int num_classes, int height, int width, const int64_t* labels, const float* bbox_targets,
+                                         const float* bbox_weights, const int64_t* dir_targets, const float* dir_weights,
+                                         const float code_weight[7], const int64_t* num_total_pos, float loss_weight_bbox,
+                                         float loss_weight_dir, const float* grad_losses, float* grad_bbox_pred,
+                                         float* grad_dir_cls_preds);
+
 #ifdef __cplusplus
 }
 #endif

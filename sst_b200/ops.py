@@ -17,6 +17,8 @@ and error behaviour; no CPU path - CPU tensors raise.
                                       ops/roiaware_pool3d                    (box membership, RoI-aware pooling)
     deform_conv2d, DeformConv2dFunction
                                       mmcv.ops.deform_conv (1.3.8-1.4.0)    (CenterHead's DCN)
+    anchor3d_targets, anchor_focal_loss, anchor_reg_dir_loss
+                                      models/dense_heads/anchor3d_head.py, train_mixins.py (Anchor3DHead training)
 """
 import ctypes as C
 import math
@@ -1217,3 +1219,189 @@ class CenterPointL1LossFunction(Function):
 def centerpoint_l1_loss(preds, anno_box, ind, mask, code_weights, loss_weight=1.0):
     """preds: a dict with 'reg', 'height', 'dim', 'rot', 'vel' [B, C, H, W] -> the loss (fp32 device scalar)"""
     return CenterPointL1LossFunction.apply(anno_box, ind, mask, code_weights, loss_weight, *[preds[k] for k, _ in CENTERPOINT_HEADS])
+
+
+# ----------------------------------------------------------------------------------------------
+# Anchor3DHead training (mmdet3d/models/dense_heads/anchor3d_head.py:197-379, train_mixins.py:11-346)
+# ----------------------------------------------------------------------------------------------
+L.SIGNATURES["sstb200_anchor3d_targets"] = (C.c_int, [L.vp, L.vp, C.c_int, L.vp, C.c_int, L.vp, L.vp, C.c_int, L.vp, C.c_int, L.vp, L.vp,
+                                                      L.P_i32, C.c_int, L.P_f32, L.P_f32, L.P_f32, L.P_i32, C.c_int, C.c_int, C.c_float,
+                                                      L.vp, L.vp, L.vp, L.vp, L.vp, L.vp, L.vp])
+_FOCAL_ARGS = [L.vp, L.vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, L.vp, L.vp, L.vp, C.c_float]
+L.SIGNATURES["sstb200_anchor_focal_loss_forward"] = (C.c_int, _FOCAL_ARGS + [L.vp])
+L.SIGNATURES["sstb200_anchor_focal_loss_backward"] = (C.c_int, _FOCAL_ARGS + [L.vp, L.vp])
+_REG_ARGS = [L.vp, L.vp, L.vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, L.vp, L.vp, L.vp, L.vp, L.vp, L.P_f32, L.vp, C.c_float,
+             C.c_float]
+L.SIGNATURES["sstb200_anchor_reg_dir_loss_forward"] = (C.c_int, _REG_ARGS + [L.vp, L.vp])
+L.SIGNATURES["sstb200_anchor_reg_dir_loss_backward"] = (C.c_int, _REG_ARGS + [L.vp, L.vp, L.vp])
+
+
+def anchor3d_targets(x_centers, y_centers, size_z, size_wlh, rotations, gt_boxes, gt_labels, sample_sizes, num_classes, pos_iou_thr,
+                     neg_iou_thr, min_pos_iou, gt_max_assign_all=True, assign_per_class=False, dir_offset=0.0):
+    """anchor_target_3d of one level (AlignedAnchor3DRangeGenerator anchors, one MaxIoUAssigner per size, PseudoSampler,
+    DeltaXYZWLHRBBoxCoder) for the whole batch.  The anchors are given by their separable axes, all fp32 CUDA tensors: x_centers [W],
+    y_centers [H], size_z [S], size_wlh [S, 3], rotations [R]; anchor ((y W + x) S + s) R + r.  gt_boxes [N, 7] fp32 bottom-centre and
+    gt_labels [N] on the GPU, the samples concatenated (sample_sizes: host ints).  pos_iou_thr / neg_iou_thr / min_pos_iou /
+    gt_max_assign_all: one value per size (or one for all).  Returns (labels int64 [B, A], label_weights [B, A], bbox_targets [B, A, 7],
+    bbox_weights [B, A, 7], dir_targets int64 [B, A], dir_weights [B, A], num_total_pos int64 device scalar), the reference's tensors in
+    its anchor order.  No host sync; bit-identical from run to run."""
+    axes = [_fp32_cuda(n, t) for n, t in (("x_centers", x_centers), ("y_centers", y_centers), ("size_z", size_z),
+                                          ("size_wlh", size_wlh), ("rotations", rotations))]
+    xc, yc, sz, wlh, rot = axes
+    W, H, S, R = xc.numel(), yc.numel(), sz.numel(), rot.numel()
+    if wlh.numel() != 3 * S:
+        raise L.SSTB200Error(f"anchor3d_targets: size_wlh must be [{S}, 3], got {tuple(wlh.shape)}")
+    if not isinstance(gt_boxes, torch.Tensor) or not gt_boxes.is_cuda or not isinstance(gt_labels, torch.Tensor) or not gt_labels.is_cuda:
+        raise L.SSTB200Error("anchor3d_targets: gt_boxes and gt_labels must be CUDA tensors (there is no CPU path)")
+    if gt_boxes.dtype != torch.float32 or gt_boxes.dim() != 2 or gt_boxes.shape[1] != 7:
+        raise L.SSTB200Error(f"anchor3d_targets: gt_boxes must be float32 [N, 7], got {gt_boxes.dtype} {tuple(gt_boxes.shape)}")
+    if gt_labels.dim() != 1 or gt_labels.shape[0] != gt_boxes.shape[0]:
+        raise L.SSTB200Error(f"anchor3d_targets: gt_labels {tuple(gt_labels.shape)} do not match gt_boxes {tuple(gt_boxes.shape)}")
+    sizes = [int(n) for n in sample_sizes]
+    if sum(sizes) != gt_boxes.shape[0] or min(sizes, default=-1) < 0:
+        raise L.SSTB200Error(f"anchor3d_targets: sample sizes {sizes} do not add up to the {gt_boxes.shape[0]} boxes")
+
+    def per_size(name, v, ctype):
+        vals = list(v) if isinstance(v, (list, tuple)) else [v] * S
+        if len(vals) != S:
+            raise L.SSTB200Error(f"anchor3d_targets: {name} needs {S} values, got {len(vals)}")
+        return L.arr(ctype, [ctype(x).value if ctype is C.c_float else int(bool(x)) for x in vals])
+
+    B, A, dev = len(sizes), H * W * S * R, xc.device
+    gt, gl = gt_boxes.contiguous(), gt_labels.long().contiguous()
+    offsets = [0]
+    for n in sizes:
+        offsets.append(offsets[-1] + n)
+    labels = torch.empty((B, A), dtype=torch.int64, device=dev)
+    label_weights = torch.empty((B, A), dtype=torch.float32, device=dev)
+    bbox_targets = torch.empty((B, A, 7), dtype=torch.float32, device=dev)
+    bbox_weights = torch.empty((B, A, 7), dtype=torch.float32, device=dev)
+    dir_targets = torch.empty((B, A), dtype=torch.int64, device=dev)
+    dir_weights = torch.empty((B, A), dtype=torch.float32, device=dev)
+    num_total_pos = torch.empty((), dtype=torch.int64, device=dev)
+    c = L.ctx(dev)
+    L.check(c, L.lib().sstb200_anchor3d_targets(
+        c, L.ptr(xc), W, L.ptr(yc), H, L.ptr(sz), L.ptr(wlh), S, L.ptr(rot), R, L.ptr(gt) if gt.numel() else None,
+        L.ptr(gl) if gl.numel() else None, L.arr(C.c_int32, offsets), B, per_size("pos_iou_thr", pos_iou_thr, C.c_float),
+        per_size("neg_iou_thr", neg_iou_thr, C.c_float), per_size("min_pos_iou", min_pos_iou, C.c_float),
+        per_size("gt_max_assign_all", gt_max_assign_all, C.c_int32), int(bool(assign_per_class)), int(num_classes), float(dir_offset),
+        L.ptr(labels), L.ptr(label_weights), L.ptr(bbox_targets), L.ptr(bbox_weights), L.ptr(dir_targets), L.ptr(dir_weights),
+        L.ptr(num_total_pos)))
+    return labels, label_weights, bbox_targets, bbox_weights, dir_targets, dir_weights, num_total_pos
+
+
+def _anchor_geom(name, t, num_anchors, per_anchor, B=None, H=None, W=None):
+    t = _fp32_cuda(name, t, 4)
+    b, ch, h, w = t.shape
+    if ch != num_anchors * per_anchor or (B is not None and (b, h, w) != (B, H, W)):
+        raise L.SSTB200Error(f"{name} must be [B, {num_anchors} x {per_anchor}, H, W] on one map, got {tuple(t.shape)}")
+    return t
+
+
+def _anchor_targets_check(name, B, A, labels, *ts):
+    if tuple(labels.shape) != (B, A) or labels.dtype != torch.int64 or not labels.is_cuda:
+        raise L.SSTB200Error(f"{name}: labels must be int64 [{B}, {A}] on the GPU, got {labels.dtype} {tuple(labels.shape)}")
+    for t in ts:
+        if not t.is_cuda or t.shape[:2] != (B, A):
+            raise L.SSTB200Error(f"{name}: targets must be [{B}, {A}, ...] on the GPU, got {tuple(t.shape)}")
+
+
+class AnchorFocalLossFunction(Function):
+    """Anchor3DHead.loss_single's classification term: mmdet 2.14 FocalLoss(use_sigmoid=True, gamma 2, alpha 0.25) of cls_score
+    [B, A_loc C, H, W], read in place (no permuted copy), against labels [B, A] (background = num_classes) weighted by label_weights,
+    divided by the device num_total_pos and multiplied by loss_weight.  The log-sigmoid is the stable softplus form (mmdet's
+    py_sigmoid_focal_loss), exact out to any logit; mmcv's CUDA kernel instead saturates near 87 beyond about +-17.  A NaN logit makes the
+    loss NaN and its own gradient NaN."""
+
+    @staticmethod
+    def forward(ctx, cls_score, labels, label_weights, num_total_pos, num_classes, loss_weight=1.0):
+        x = _fp32_cuda("cls_score", cls_score, 4)
+        B, ch, H, W = x.shape
+        if ch % num_classes:
+            raise L.SSTB200Error(f"anchor_focal_loss: {ch} channels are not a multiple of {num_classes} classes")
+        A_loc = ch // num_classes
+        lw = _fp32_cuda("label_weights", label_weights)
+        _anchor_targets_check("anchor_focal_loss", B, H * W * A_loc, labels, lw)
+        loss = torch.empty((), dtype=torch.float32, device=x.device)
+        c = L.ctx(x.device)
+        L.check(c, L.lib().sstb200_anchor_focal_loss_forward(c, L.ptr(x), B, A_loc, int(num_classes), H, W, L.ptr(labels), L.ptr(lw),
+                                                             L.ptr(num_total_pos), float(loss_weight), L.ptr(loss)))
+        ctx.save_for_backward(x, labels, lw, num_total_pos)
+        ctx.cfg = (int(num_classes), float(loss_weight), cls_score.dtype)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        x, labels, lw, ntp = ctx.saved_tensors
+        num_classes, loss_weight, dtype = ctx.cfg
+        B, ch, H, W = x.shape
+        g = torch.empty_like(x)
+        gl = grad_loss.float().contiguous()
+        c = L.ctx(x.device)
+        L.check(c, L.lib().sstb200_anchor_focal_loss_backward(c, L.ptr(x), B, ch // num_classes, num_classes, H, W, L.ptr(labels), L.ptr(lw),
+                                                              L.ptr(ntp), loss_weight, L.ptr(gl), L.ptr(g)))
+        return g.to(dtype), None, None, None, None, None
+
+
+def anchor_focal_loss(cls_score, labels, label_weights, num_total_pos, num_classes, loss_weight=1.0):
+    """the loss (fp32 device scalar) of AnchorFocalLossFunction"""
+    return AnchorFocalLossFunction.apply(cls_score, labels, label_weights, num_total_pos, num_classes, loss_weight)
+
+
+class AnchorRegDirLossFunction(Function):
+    """Anchor3DHead.loss_single's box and direction terms over the positives (0 <= label < num_classes): mmdet 2.14 L1Loss of bbox_pred
+    [B, A_loc 7, H, W] against bbox_targets, weighted by bbox_weights * code_weight, with add_sin_difference on the yaw; and
+    CrossEntropyLoss(use_sigmoid=False) of dir_cls_preds [B, A_loc 2, H, W] against dir_targets weighted by dir_weights.  Both divided by
+    the device num_total_pos and multiplied by their loss weights; both heads are read in place.  Returns (loss_bbox, loss_dir); with no
+    positive both are 0 with zero gradients, as the reference's pos_bbox_pred.sum().  The backward writes both gradients in full with no
+    atomics: every positive anchor owns its own channels."""
+
+    @staticmethod
+    def forward(ctx, bbox_pred, dir_cls_preds, labels, bbox_targets, bbox_weights, dir_targets, dir_weights, num_total_pos, num_classes,
+                code_weight, loss_weight_bbox, loss_weight_dir):
+        p = _fp32_cuda("bbox_pred", bbox_pred, 4)
+        B, ch, H, W = p.shape
+        if ch % 7:
+            raise L.SSTB200Error(f"anchor_reg_dir_loss: bbox_pred has {ch} channels, not a multiple of 7")
+        A_loc = ch // 7
+        d = _anchor_geom("dir_cls_preds", dir_cls_preds, A_loc, 2, B, H, W)
+        bt, bw, dw = (_fp32_cuda(n, t) for n, t in (("bbox_targets", bbox_targets), ("bbox_weights", bbox_weights),
+                                                     ("dir_weights", dir_weights)))
+        _anchor_targets_check("anchor_reg_dir_loss", B, H * W * A_loc, labels, bt, bw, dir_targets, dw)
+        if dir_targets.dtype != torch.int64 or bt.shape[-1] != 7 or bw.shape[-1] != 7:
+            raise L.SSTB200Error("anchor_reg_dir_loss: dir_targets must be int64 and the box targets / weights [B, A, 7]")
+        cw = [float(v) for v in (code_weight if code_weight else [1.0] * 7)]
+        if len(cw) != 7:
+            raise L.SSTB200Error(f"anchor_reg_dir_loss: 7 code weights are needed, got {len(cw)}")
+        lb = torch.empty((), dtype=torch.float32, device=p.device)
+        ld = torch.empty((), dtype=torch.float32, device=p.device)
+        dt = dir_targets.contiguous()
+        c = L.ctx(p.device)
+        L.check(c, L.lib().sstb200_anchor_reg_dir_loss_forward(c, L.ptr(p), L.ptr(d), B, A_loc, int(num_classes), H, W, L.ptr(labels),
+                                                               L.ptr(bt), L.ptr(bw), L.ptr(dt), L.ptr(dw), L.arr(C.c_float, cw),
+                                                               L.ptr(num_total_pos), float(loss_weight_bbox), float(loss_weight_dir),
+                                                               L.ptr(lb), L.ptr(ld)))
+        ctx.save_for_backward(p, d, labels, bt, bw, dt, dw, num_total_pos)
+        ctx.cfg = (int(num_classes), cw, float(loss_weight_bbox), float(loss_weight_dir), bbox_pred.dtype, dir_cls_preds.dtype)
+        return lb, ld
+
+    @staticmethod
+    def backward(ctx, grad_bbox, grad_dir):
+        p, d, labels, bt, bw, dt, dw, ntp = ctx.saved_tensors
+        num_classes, cw, wb, wd, pdt, ddt = ctx.cfg
+        B, ch, H, W = p.shape
+        zero = torch.zeros((), dtype=torch.float32, device=p.device)
+        gl = torch.stack([zero if grad_bbox is None else grad_bbox.float(), zero if grad_dir is None else grad_dir.float()]).contiguous()
+        gp, gd = torch.empty_like(p), torch.empty_like(d)
+        c = L.ctx(p.device)
+        L.check(c, L.lib().sstb200_anchor_reg_dir_loss_backward(c, L.ptr(p), L.ptr(d), B, ch // 7, num_classes, H, W, L.ptr(labels),
+                                                                L.ptr(bt), L.ptr(bw), L.ptr(dt), L.ptr(dw), L.arr(C.c_float, cw),
+                                                                L.ptr(ntp), wb, wd, L.ptr(gl), L.ptr(gp), L.ptr(gd)))
+        return (gp.to(pdt), gd.to(ddt)) + (None,) * 10
+
+
+def anchor_reg_dir_loss(bbox_pred, dir_cls_preds, labels, bbox_targets, bbox_weights, dir_targets, dir_weights, num_total_pos, num_classes,
+                        code_weight=None, loss_weight_bbox=1.0, loss_weight_dir=1.0):
+    """(loss_bbox, loss_dir), fp32 device scalars, of AnchorRegDirLossFunction"""
+    return AnchorRegDirLossFunction.apply(bbox_pred, dir_cls_preds, labels, bbox_targets, bbox_weights, dir_targets, dir_weights,
+                                          num_total_pos, num_classes, code_weight, loss_weight_bbox, loss_weight_dir)
