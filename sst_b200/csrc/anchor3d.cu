@@ -534,17 +534,16 @@ extern "C" int sstb200_anchor3d_targets(sstb200_ctx* c, const float* x_centers, 
   a.dir_w = dir_weights, a.num_total_pos = num_total_pos;
   const size_t SN = std::max<size_t>(1, (size_t)num_sizes * N), BA = (size_t)batch * A;
   arena_reset(c);
-  int rc = arena_reserve(c, al256(SN * 4) * 2 + al256((size_t)batch * num_sizes * 4) + al256((size_t)batch * 4) + al256(BA * 4) * 3);
+  int rc = arena_carve(c, [&](Carve& cv) {
+    a.gt_max = cv.take<unsigned>(SN);
+    a.gt_arg = cv.take<int>(SN);
+    a.nvalid = cv.take<int>((size_t)batch * num_sizes);
+    a.npos = cv.take<int>(batch);
+    a.max_iou = cv.take<float>(BA);
+    a.argmax = cv.take<int>(BA);
+    a.lowq = cv.take<int>(BA);
+  });
   if (rc) return rc;
-  a.gt_max = arena_alloc<unsigned>(c, SN);
-  a.gt_arg = arena_alloc<int>(c, SN);
-  a.nvalid = arena_alloc<int>(c, (size_t)batch * num_sizes);
-  a.npos = arena_alloc<int>(c, batch);
-  a.max_iou = arena_alloc<float>(c, BA);
-  a.argmax = arena_alloc<int>(c, BA);
-  a.lowq = arena_alloc<int>(c, BA);
-  if (!a.gt_max || !a.gt_arg || !a.nvalid || !a.npos || !a.max_iou || !a.argmax || !a.lowq)
-    return sstb_fail(c, SSTB_ERR_WORKSPACE, "anchor3d_targets: arena too small");
   cudaStream_t st = c->stream;
   const int small = (int)std::min<long long>(c->num_sms * 4LL, std::max<long long>(1, ((long long)SN + A3_THREADS - 1) / A3_THREADS));
   a3_init_kernel<<<std::max(small, (batch * num_sizes + A3_THREADS - 1) / A3_THREADS), A3_THREADS, 0, st>>>(a);
@@ -574,10 +573,9 @@ extern "C" int sstb200_anchor_focal_loss_forward(sstb200_ctx* c, const float* cl
   CHECK_ARG(c, loss);
   const int nb = loss_grid(c, a.n);
   arena_reset(c);
-  rc = arena_reserve(c, al256(nb * sizeof(double)));
+  double* part;
+  rc = arena_carve(c, [&](Carve& cv) { part = cv.take<double>(nb); });
   if (rc) return rc;
-  double* part = arena_alloc<double>(c, nb);
-  if (!part) return sstb_fail(c, SSTB_ERR_WORKSPACE, "anchor_focal_loss: arena too small");
   focal_forward_kernel<<<nb, A3_THREADS, 0, c->stream>>>(a, part);
   LAUNCH_CHECK(c);
   a3_final_kernel<<<1, A3_THREADS, 0, c->stream>>>(part, nb, 1, loss_weight, 0.f, num_total_pos, loss, nullptr);
@@ -610,10 +608,9 @@ extern "C" int sstb200_anchor_reg_dir_loss_forward(sstb200_ctx* c, const float* 
   CHECK_ARG(c, loss_bbox && loss_dir);
   const int nb = loss_grid(c, a.n);
   arena_reset(c);
-  rc = arena_reserve(c, al256(2 * nb * sizeof(double)));
+  double* part;
+  rc = arena_carve(c, [&](Carve& cv) { part = cv.take<double>(2 * nb); });
   if (rc) return rc;
-  double* part = arena_alloc<double>(c, 2 * nb);
-  if (!part) return sstb_fail(c, SSTB_ERR_WORKSPACE, "anchor_reg_dir_loss: arena too small");
   reg_forward_kernel<<<nb, A3_THREADS, 0, c->stream>>>(a, part, nb);
   LAUNCH_CHECK(c);
   a3_final_kernel<<<1, A3_THREADS, 0, c->stream>>>(part, nb, 2, loss_weight_bbox, loss_weight_dir, num_total_pos, loss_bbox, loss_dir);

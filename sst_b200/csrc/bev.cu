@@ -80,10 +80,9 @@ extern "C" int sstb200_recover_bev(sstb200_ctx* c, const float* voxel_feat, cons
   CHECK_ARG(c, ny <= 65535 && B <= 65535);
   const size_t cells = (size_t)B * ny * nx;
   arena_reset(c);
-  int rc = arena_reserve(c, al256(cells * 4) + 4096);
+  int32_t* cell_map;
+  int rc = arena_carve(c, [&](Carve& cv) { cell_map = cv.take<int32_t>(cells + 64); });
   if (rc) return rc;
-  int32_t* cell_map = arena_alloc<int32_t>(c, cells + 64);
-  if (!cell_map) return sstb_fail(c, SSTB_ERR_WORKSPACE, "recover_bev: arena");
   int32_t* err = cell_map + cells;
   CUDA_TRY(c, cudaMemsetAsync(cell_map, 0xFF, cells * 4, c->stream));
   CUDA_TRY(c, cudaMemsetAsync(err, 0, 4, c->stream));
@@ -184,10 +183,9 @@ extern "C" int sstb200_recover_bev_backward(sstb200_ctx* c, const float* grad_ca
   CHECK_ARG(c, ny <= 65535 && B <= 65535);
   const size_t cells = (size_t)B * ny * nx;
   arena_reset(c);
-  int rc = arena_reserve(c, al256(cells * 4) + 4096);
+  int32_t* cell_map;
+  int rc = arena_carve(c, [&](Carve& cv) { cell_map = cv.take<int32_t>(cells + 64); });
   if (rc) return rc;
-  int32_t* cell_map = arena_alloc<int32_t>(c, cells + 64);
-  if (!cell_map) return sstb_fail(c, SSTB_ERR_WORKSPACE, "recover_bev_backward: arena");
   int32_t* err = cell_map + cells;  // bev_map_kernel's flag; out-of-canvas rows are zero-filled by bev_dup_kernel instead
   CUDA_TRY(c, cudaMemsetAsync(cell_map, 0xFF, cells * 4, c->stream));
   launch_pdl(bev_map_kernel, dim3((M + 255) / 256), dim3(256), (size_t)0, c->stream, (const long long*)coors, M, B, ny, nx, cell_map, err);

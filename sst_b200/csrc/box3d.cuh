@@ -162,41 +162,47 @@ __device__ __forceinline__ uint32_t block_sum(uint32_t v, uint32_t* sh) {
   return t;
 }
 
-// ---- host side: table size, arena bytes and the build of the grid over num_pts points ------------------------------------------
+// ---- host side: table size, workspace and the build of the grid over num_pts points -------------------------------------------
 static uint32_t grid_table_size(int num_pts) {
   uint32_t T = 1024;
   while (T < 2u * (uint32_t)num_pts && T < (1u << 24)) T <<= 1;
   return T;
 }
-static size_t grid_bytes(int num_pts, uint32_t T) {
+struct GridWs {
+  int32_t* count;
+  int32_t* bucket;
+  uint32_t* key;
+  float4* spts;
+  int2* skey;
+  Csr csr;
+};
+static void grid_carve(Carve& cv, GridWs& w, int num_pts, uint32_t T) {
   const size_t N = (size_t)num_pts;
-  return al256(((size_t)T + 2) * 4) + csr_bytes(N, T) + al256(N * 4) * 2 + al256(N * 16) + al256(N * 8);
+  w.count = cv.take<int32_t>((size_t)T + 2);
+  w.bucket = cv.take<int32_t>(N + 1);
+  w.key = cv.take<uint32_t>(N + 1);
+  w.spts = cv.take<float4>(N + 1);
+  w.skey = cv.take<int2>(N + 1);
+  csr_carve(cv, w.csr, N, T);
 }
 // Bins the points (flags[0] = 1 when a batch id is negative; flags must be zeroed already) and fills g.  *binned: device count of
 // the points with a batch id >= 0 (the length of g.spts / g.skey).
-static int grid_build(sstb200_ctx* c, const float* pts, const int32_t* pts_batch, int N, uint32_t T, float3 ex, int32_t* flags, Grid& g,
-                      const uint32_t** binned) {
-  int32_t* count = arena_alloc<int32_t>(c, (size_t)T + 2);
-  int32_t* bucket = arena_alloc<int32_t>(c, (size_t)N + 1);
-  uint32_t* key = arena_alloc<uint32_t>(c, (size_t)N + 1);
-  float4* spts = arena_alloc<float4>(c, (size_t)N + 1);
-  int2* skey = arena_alloc<int2>(c, (size_t)N + 1);
-  if (!count || !bucket || !key || !spts || !skey) return sstb_fail(c, SSTB_ERR_WORKSPACE, "point grid: arena too small");
-  CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)T + 2) * 4, c->stream));
+static int grid_build(sstb200_ctx* c, GridWs& w, const float* pts, const int32_t* pts_batch, int N, uint32_t T, float3 ex, int32_t* flags,
+                      Grid& g, const uint32_t** binned) {
+  CUDA_TRY(c, cudaMemsetAsync(w.count, 0, ((size_t)T + 2) * 4, c->stream));
   if (N > 0)
-    launch_pdl(rp_bin_kernel, dim3((N + 255) / 256), dim3(256), (size_t)0, c->stream, pts, pts_batch, N, T - 1, bucket, key, count, flags);
-  Csr csr;
-  int rc = csr_build<int32_t>(c, csr, bucket, N, count, T, nullptr);
+    launch_pdl(rp_bin_kernel, dim3((N + 255) / 256), dim3(256), (size_t)0, c->stream, pts, pts_batch, N, T - 1, w.bucket, w.key, w.count, flags);
+  int rc = csr_build<int32_t>(c, w.csr, w.bucket, N, w.count, T, nullptr);
   if (rc) return rc;
   if (N > 0)
-    launch_pdl(rp_gather_kernel, dim3((N + 255) / 256), dim3(256), (size_t)0, c->stream, pts, pts_batch, (const int32_t*)csr.order,
-               (const uint32_t*)key, (const uint32_t*)(csr.offsets + T), spts, skey);
-  g.offsets = csr.offsets;
-  g.spts = spts;
-  g.skey = skey;
+    launch_pdl(rp_gather_kernel, dim3((N + 255) / 256), dim3(256), (size_t)0, c->stream, pts, pts_batch, (const int32_t*)w.csr.order,
+               (const uint32_t*)w.key, (const uint32_t*)(w.csr.offsets + T), w.spts, w.skey);
+  g.offsets = w.csr.offsets;
+  g.spts = w.spts;
+  g.skey = w.skey;
   g.mask = T - 1;
   g.ex = ex;
-  *binned = csr.offsets + T;  // points with a batch id >= 0
+  *binned = w.csr.offsets + T;  // points with a batch id >= 0
   return SSTB_OK;
 }
 

@@ -140,19 +140,21 @@ extern "C" int sstb200_connected_components(sstb200_ctx* c, const float* centers
   rc = make_extents(c, er, 1, lor, hir, &Tr);
   if (rc) return rc;
   arena_reset(c);
-  rc = arena_reserve(c, key_index_bytes(n, T) + key_index_bytes(1, Tr) + csr_bytes(n, n) + al256((size_t)n * 12) + al256((size_t)n * 4) * 4 + 16384);
-  if (rc) return rc;
   KeyIndex k, kr;
-  rc = key_index_alloc(c, k, n, T);
+  int32_t *rows, *parent, *root, *cellmap, *count;
+  Csr r;
+  rc = arena_carve(c, [&](Carve& cv) {
+    key_index_carve(cv, k, n, T);
+    key_index_carve(cv, kr, 1, Tr);
+    rows = cv.take<int32_t>((size_t)n * 3);
+    parent = cv.take<int32_t>(n);
+    root = cv.take<int32_t>(n);
+    cellmap = cv.take<int32_t>(n);
+    count = cv.take<int32_t>((size_t)n + 2);
+    csr_carve(cv, r, n, n);
+  });
   if (rc) return rc;
-  rc = key_index_alloc(c, kr, 1, Tr);
-  if (rc) return rc;
-  int32_t* rows = arena_alloc<int32_t>(c, (size_t)n * 3);
-  int32_t* parent = arena_alloc<int32_t>(c, n);
-  int32_t* root = arena_alloc<int32_t>(c, n);
-  int32_t* cellmap = arena_alloc<int32_t>(c, n);
-  int32_t* count = arena_alloc<int32_t>(c, (size_t)n + 2);
-  if (!rows || !parent || !root || !cellmap || !count) return sstb_fail(c, SSTB_ERR_WORKSPACE, "connected_components: arena too small");
+  if ((rc = key_index_zero(c, k)) || (rc = key_index_zero(c, kr))) return rc;
   CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)n + 2) * 4, c->stream));
   const int nb = (n + 255) / 256;
   launch_pdl(ccl_rows_kernel, dim3(nb), dim3(256), (size_t)0, c->stream, centers, stride, batch_idx, n, g, rows, parent);
@@ -160,7 +162,6 @@ extern "C" int sstb200_connected_components(sstb200_ctx* c, const float* centers
   key_index_scan(c, k);
   launch_pdl(map_count_kernel<int32_t>, dim3(nb), dim3(256), (size_t)0, c->stream, (const long long*)k.keys, n, (const uint32_t*)k.bitmap,
              (const uint32_t*)k.word_prefix, 0, (const int32_t*)k.flags, cellmap, count, (const int32_t*)nullptr);
-  Csr r;
   rc = csr_build<int32_t>(c, r, cellmap, n, count, n, (const int32_t*)k.total);
   if (rc) return rc;
   launch_pdl(ccl_union_kernel, dim3(nb), dim3(256), (size_t)0, c->stream, centers, stride, (const int32_t*)rows, n, g, dist, (const uint32_t*)k.bitmap,

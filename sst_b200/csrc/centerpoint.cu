@@ -409,10 +409,8 @@ extern "C" int sstb200_centerpoint_targets(sstb200_ctx* c, const float* boxes, c
   a.k1m = (float)(1.0 - o), a.k1p = (float)(1.0 + o), a.km2o = (float)(-2.0 * o), a.kom1 = (float)(o - 1.0), a.k4a3 = (float)(4.0 * (4.0 * o));
   const int nrec = batch * num_tasks * max_objs;
   arena_reset(c);
-  int rc = arena_reserve(c, al256((size_t)nrec * sizeof(int4)));
+  int rc = arena_carve(c, [&](Carve& cv) { a.records = cv.take<int4>(nrec); });
   if (rc) return rc;
-  a.records = arena_alloc<int4>(c, nrec);
-  if (!a.records) return sstb_fail(c, SSTB_ERR_WORKSPACE, "centerpoint_targets: arena too small");
   cudaStream_t st = c->stream;
   cp_slots_kernel<<<batch * num_tasks, CP_THREADS, 0, st>>>(a);
   LAUNCH_CHECK(c);
@@ -428,11 +426,13 @@ extern "C" int sstb200_gaussian_focal_loss_forward(sstb200_ctx* c, const float* 
   CHECK_ARG(c, n >= 1 && logits && target && loss && num_pos);
   const int nb = fl_grid(c, n);
   arena_reset(c);
-  int rc = arena_reserve(c, al256(nb * sizeof(double)) + al256(nb * sizeof(long long)));
+  double* pl;
+  long long* pp;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    pl = cv.take<double>(nb);
+    pp = cv.take<long long>(nb);
+  });
   if (rc) return rc;
-  double* pl = arena_alloc<double>(c, nb);
-  long long* pp = arena_alloc<long long>(c, nb);
-  if (!pl || !pp) return sstb_fail(c, SSTB_ERR_WORKSPACE, "gaussian_focal_loss: arena too small");
   fl_forward_kernel<<<nb, CP_THREADS, 0, c->stream>>>(logits, target, n, pl, pp);
   LAUNCH_CHECK(c);
   fl_final_kernel<<<1, CP_THREADS, 0, c->stream>>>(pl, pp, nb, loss_weight, loss, num_pos);

@@ -63,38 +63,65 @@ inline int sstb_fail(sstb200_ctx* c, int code, const char* fmt, ...) {
 
 #define LAUNCH_CHECK(ctx) CUDA_TRY(ctx, cudaGetLastError())
 
+static inline size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// ---- workspace carving ----------------------------------------------------------------------------------------------------------
+// A workspace layout is written once, as a carve function f(Carve&) that takes its pieces in order.  Over base == nullptr the
+// cursor only measures (every take returns nullptr); over a real base it hands out the same pieces.  Each piece starts on a
+// 256-byte boundary.  A carve function only carves - no launches, no memsets, no arithmetic on the pointers it gets back - and
+// takes the same branches in both passes.
+struct Carve {
+  char* base = nullptr;
+  size_t off = 0;
+  template <typename T>
+  T* take(size_t n) {
+    off = al256(off);
+    T* p = base ? (T*)(base + off) : nullptr;
+    off += n * sizeof(T);
+    return p;
+  }
+  size_t mark() const { return al256(off); }  // where the next piece starts: cv.off - cv.mark() spans the pieces taken since
+};
+
+// bytes of a caller-owned workspace laid out by f from offset 0
+template <typename F>
+static inline size_t carve_bytes(F&& f) {
+  Carve m;
+  f(m);
+  return al256(m.off);
+}
+
 // ---- arena ---------------------------------------------------------------
+// bump arena for the temporaries of one call: arena_reset starts a phase, arena_carve lays out its pieces from c->arena_off
 inline void arena_reset(sstb200_ctx* c) {
   c->arena_off = 0;
   c->arena_epoch++;
 }
 
-// Reserve: make sure `bytes` are available from offset 0 (called once at the top of an op
-// with an upper bound, so that no growth happens mid-op).
-inline int arena_reserve(sstb200_ctx* c, size_t bytes) {
-  bytes += 4096;
-  if (bytes <= c->arena_cap) return SSTB_OK;
-  size_t cap = c->arena_cap ? c->arena_cap : (size_t)1 << 24;
-  while (cap < bytes) cap *= 2;
-  void* p = nullptr;
-  cudaError_t e = cudaMalloc(&p, cap);
-  if (e != cudaSuccess) return sstb_fail(c, SSTB_ERR_WORKSPACE, "arena cudaMalloc(%zu) failed: %s", cap, cudaGetErrorString(e));
-  if (c->arena) c->retired.push_back(c->arena);
-  c->arena = (char*)p;
-  c->arena_cap = cap;
+// Measures f from c->arena_off, grows the arena (with a sync) when it is too small, then carves f out of it and advances
+// c->arena_off.  Growth happens only here, before any piece of the phase is handed out, so a warm-up call sizes the arena once
+// for the CUDA graph captured after it.  A grown arena retires the old one: pieces an earlier carve of the same phase handed
+// out stay valid until destroy.
+template <typename F>
+static inline int arena_carve(sstb200_ctx* c, F&& f) {
+  Carve m{nullptr, c->arena_off};
+  f(m);
+  if (m.off > c->arena_cap) {
+    size_t cap = c->arena_cap ? c->arena_cap : (size_t)1 << 24;
+    while (cap < m.off) cap *= 2;
+    void* p = nullptr;
+    cudaError_t e = cudaMalloc(&p, cap);
+    if (e != cudaSuccess) return sstb_fail(c, SSTB_ERR_WORKSPACE, "arena cudaMalloc(%zu) failed: %s", cap, cudaGetErrorString(e));
+    if (c->arena) c->retired.push_back(c->arena);
+    c->arena = (char*)p;
+    c->arena_cap = cap;
+  }
+  Carve r{c->arena, c->arena_off};
+  f(r);
+  if (r.off != m.off) return sstb_fail(c, SSTB_ERR_WORKSPACE, "arena carve: the measuring and carving passes disagree");
+  c->arena_off = r.off;
   return SSTB_OK;
 }
-
-template <typename T>
-inline T* arena_alloc(sstb200_ctx* c, size_t n) {
-  size_t off = (c->arena_off + 255) & ~(size_t)255;
-  size_t bytes = n * sizeof(T);
-  if (off + bytes > c->arena_cap) return nullptr;
-  c->arena_off = off + bytes;
-  return (T*)(c->arena + off);
-}
-
-static inline size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-DEVICE property of a kernel: remember the largest value applied per device
 // (one static SmemAttr per call site / kernel instantiation), so a process that drives several GPUs sets it on each of them.
@@ -254,7 +281,7 @@ __device__ __forceinline__ int4 pack8_h16(float4 a, float4 b) {
 // ONE launch, any length: single-pass chained scan with decoupled look-back.  Tiles of 256 threads x 8 items are
 // claimed through an atomic ticket (so a tile only ever waits for tiles that are already running), publish
 // (status, value) as one 64-bit word and look back 32 predecessors at a time.  `Load` maps element index -> uint32.
-// ScanTemps must be zero before the launch (scan_temps_alloc memsets it; one scan per allocation).
+// ScanTemps must be zero before the launch (its owner memsets what scan_carve took; one scan per carve).
 #define SCAN_ITEMS 8
 #define SCAN_THREADS 256
 #define SCAN_TILE (SCAN_ITEMS * SCAN_THREADS)
@@ -316,7 +343,10 @@ struct ScanTemps {
   unsigned long long* state;   // [tiles] (status << 32 | value); status 0 = empty, 1 = tile aggregate, 2 = inclusive prefix
 };
 static inline size_t scan_num_blocks(size_t n_cap) { return (n_cap + 1 + SCAN_TILE - 1) / SCAN_TILE; }
-static inline size_t scan_temps_bytes(size_t n_cap) { return al256(64 * 4 + (scan_num_blocks(n_cap) + 1) * 8); }
+static inline void scan_carve(Carve& cv, ScanTemps& t, size_t n_cap) {
+  t.ticket = cv.take<uint32_t>(64);
+  t.state = cv.take<unsigned long long>(scan_num_blocks(n_cap) + 1);
+}
 
 // n may be read from device memory (n_dev != nullptr) so that data-dependent sizes never sync.
 template <typename Load>

@@ -378,33 +378,40 @@ int bits_for(long long n) {  // bits to hold 0 .. n - 1
   return b;
 }
 
-struct DcnBwdLayout {
-  size_t xT, gyT, keys, vals, skeys, svals, cub, part, total, cub_bytes;
+// the backward's caller-owned workspace: dcn_bwd_ws sizes it, dcn_bwd_carve lays it out
+struct DcnBwdWs {
   long long M;  // 4 * samples
   int splits, end_bit;
+  size_t cub_bytes;
+  float *xT, *gyT, *part;
+  uint32_t *keys, *vals, *skeys, *svals;
+  uint8_t* cub;
 };
 
-DcnBwdLayout dcn_bwd_layout(const DcnGeom& g) {
-  DcnBwdLayout l;
+DcnBwdWs dcn_bwd_ws(const DcnGeom& g) {
+  DcnBwdWs l;
   l.M = 4 * g.NP * g.D * g.K;
   l.splits = (int)((g.NP + DCN_DW_CHUNK - 1) / DCN_DW_CHUNK);
   l.end_bit = max(1, bits_for((long long)g.N * g.D * g.H * g.W + 1));
   l.cub_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, l.cub_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
                                   (uint32_t*)nullptr, (int)l.M, 0, l.end_bit, (cudaStream_t)0);
-  const size_t cub_bytes = l.cub_bytes;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t at = o; o += al256(bytes); return at; };
-  l.xT = take((size_t)g.N * g.H * g.W * g.C * 4);
-  l.gyT = take((size_t)g.NP * g.O * 4);
-  l.keys = take((size_t)l.M * 4);
-  l.vals = take((size_t)l.M * 4);
-  l.skeys = take((size_t)l.M * 4);
-  l.svals = take((size_t)l.M * 4);
-  l.cub = take(cub_bytes + 16);
-  l.part = take((size_t)l.splits * g.O * g.Cg * g.K * 4);
-  l.total = o;
   return l;
+}
+
+void dcn_bwd_carve(Carve& cv, DcnBwdWs& l, const DcnGeom& g) {
+  l.xT = cv.take<float>((size_t)g.N * g.H * g.W * g.C);
+  l.gyT = cv.take<float>((size_t)g.NP * g.O);
+  l.keys = cv.take<uint32_t>(l.M);
+  l.vals = cv.take<uint32_t>(l.M);
+  l.skeys = cv.take<uint32_t>(l.M);
+  l.svals = cv.take<uint32_t>(l.M);
+  l.cub = cv.take<uint8_t>(l.cub_bytes + 16);
+  l.part = cv.take<float>((size_t)l.splits * g.O * g.Cg * g.K);
+}
+
+size_t dcn_bwd_bytes(DcnBwdWs l, const DcnGeom& g) {
+  return carve_bytes([&](Carve& cv) { dcn_bwd_carve(cv, l, g); });
 }
 
 }  // namespace
@@ -415,11 +422,9 @@ extern "C" int sstb200_dcn_forward(sstb200_ctx* c, const int32_t geom[15], const
   if (rc) return rc;
   CHECK_ARG(c, x && offset && weight && y);
   arena_reset(c);
-  const size_t xb = (size_t)g.N * g.H * g.W * g.C;
-  rc = arena_reserve(c, al256(xb * 4));
+  float* xT;
+  rc = arena_carve(c, [&](Carve& cv) { xT = cv.take<float>((size_t)g.N * g.H * g.W * g.C); });
   if (rc) return rc;
-  float* xT = arena_alloc<float>(c, xb);
-  if (!xT) return sstb_fail(c, SSTB_ERR_WORKSPACE, "dcn_forward: arena too small");
   cudaStream_t st = c->stream;
   CUDA_TRY(c, launch_nhwc(st, x, g.N, g.C, (long long)g.H * g.W, xT));
   const int BN = dcn_bn(g.Og), otiles = (g.Og + BN - 1) / BN;
@@ -437,7 +442,7 @@ extern "C" int sstb200_dcn_backward_workspace_bytes(sstb200_ctx* c, const int32_
   int rc = dcn_bwd_geom(c, geom, g);
   if (rc) return rc;
   CHECK_ARG(c, bytes);
-  *bytes = (int64_t)dcn_bwd_layout(g).total;
+  *bytes = (int64_t)dcn_bwd_bytes(dcn_bwd_ws(g), g);
   return SSTB_OK;
 }
 
@@ -448,18 +453,19 @@ extern "C" int sstb200_dcn_backward(sstb200_ctx* c, const int32_t geom[15], cons
   int rc = dcn_bwd_geom(c, geom, g);
   if (rc) return rc;
   CHECK_ARG(c, x && offset && weight && grad_y && workspace);
-  const DcnBwdLayout l = dcn_bwd_layout(g);
-  if (workspace_bytes < (int64_t)l.total)
-    return sstb_fail(c, SSTB_ERR_WORKSPACE, "dcn_backward: workspace of %lld bytes, %zu needed", (long long)workspace_bytes, l.total);
-  char* ws = (char*)workspace;
-  float* xT = (float*)(ws + l.xT);
-  float* gyT = (float*)(ws + l.gyT);
+  DcnBwdWs l = dcn_bwd_ws(g);
+  const size_t need = dcn_bwd_bytes(l, g);
+  if (workspace_bytes < (int64_t)need)
+    return sstb_fail(c, SSTB_ERR_WORKSPACE, "dcn_backward: workspace of %lld bytes, %zu needed", (long long)workspace_bytes, need);
+  Carve wc{(char*)workspace, 0};
+  dcn_bwd_carve(wc, l, g);
+  float *xT = l.xT, *gyT = l.gyT;
   cudaStream_t st = c->stream;
   CUDA_TRY(c, launch_nhwc(st, x, g.N, g.C, (long long)g.H * g.W, xT));
   CUDA_TRY(c, launch_nhwc(st, grad_y, g.N, g.O, g.HoWo, gyT));
   if (grad_weight) {
     const int BN = dcn_bn(g.Og), otiles = (g.Og + BN - 1) / BN, rchunks = (g.Cg * g.K + DCN_CC - 1) / DCN_CC;
-    float* part = (float*)(ws + l.part);
+    float* part = l.part;
     const dim3 grid((unsigned)l.splits, (unsigned)(g.G * rchunks), (unsigned)otiles);
     if (BN == 16) CUDA_TRY(c, launch_pdl(dcn_dw_kernel<16>, grid, dim3(DCN_THREADS), (size_t)0, st, g, (const float*)xT, offset, (const float*)gyT, rchunks, part));
     else if (BN == 32) CUDA_TRY(c, launch_pdl(dcn_dw_kernel<32>, grid, dim3(DCN_THREADS), (size_t)0, st, g, (const float*)xT, offset, (const float*)gyT, rchunks, part));
@@ -474,15 +480,12 @@ extern "C" int sstb200_dcn_backward(sstb200_ctx* c, const int32_t geom[15], cons
                            weight, (const float*)gyT, grad_offset));
   }
   if (grad_x) {
-    uint32_t* keys = (uint32_t*)(ws + l.keys);
-    uint32_t* vals = (uint32_t*)(ws + l.vals);
-    uint32_t* skeys = (uint32_t*)(ws + l.skeys);
-    uint32_t* svals = (uint32_t*)(ws + l.svals);
+    uint32_t *keys = l.keys, *vals = l.vals, *skeys = l.skeys, *svals = l.svals;
     const long long pixels = (long long)g.N * g.D * g.H * g.W, samples = l.M / 4;
     CUDA_TRY(c, launch_pdl(dcn_keys_kernel, dim3((unsigned)((samples + 255) / 256)), dim3(256), (size_t)0, st, g, offset, samples,
                            (uint32_t)pixels, keys, vals));
     size_t cub_bytes = l.cub_bytes;
-    cudaError_t ce = cub::DeviceRadixSort::SortPairs(ws + l.cub, cub_bytes, (const uint32_t*)keys, skeys, (const uint32_t*)vals, svals,
+    cudaError_t ce = cub::DeviceRadixSort::SortPairs(l.cub, cub_bytes, (const uint32_t*)keys, skeys, (const uint32_t*)vals, svals,
                                                      (int)l.M, 0, l.end_bit, st);
     if (ce != cudaSuccess) return sstb_fail(c, SSTB_ERR_CUDA, "cub radix sort: %s", cudaGetErrorString(ce));
     CUDA_TRY(c, launch_pdl(dcn_dx_kernel, dim3((unsigned)((pixels + 7) / 8)), dim3(DCN_THREADS), (size_t)0, st, g, offset, weight,

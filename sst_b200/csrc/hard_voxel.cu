@@ -120,32 +120,35 @@ extern "C" int sstb200_hard_voxelize(sstb200_ctx* c, const float* points, int P,
                                   P, 0, end_bit, st);
   const size_t pwords = ((size_t)P + 31) / 32;
   arena_reset(c);
-  rc = arena_reserve(c, key_index_bytes(P, T) + al256((size_t)P * 12) + 7 * al256((size_t)P * 4 + 64) + al256(pwords * 4) * 2 +
-                            scan_temps_bytes(pwords) + scan_temps_bytes(P) + al256(cub_bytes) + 65536);
-  if (rc) return rc;
   KeyIndex k;
-  rc = key_index_alloc(c, k, P, T);
+  int32_t *pcoors, *vid, *count, *first, *vnum;
+  uint32_t *iota, *vid_s, *idx_s, *offsets, *fbits, *fprefix;
+  ScanTemps fst, ost;
+  size_t zero_bytes;
+  void* cub_tmp;
+  rc = arena_carve(c, [&](Carve& cv) {
+    key_index_carve(cv, k, P, T);
+    pcoors = cv.take<int32_t>((size_t)P * 3);
+    vid = cv.take<int32_t>(P);
+    count = cv.take<int32_t>((size_t)P + 2);
+    first = cv.take<int32_t>(P);
+    vnum = cv.take<int32_t>(P);
+    iota = cv.take<uint32_t>(P);
+    vid_s = cv.take<uint32_t>(P);
+    idx_s = cv.take<uint32_t>(P);
+    offsets = cv.take<uint32_t>((size_t)P + 2);
+    // first-point bitmap + its scan state + the offsets scan's state: one zero fill
+    const size_t z = cv.mark();
+    fbits = cv.take<uint32_t>(pwords);
+    scan_carve(cv, fst, pwords);
+    scan_carve(cv, ost, P);
+    zero_bytes = cv.off - z;
+    fprefix = cv.take<uint32_t>(pwords + 2);
+    cub_tmp = cv.take<uint8_t>(cub_bytes + 16);
+  });
   if (rc) return rc;
-  int32_t* pcoors = arena_alloc<int32_t>(c, (size_t)P * 3);
-  int32_t* vid = arena_alloc<int32_t>(c, P);
-  int32_t* count = arena_alloc<int32_t>(c, (size_t)P + 2);
-  int32_t* first = arena_alloc<int32_t>(c, P);
-  int32_t* vnum = arena_alloc<int32_t>(c, P);
-  uint32_t* iota = arena_alloc<uint32_t>(c, P);
-  uint32_t* vid_s = arena_alloc<uint32_t>(c, P);
-  uint32_t* idx_s = arena_alloc<uint32_t>(c, P);
-  uint32_t* offsets = arena_alloc<uint32_t>(c, (size_t)P + 2);
-  // first-point bitmap + its scan state: one zero fill
-  const size_t fb_bytes = al256(pwords * 4), fst_bytes = scan_temps_bytes(pwords), ost_bytes = scan_temps_bytes(P);
-  uint8_t* z = arena_alloc<uint8_t>(c, fb_bytes + fst_bytes + ost_bytes);
-  uint32_t* fprefix = arena_alloc<uint32_t>(c, pwords + 2);
-  void* cub_tmp = arena_alloc<uint8_t>(c, cub_bytes + 16);
-  if (!pcoors || !vid || !count || !first || !vnum || !iota || !vid_s || !idx_s || !offsets || !z || !fprefix || !cub_tmp)
-    return sstb_fail(c, SSTB_ERR_WORKSPACE, "hard_voxelize: arena");
-  uint32_t* fbits = (uint32_t*)z;
-  ScanTemps fst{(uint32_t*)(z + fb_bytes), (unsigned long long*)(z + fb_bytes) + 32};
-  ScanTemps ost{(uint32_t*)(z + fb_bytes + fst_bytes), (unsigned long long*)(z + fb_bytes + fst_bytes) + 32};
-  CUDA_TRY(c, cudaMemsetAsync(z, 0, fb_bytes + fst_bytes + ost_bytes, st));
+  if ((rc = key_index_zero(c, k))) return rc;
+  CUDA_TRY(c, cudaMemsetAsync(fbits, 0, zero_bytes, st));
   CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)P + 2) * 4, st));
   CUDA_TRY(c, cudaMemsetAsync(first, 0x7F, (size_t)P * 4, st));
   const int nb = (P + 255) / 256;

@@ -19,28 +19,26 @@ struct KeyIndex {
   ScanTemps st;
   size_t nwords;
   long long T;
+  size_t zero_bytes;      // bitmap .. end of the scan temporaries
 };
 
-static size_t key_index_bytes(size_t P, long long T) {
-  size_t nwords = (size_t)((T + 31) / 32);
-  return al256(P * 8) + al256(nwords * 4) + al256((nwords + 1) * 4) + scan_temps_bytes(nwords) + 1024;
-}
-
-static int key_index_alloc(sstb200_ctx* c, KeyIndex& k, size_t P, long long T) {
+static void key_index_carve(Carve& cv, KeyIndex& k, size_t P, long long T) {
   k.T = T;
   k.nwords = (size_t)((T + 31) / 32);
-  k.keys = arena_alloc<long long>(c, P ? P : 1);
+  k.keys = cv.take<long long>(P ? P : 1);
   // bitmap and scan temporaries are adjacent: ONE memset clears both
-  size_t bm_bytes = al256(k.nwords * 4), st_bytes = scan_temps_bytes(k.nwords);
-  uint8_t* z = arena_alloc<uint8_t>(c, bm_bytes + st_bytes);
-  k.word_prefix = arena_alloc<uint32_t>(c, k.nwords + 1);
-  if (!k.keys || !z || !k.word_prefix) return sstb_fail(c, SSTB_ERR_WORKSPACE, "key index: arena too small");
-  k.bitmap = (uint32_t*)z;
-  k.st.ticket = (uint32_t*)(z + bm_bytes);
-  k.st.state = (unsigned long long*)(k.st.ticket + 64);
+  const size_t z = cv.mark();
+  k.bitmap = cv.take<uint32_t>(k.nwords);
+  scan_carve(cv, k.st, k.nwords);
+  k.zero_bytes = cv.off - z;
+  k.word_prefix = cv.take<uint32_t>(k.nwords + 1);
+}
+
+// clears the bitmap, the scan temporaries and the total / flags words that live in the scan's ticket block
+static int key_index_zero(sstb200_ctx* c, KeyIndex& k) {
   k.total = k.st.ticket + 1;
   k.flags = (int32_t*)(k.st.ticket + 2);
-  CUDA_TRY(c, cudaMemsetAsync(z, 0, bm_bytes + st_bytes, c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(k.bitmap, 0, k.zero_bytes, c->stream));
   return SSTB_OK;
 }
 
@@ -482,24 +480,23 @@ struct Csr {
   int32_t* cursor;
   ScanTemps st;
   uint32_t* total;
+  size_t zero_bytes;            // cursor .. end of the scan temporaries
 };
-static size_t csr_bytes(size_t n, size_t nseg_cap) {
-  return al256((nseg_cap + 2) * 4) * 2 + al256(n * 4 + 4) + scan_temps_bytes(nseg_cap) + 2048;
+// offsets / order set before the carve are the caller's own buffers (offsets [nseg_cap + 1]) and are not carved
+static void csr_carve(Carve& cv, Csr& r, size_t n, size_t nseg_cap) {
+  if (!r.offsets) r.offsets = cv.take<uint32_t>(nseg_cap + 2);
+  // cursor and scan temporaries are adjacent: ONE memset clears both
+  const size_t z = cv.mark();
+  r.cursor = cv.take<int32_t>(nseg_cap + 2);
+  scan_carve(cv, r.st, nseg_cap);
+  r.zero_bytes = cv.off - z;
+  if (!r.order) r.order = cv.take<int32_t>(n + 1);
 }
 template <typename TM>
 static int csr_build(sstb200_ctx* c, Csr& r, const TM* map, int n, const int32_t* count, size_t nseg_cap,
                      const int32_t* nseg_dev, const int32_t* n_dev = nullptr, int small_nseg = 0) {
-  if (!r.offsets) r.offsets = arena_alloc<uint32_t>(c, nseg_cap + 2);  // preset = caller-owned [nseg_cap + 1]
-  // cursor and scan temporaries are adjacent: ONE memset clears both
-  size_t cur_bytes = al256((nseg_cap + 2) * 4), st_bytes = scan_temps_bytes(nseg_cap);
-  uint8_t* z = arena_alloc<uint8_t>(c, cur_bytes + st_bytes);
-  if (!r.order) r.order = arena_alloc<int32_t>(c, n + 1);
-  if (!r.offsets || !z || !r.order) return sstb_fail(c, SSTB_ERR_WORKSPACE, "csr: arena too small");
-  r.cursor = (int32_t*)z;
-  r.st.ticket = (uint32_t*)(z + cur_bytes);
-  r.st.state = (unsigned long long*)(r.st.ticket + 64);
   r.total = r.st.ticket + 1;
-  CUDA_TRY(c, cudaMemsetAsync(z, 0, cur_bytes + st_bytes, c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(r.cursor, 0, r.zero_bytes, c->stream));
   launch_exclusive_scan(c->stream, LoadU32{(const uint32_t*)count}, nseg_cap, nseg_dev, r.st, r.offsets, r.total, true);
   if (n > 0 && small_nseg > 0 && small_nseg <= CSR_SMALL_MAX && !n_dev)
     launch_pdl(csr_fill_small_kernel<TM>, dim3((n + CSR_SMALL_ITEMS - 1) / CSR_SMALL_ITEMS), dim3(1024), (size_t)small_nseg * 8, c->stream, map, n, small_nseg,

@@ -281,24 +281,30 @@ __global__ void nms_pack_kernel(const SegRow* __restrict__ seg, int S, const int
   for (int q = threadIdx.x; q < c; q += blockDim.x) keep_out[at + q] = g.start + keep_local[g.start + q];
 }
 
-// workspace layout (every part 256-byte aligned): mask words | segment table | per-segment kept lists (int32 [num]) | counts
-struct NmsLayout {
-  size_t mask, table, lists, counts, total;
+// the caller-owned workspace: mask words | segment table | per-segment kept lists (int32 [num]) | counts
+struct NmsWs {
+  unsigned long long* mask;
+  SegRow* table;
+  int32_t *lists, *counts;
 };
 
-NmsLayout nms_layout(int num, const int32_t* off, int S) {
-  NmsLayout L;
+void nms_carve(Carve& cv, NmsWs& w, int num, const int32_t* off, int S) {
   size_t words = 0;
   for (int s = 0; s < S; s++) {
     const size_t n = (size_t)(off[s + 1] - off[s]);
     words += n * ((n + NMS_BLK - 1) / NMS_BLK);
   }
-  L.mask = 0;
-  L.table = al256(words * 8);
-  L.lists = L.table + al256((size_t)S * sizeof(SegRow));
-  L.counts = L.lists + al256((size_t)num * 4);
-  L.total = L.counts + al256((size_t)S * 4);
-  return L;
+  w.mask = cv.take<unsigned long long>(words);
+  w.table = cv.take<SegRow>(S);
+  w.lists = cv.take<int32_t>(num);
+  w.counts = cv.take<int32_t>(S);
+}
+
+size_t nms_bytes(int num, const int32_t* off, int S) {
+  return carve_bytes([&](Carve& cv) {
+    NmsWs w;
+    nms_carve(cv, w, num, off, S);
+  });
 }
 
 int check_segments(sstb200_ctx* c, int num, const int32_t* off, int S) {
@@ -339,7 +345,7 @@ extern "C" int sstb200_nms_bev_workspace_bytes(sstb200_ctx* c, int num, const in
   CHECK_ARG(c, c && bytes);
   const int rc = check_segments(c, num, seg_offsets, num_segs);
   if (rc) return rc;
-  *bytes = (int64_t)nms_layout(num, seg_offsets, num_segs).total;
+  *bytes = (int64_t)nms_bytes(num, seg_offsets, num_segs);
   return SSTB_OK;
 }
 
@@ -350,11 +356,13 @@ extern "C" int sstb200_nms_bev(sstb200_ctx* c, const float* boxes, int num, cons
   int rc = check_segments(c, num, seg_offsets, num_segs);
   if (rc) return rc;
   CHECK_ARG(c, (num == 0 || (boxes && keep_out)) && (num_segs == 0 || thresh));
-  const NmsLayout L = nms_layout(num, seg_offsets, num_segs);
-  if (!workspace) return sstb_fail(c, SSTB_ERR_ARG, "nms_bev: workspace is NULL (%zu bytes needed)", L.total);
-  if (workspace_bytes < (int64_t)L.total)
-    return sstb_fail(c, SSTB_ERR_WORKSPACE, "nms_bev: workspace of %lld bytes, %zu needed", (long long)workspace_bytes, L.total);
-  char* ws = (char*)workspace;
+  const size_t need = nms_bytes(num, seg_offsets, num_segs);
+  if (!workspace) return sstb_fail(c, SSTB_ERR_ARG, "nms_bev: workspace is NULL (%zu bytes needed)", need);
+  if (workspace_bytes < (int64_t)need)
+    return sstb_fail(c, SSTB_ERR_WORKSPACE, "nms_bev: workspace of %lld bytes, %zu needed", (long long)workspace_bytes, need);
+  NmsWs w;
+  Carve wc{(char*)workspace, 0};
+  nms_carve(wc, w, num, seg_offsets, num_segs);
   if (num_segs == 0) {
     CUDA_TRY(c, cudaMemsetAsync(num_keep_dev, 0, 4, c->stream));
   } else {
@@ -367,10 +375,9 @@ extern "C" int sstb200_nms_bev(sstb200_ctx* c, const float* boxes, int num, cons
       blocks += nb * (nb + 1) / 2;
     }
     if (blocks > 0x7fffffffLL) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "nms_bev: %lld mask blocks exceed one grid", blocks);
-    SegRow* dtab = (SegRow*)(ws + L.table);
-    int32_t* lists = (int32_t*)(ws + L.lists);
-    int32_t* counts = (int32_t*)(ws + L.counts);
-    unsigned long long* mask = (unsigned long long*)(ws + L.mask);
+    SegRow* dtab = w.table;
+    int32_t *lists = w.lists, *counts = w.counts;
+    unsigned long long* mask = w.mask;
     // from pageable memory: staged before the call returns, so `tab` may go out of scope
     CUDA_TRY(c, cudaMemcpyAsync(dtab, tab.data(), (size_t)num_segs * sizeof(SegRow), cudaMemcpyHostToDevice, c->stream));
     if (blocks > 0) {

@@ -73,14 +73,18 @@ extern "C" int sstb200_voxel2point(sstb200_ctx* c, const float* points, int Cp, 
   }
   CHECK_ARG(c, points && pts_coors && voxel_feats && voxel2point_inds && out && mask_out && voxel_size && pc_min);
   arena_reset(c);
-  int rc = arena_reserve(c, 2 * al256((size_t)N * 4 + 64) + scan_temps_bytes(N) + 4096);
+  uint32_t *keep, *pos;
+  ScanTemps st;
+  size_t st_bytes;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    keep = cv.take<uint32_t>((size_t)N + 2);
+    pos = cv.take<uint32_t>((size_t)N + 2);
+    const size_t z = cv.mark();
+    scan_carve(cv, st, N);
+    st_bytes = cv.off - z;
+  });
   if (rc) return rc;
-  uint32_t* keep = arena_alloc<uint32_t>(c, (size_t)N + 2);
-  uint32_t* pos = arena_alloc<uint32_t>(c, (size_t)N + 2);
-  uint8_t* z = arena_alloc<uint8_t>(c, scan_temps_bytes(N));
-  if (!keep || !pos || !z) return sstb_fail(c, SSTB_ERR_WORKSPACE, "voxel2point: arena");
-  ScanTemps st{(uint32_t*)z, (unsigned long long*)z + 32};
-  CUDA_TRY(c, cudaMemsetAsync(z, 0, scan_temps_bytes(N), c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(st.ticket, 0, st_bytes, c->stream));
   int32_t* err = (int32_t*)(st.ticket + 2);
   const unsigned blocks = (unsigned)(((size_t)N * 32 + 255) / 256);
   launch_pdl(v2p_mask_kernel, dim3(blocks), dim3(256), (size_t)0, c->stream, voxel_feats, C, (const long long*)voxel2point_inds, N, M, padding, keep,
@@ -137,24 +141,30 @@ extern "C" int sstb200_voxel2point_backward(sstb200_ctx* c, const float* grad_ou
   CHECK_ARG(c, grad_out && mask && voxel2point_inds);
   const int ld = C + (with_xyz ? 3 : 0);
   arena_reset(c);
-  int rc = arena_reserve(c, al256((size_t)N * 4 + 64) + scan_temps_bytes(N) + al256((size_t)K * 8) + al256((size_t)M * 4 + 4) +
-                                csr_bytes(K, M) + 4096);
+  uint32_t* pos;
+  ScanTemps st;
+  size_t st_bytes;
+  long long* row_voxel;
+  int32_t* count;
+  Csr r;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    pos = cv.take<uint32_t>((size_t)N + 2);
+    const size_t z = cv.mark();
+    scan_carve(cv, st, N);
+    st_bytes = cv.off - z;
+    row_voxel = cv.take<long long>(K);
+    count = cv.take<int32_t>((size_t)M + 1);
+    csr_carve(cv, r, K, M);
+  });
   if (rc) return rc;
-  uint32_t* pos = arena_alloc<uint32_t>(c, (size_t)N + 2);
-  uint8_t* z = arena_alloc<uint8_t>(c, scan_temps_bytes(N));
-  long long* row_voxel = arena_alloc<long long>(c, (size_t)K);
-  int32_t* count = arena_alloc<int32_t>(c, (size_t)M + 1);
-  if (!pos || !z || !row_voxel || !count) return sstb_fail(c, SSTB_ERR_WORKSPACE, "voxel2point_backward: arena");
-  ScanTemps st{(uint32_t*)z, (unsigned long long*)z + 32};
   int32_t* err = (int32_t*)(st.ticket + 2);  // count_index_kernel's flag for -1 rows; nothing reads it
-  CUDA_TRY(c, cudaMemsetAsync(z, 0, scan_temps_bytes(N), c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(st.ticket, 0, st_bytes, c->stream));
   CUDA_TRY(c, cudaMemsetAsync(row_voxel, 0xFF, (size_t)K * 8, c->stream));
   CUDA_TRY(c, cudaMemsetAsync(count, 0, (size_t)M * 4, c->stream));
   launch_exclusive_scan(c->stream, LoadMaskU8{mask}, (size_t)N, nullptr, st, pos, st.ticket + 1, true);
   launch_pdl(v2p_compact_kernel, dim3((N + 255) / 256), dim3(256), (size_t)0, c->stream, mask, (const uint32_t*)pos,
              (const long long*)voxel2point_inds, N, K, M, row_voxel);
   launch_pdl(count_index_kernel, dim3((K + 255) / 256), dim3(256), (size_t)0, c->stream, (const long long*)row_voxel, K, M, count, err);
-  Csr r;
   rc = csr_build(c, r, (const long long*)row_voxel, K, count, (size_t)M, nullptr);
   if (rc) return rc;
   launch_segment_reduce(c, grad_out, C, r.offsets, r.order, M, nullptr, SSTB200_REDUCE_SUM, 0.f, grad_voxel, nullptr, K, ld);

@@ -192,28 +192,32 @@ extern "C" int sstb200_dynamic_point_pool(sstb200_ctx* c, const float* rois, con
   const int R = num_rois, N = num_pts;
   const uint32_t T = grid_table_size(N);
   arena_reset(c);
-  const size_t Rc = (size_t)R + 1, st_roi = scan_temps_bytes(Rc);
-  int rc = arena_reserve(c, grid_bytes(N, T) + al256(Rc * 4) * 5 + al256(256 + 2 * st_roi) + 8192);
-  if (rc) return rc;
-  uint32_t* kept = arena_alloc<uint32_t>(c, Rc);
-  uint32_t* off = arena_alloc<uint32_t>(c, Rc);
-  uint32_t* take = arena_alloc<uint32_t>(c, Rc);
-  uint32_t* rows = arena_alloc<uint32_t>(c, Rc);
-  uint32_t* pos = arena_alloc<uint32_t>(c, Rc);
+  const size_t Rc = (size_t)R + 1;
+  uint32_t *kept, *off, *take, *rows, *pos;
   // flags [0] negative point batch, [1] negative RoI batch, [2] RoI batch ids not ascending (per-sample mode), [3] fake rows; then the
   // temporaries of the two scans
-  uint8_t* z = arena_alloc<uint8_t>(c, 256 + 2 * st_roi);
-  if (!kept || !off || !take || !rows || !pos || !z) return sstb_fail(c, SSTB_ERR_WORKSPACE, "dynamic_point_pool: arena too small");
-  int32_t* flags = (int32_t*)z;
+  int32_t* flags;
   ScanTemps s1, s2;
-  s1.ticket = (uint32_t*)(z + 256);
-  s1.state = (unsigned long long*)(s1.ticket + 64);
-  s2.ticket = (uint32_t*)(z + 256 + st_roi);
-  s2.state = (unsigned long long*)(s2.ticket + 64);
-  CUDA_TRY(c, cudaMemsetAsync(z, 0, 256 + 2 * st_roi, c->stream));
+  size_t zero_bytes;
+  GridWs gw;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    kept = cv.take<uint32_t>(Rc);
+    off = cv.take<uint32_t>(Rc);
+    take = cv.take<uint32_t>(Rc);
+    rows = cv.take<uint32_t>(Rc);
+    pos = cv.take<uint32_t>(Rc);
+    const size_t z = cv.mark();
+    flags = cv.take<int32_t>(64);
+    scan_carve(cv, s1, Rc);
+    scan_carve(cv, s2, Rc);
+    zero_bytes = cv.off - z;
+    grid_carve(cv, gw, N, T);
+  });
+  if (rc) return rc;
+  CUDA_TRY(c, cudaMemsetAsync(flags, 0, zero_bytes, c->stream));
   Grid g;
   const uint32_t* binned = nullptr;
-  rc = grid_build(c, pts, pts_batch, N, T, make_float3(extra_wlh[0], extra_wlh[1], extra_wlh[2]), flags, g, &binned);
+  rc = grid_build(c, gw, pts, pts_batch, N, T, make_float3(extra_wlh[0], extra_wlh[1], extra_wlh[2]), flags, g, &binned);
   if (rc) return rc;
   if (R > 0)
     launch_pdl(rp_count_kernel, dim3(R), dim3(RP_THREADS), (size_t)0, c->stream, rois, rois_batch, g, binned, max_inbox_point, per_sample,

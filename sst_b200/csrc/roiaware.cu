@@ -403,19 +403,24 @@ extern "C" int sstb200_roiaware_pool3d_plan(sstb200_ctx* c, const float* rois, c
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "roiaware_pool3d: %d RoIs x %lld voxels x %d points exceed a 64-bit pair key", R, nvox, N);
   const uint32_t T = grid_table_size(N);
   arena_reset(c);
-  const size_t Rc = (size_t)R + 1, st = scan_temps_bytes(Rc);
-  int rc = arena_reserve(c, grid_bytes(N, T) + al256(Rc * 4) * 2 + al256(256 + st) + 8192);
-  if (rc) return rc;
-  uint32_t* hits = arena_alloc<uint32_t>(c, Rc);
-  uint32_t* off = arena_alloc<uint32_t>(c, Rc);
-  uint8_t* z = arena_alloc<uint8_t>(c, 256 + st);  // flags [0] negative point batch, [1] negative RoI batch; then the scan's temporaries
-  if (!hits || !off || !z) return sstb_fail(c, SSTB_ERR_WORKSPACE, "roiaware_pool3d: arena too small");
-  int32_t* flags = (int32_t*)z;
+  const size_t Rc = (size_t)R + 1;
+  uint32_t *hits, *off;
+  int32_t* flags;  // [0] negative point batch, [1] negative RoI batch; then the scan's temporaries
   ScanTemps s;
-  s.ticket = (uint32_t*)(z + 256);
-  s.state = (unsigned long long*)(s.ticket + 64);
-  CUDA_TRY(c, cudaMemsetAsync(z, 0, 256 + st, c->stream));
-  rc = grid_build(c, pts, pts_batch, N, T, make_float3(0.f, 0.f, 0.f), flags, plan->g, &plan->binned);
+  size_t zero_bytes;
+  GridWs gw;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    hits = cv.take<uint32_t>(Rc);
+    off = cv.take<uint32_t>(Rc);
+    const size_t z = cv.mark();
+    flags = cv.take<int32_t>(64);
+    scan_carve(cv, s, Rc);
+    zero_bytes = cv.off - z;
+    grid_carve(cv, gw, N, T);
+  });
+  if (rc) return rc;
+  CUDA_TRY(c, cudaMemsetAsync(flags, 0, zero_bytes, c->stream));
+  rc = grid_build(c, gw, pts, pts_batch, N, T, make_float3(0.f, 0.f, 0.f), flags, plan->g, &plan->binned);
   if (rc) return rc;
   if (R > 0)
     launch_pdl(ra_count_kernel, dim3(R), dim3(RP_THREADS), (size_t)0, c->stream, rois, rois_batch, plan->g, plan->binned, hits, flags);
@@ -457,21 +462,28 @@ extern "C" int sstb200_roiaware_pool3d_forward(sstb200_ctx* c, const float* pts_
   size_t cub_bytes = 0;
   cub::DeviceRadixSort::SortKeys(nullptr, cub_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)P, 0, end_bit,
                                  st);
-  const size_t Pc = (size_t)P + 1, sc = scan_temps_bytes(Pc);
-  int rc = arena_reserve(c, c->arena_off + al256(Pc * 8) * 2 + al256(Pc * 4 + 4) * 4 + al256(2 * sc) + al256(cub_bytes) + 8192);
+  const size_t Pc = (size_t)P + 1;
+  unsigned long long *keys, *skeys;
+  uint32_t *head, *gid, *gstart, *kcnt;
+  ScanTemps s1, s2;
+  size_t zero_bytes;
+  void* cub_tmp;
+  // carved after the plan's pieces, which this call still reads
+  int rc = arena_carve(c, [&](Carve& cv) {
+    keys = cv.take<unsigned long long>(Pc);
+    skeys = cv.take<unsigned long long>(Pc);
+    head = cv.take<uint32_t>(Pc + 1);
+    gid = cv.take<uint32_t>(Pc + 1);
+    gstart = cv.take<uint32_t>(Pc + 1);
+    kcnt = cv.take<uint32_t>(Pc + 1);
+    const size_t z = cv.mark();
+    scan_carve(cv, s1, Pc);
+    scan_carve(cv, s2, Pc);
+    zero_bytes = cv.off - z;
+    cub_tmp = cv.take<uint8_t>(cub_bytes + 16);
+  });
   if (rc) return rc;
-  unsigned long long* keys = arena_alloc<unsigned long long>(c, Pc);
-  unsigned long long* skeys = arena_alloc<unsigned long long>(c, Pc);
-  uint32_t* head = arena_alloc<uint32_t>(c, Pc + 1);
-  uint32_t* gid = arena_alloc<uint32_t>(c, Pc + 1);
-  uint32_t* gstart = arena_alloc<uint32_t>(c, Pc + 1);
-  uint32_t* kcnt = arena_alloc<uint32_t>(c, Pc + 1);
-  uint8_t* z = arena_alloc<uint8_t>(c, 2 * sc);
-  void* cub_tmp = arena_alloc<uint8_t>(c, cub_bytes + 16);
-  if (!keys || !skeys || !head || !gid || !gstart || !kcnt || !z || !cub_tmp)
-    return sstb_fail(c, SSTB_ERR_WORKSPACE, "roiaware_pool3d_forward: arena too small");
-  ScanTemps s1{(uint32_t*)z, (unsigned long long*)(z + 256)}, s2{(uint32_t*)(z + sc), (unsigned long long*)(z + sc + 256)};
-  CUDA_TRY(c, cudaMemsetAsync(z, 0, 2 * sc, st));
+  CUDA_TRY(c, cudaMemsetAsync(s1.ticket, 0, zero_bytes, st));
   const int nb = (int)((P + 255) / 256);
   if (P > 0) {
     launch_pdl(ra_emit_kernel, dim3(p.R), dim3(RP_THREADS), (size_t)0, st, p.rois, p.rois_batch, p.g, p.binned, p.off, p.v, keys);
@@ -523,14 +535,16 @@ extern "C" int sstb200_roiaware_pool3d_backward(sstb200_ctx* c, int num_pts, int
                                   (int)P, 0, end_bit, st);
   arena_reset(c);
   const size_t Pc = (size_t)P + 1;
-  int rc = arena_reserve(c, al256(Pc * 4) * 4 + al256(cub_bytes) + 4096);
+  uint32_t *pkey, *pgrp, *skey, *sgrp;
+  void* cub_tmp;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    pkey = cv.take<uint32_t>(Pc);
+    pgrp = cv.take<uint32_t>(Pc);
+    skey = cv.take<uint32_t>(Pc);
+    sgrp = cv.take<uint32_t>(Pc);
+    cub_tmp = cv.take<uint8_t>(cub_bytes + 16);
+  });
   if (rc) return rc;
-  uint32_t* pkey = arena_alloc<uint32_t>(c, Pc);
-  uint32_t* pgrp = arena_alloc<uint32_t>(c, Pc);
-  uint32_t* skey = arena_alloc<uint32_t>(c, Pc);
-  uint32_t* sgrp = arena_alloc<uint32_t>(c, Pc);
-  void* cub_tmp = arena_alloc<uint8_t>(c, cub_bytes + 16);
-  if (!pkey || !pgrp || !skey || !sgrp || !cub_tmp) return sstb_fail(c, SSTB_ERR_WORKSPACE, "roiaware_pool3d_backward: arena too small");
   if (P > 0) {
     launch_pdl(ra_inverse_kernel, dim3((unsigned)((P + 255) / 256)), dim3(256), (size_t)0, st, voxel_offsets, point_idx, counts_dev, P, N,
                pkey, pgrp);

@@ -166,28 +166,26 @@ __global__ void shortcut_kernel(float* __restrict__ out, const float* __restrict
   out[i] += in_feats[(size_t)p * cin + 3 + ch];
 }
 
-// Group CSR (offsets [G+1] int32, order [N] int32): points grouped by `inv`; shared by every block of a SIR backbone.
-static int group_csr(sstb200_ctx* c, const long long* inv, int N, int G, int32_t* offsets_out, int32_t* order_out) {
+// Group CSR: points grouped by `inv`; shared by every block of a SIR backbone.  csr.offsets / csr.order set before the carve are
+// the caller's own buffers.
+void sstb_sir_group_csr_carve(Carve& cv, SirGroupCsr& g, int N, int G) {
+  g.count = cv.take<int32_t>((size_t)G + 2);
+  csr_carve(cv, g.csr, N, G);
+}
+
+int sstb_sir_group_csr(sstb200_ctx* c, SirGroupCsr& g, const long long* inv, int N, int G) {
   cudaStream_t st = c->stream;
-  int32_t* count = arena_alloc<int32_t>(c, (size_t)G + 2);
-  if (!count) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
+  int32_t* count = g.count;
   CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)G + 2) * 4, st));
   const bool small = G <= CSR_SMALL_MAX;
   if (small)
     launch_pdl(count_small_kernel<long long>, dim3((N + CSR_SMALL_ITEMS - 1) / CSR_SMALL_ITEMS), dim3(1024), (size_t)G * 4, st, inv, N, G, count, count + G + 1);
   else
     launch_pdl(count_index_kernel, dim3((N + 255) / 256), dim3(256), (size_t)(0), st, inv, N, G, count, count + G + 1);
-  Csr r;
-  r.offsets = (uint32_t*)offsets_out;
-  r.order = order_out;
-  int rc = csr_build<long long>(c, r, inv, N, count, G, nullptr, nullptr, small ? G : 0);
+  int rc = csr_build<long long>(c, g.csr, inv, N, count, G, nullptr, nullptr, small ? G : 0);
   if (rc) return rc;
   LAUNCH_CHECK(c);
   return SSTB_OK;
-}
-
-int sstb_sir_group_csr(sstb200_ctx* c, const long long* inv, int N, int G, int32_t* offsets, int32_t* order) {
-  return group_csr(c, inv, N, G, offsets, order);
 }
 
 extern "C" int sstb200_group_csr(sstb200_ctx* c, const int64_t* inv, int N, int G, int32_t* offsets, int32_t* order) {
@@ -195,9 +193,12 @@ extern "C" int sstb200_group_csr(sstb200_ctx* c, const int64_t* inv, int N, int 
   if (N == 0 || G == 0) return SSTB_OK;
   CHECK_ARG(c, inv && offsets && order);
   arena_reset(c);
-  int rc = arena_reserve(c, csr_bytes(N, G) + al256((size_t)G * 4 + 8) + 65536);
+  SirGroupCsr g;
+  g.csr.offsets = (uint32_t*)offsets;
+  g.csr.order = order;
+  int rc = arena_carve(c, [&](Carve& cv) { sstb_sir_group_csr_carve(cv, g, N, G); });
   if (rc) return rc;
-  return group_csr(c, (const long long*)inv, N, G, offsets, order);
+  return sstb_sir_group_csr(c, g, (const long long*)inv, N, G);
 }
 
 int sstb_sir_rel_dev(sstb200_ctx* c, const sstb200_sir_layer* L, RelDev* rd, size_t* smem_out) {
@@ -263,18 +264,24 @@ static void sir_group_max(sstb200_ctx* c, const float* src, int C, const int32_t
   launch_pdl(segmax_finalize_kernel, dim3((unsigned)((gn + 255) / 256)), dim3(256), (size_t)(0), st, (const uint32_t*)gord, G, C, out_group, Cg, col0);
 }
 
+// scratch of the fp32 forward; t (the pre-LayerNorm values) only in eval, training keeps them in the state
+struct SirFp32Ws {
+  float *x0, *t, *p0;
+};
+static void sir_fp32_carve(Carve& cv, SirFp32Ws& w, int N, int cin, int Cmax, bool train) {
+  w.x0 = cv.take<float>((size_t)N * cin);
+  w.t = train ? nullptr : cv.take<float>((size_t)N * Cmax);
+  w.p0 = cv.take<float>((size_t)N * Cmax);
+}
+
 // The fp32 forward.  s == NULL: eval.  s != NULL: training - t0 / t1 land in the state, the group maxima record their arg-max
 // rows there (off = the group CSR offsets), everything else is the same launch sequence.
 static int sir_forward_fp32(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster, const long long* inv,
-                            int N, int G, const int32_t* off, const int32_t* order, uint32_t* gord, float* gterm, float* out_point,
-                            float* out_group, const SirState* s) {
+                            int N, int G, const int32_t* off, const int32_t* order, uint32_t* gord, float* gterm, const SirFp32Ws& w,
+                            float* out_point, float* out_group, const SirState* s) {
   cudaStream_t st = c->stream;
   const int cin = L->in_channels, C0 = L->feat_channels[0], C1 = L->num_vfe > 1 ? L->feat_channels[1] : 0;
-  const int Cmax = C0 > C1 ? C0 : C1;
-  float* x0 = arena_alloc<float>(c, (size_t)N * cin);
-  float* t = s ? nullptr : arena_alloc<float>(c, (size_t)N * Cmax);
-  float* p0 = arena_alloc<float>(c, (size_t)N * Cmax);
-  if (!x0 || (!s && !t) || !p0) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
+  float *x0 = w.x0, *t = w.t, *p0 = w.p0;
   float* t0 = s ? s->t0 : t;
   float* t1 = s ? s->t1 : t;
 
@@ -328,7 +335,7 @@ int sstb_sir_train_check(sstb200_ctx* c, const sstb200_sir_layer* L) {
 
 extern "C" size_t sstb200_sir_layer_train_state_bytes(const sstb200_sir_layer* L, int N, int G) {
   if (!L || N < 0 || G < 0 || L->num_vfe < 1 || L->num_vfe > 2) return 0;
-  return sir_state_layout(N, G, L->feat_channels[0], L->num_vfe > 1 ? L->feat_channels[1] : 0, nullptr, nullptr);
+  return sir_state_bytes(N, G, L->feat_channels[0], L->num_vfe > 1 ? L->feat_channels[1] : 0);
 }
 
 extern "C" int sstb200_sir_layer_forward_train(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster,
@@ -342,28 +349,31 @@ extern "C" int sstb200_sir_layer_forward_train(sstb200_ctx* c, const sstb200_sir
   CHECK_ARG(c, (csr_offsets == nullptr) == (csr_order == nullptr));
   const int cin = L->in_channels, C0 = L->feat_channels[0], C1 = L->num_vfe > 1 ? L->feat_channels[1] : 0;
   const int Cmax = C0 > C1 ? C0 : C1;
+  const size_t need = sir_state_bytes(N, G, C0, C1);
+  if (state_bytes < need)
+    return sstb_fail(c, SSTB_ERR_WORKSPACE, "SIRLayer training state: %zu bytes given, %zu needed", state_bytes, need);
   SirState s;
-  if (state_bytes < sir_state_layout(N, G, C0, C1, state, &s))
-    return sstb_fail(c, SSTB_ERR_WORKSPACE, "SIRLayer training state: %zu bytes given, %zu needed", state_bytes,
-                     sir_state_layout(N, G, C0, C1, nullptr, nullptr));
+  Carve sc{(char*)state, 0};
+  sir_state_carve(sc, s, N, G, C0, C1);
   arena_reset(c);
-  rc = arena_reserve(c, csr_bytes(N, G) + al256((size_t)G * 4 + 8) + al256((size_t)N * cin * 4) + al256((size_t)N * Cmax * 4) +
-                            2 * al256((size_t)G * Cmax * 4) + 2 * al256(((size_t)N + 4) * 4) + 65536);
+  SirGroupCsr gc;
+  uint32_t* gord;
+  float* gterm;
+  SirFp32Ws w;
+  rc = arena_carve(c, [&](Carve& cv) {
+    if (!csr_order) sstb_sir_group_csr_carve(cv, gc, N, G);
+    gord = cv.take<uint32_t>((size_t)G * Cmax);
+    gterm = cv.take<float>((size_t)G * Cmax);
+    sir_fp32_carve(cv, w, N, cin, Cmax, true);
+  });
   if (rc) return rc;
   const int32_t *off = csr_offsets, *order = csr_order;
   if (!order) {
-    int32_t* o = arena_alloc<int32_t>(c, (size_t)G + 2);
-    int32_t* ord = arena_alloc<int32_t>(c, (size_t)N + 1);
-    if (!o || !ord) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
-    rc = group_csr(c, (const long long*)inv, N, G, o, ord);
-    if (rc) return rc;
-    off = o;
-    order = ord;
+    if ((rc = sstb_sir_group_csr(c, gc, (const long long*)inv, N, G))) return rc;
+    off = (const int32_t*)gc.csr.offsets;
+    order = gc.csr.order;
   }
-  uint32_t* gord = arena_alloc<uint32_t>(c, (size_t)G * Cmax);
-  float* gterm = arena_alloc<float>(c, (size_t)G * Cmax);
-  if (!gord || !gterm) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
-  return sir_forward_fp32(c, L, in_feats, f_cluster, (const long long*)inv, N, G, off, order, gord, gterm, out_point, out_group, &s);
+  return sir_forward_fp32(c, L, in_feats, f_cluster, (const long long*)inv, N, G, off, order, gord, gterm, w, out_point, out_group, &s);
 }
 
 int sstb_sir_layer_bf16(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster, const long long* inv,
@@ -396,28 +406,29 @@ extern "C" int sstb200_sir_layer_forward_ex(sstb200_ctx* c, const sstb200_sir_la
   CHECK_ARG(c, in_gap >= 0 && in_gap_at >= 0 && in_gap_at <= cin && in_ld >= cin + in_gap);
   if (!bf16 && (out_point_ld != Clast || in_ld != cin || in_gap != 0))
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "SIRLayer fp32 path works on dense point features (ld == C, no gap)");
+  // kernel B of the bf16 path reads the pooled layer-0 features back from out_group as float4
+  if (bf16) CHECK_ARG(c, ((uintptr_t)out_group & 15) == 0);
   arena_reset(c);
-  int rc = arena_reserve(c, csr_bytes(N, G) + al256((size_t)G * 4 + 8) + al256((size_t)N * cin * 4) + 2 * al256((size_t)N * Cmax * 4) +
-                                2 * al256((size_t)G * Cmax * 4) + al256(((size_t)N + 4) * 4) + 65536);
+  SirGroupCsr gc;
+  uint32_t* gord;
+  float* gterm;
+  __nv_bfloat16* p0buf = nullptr;
+  SirFp32Ws w;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    if (!csr_order) sstb_sir_group_csr_carve(cv, gc, N, G);
+    gord = cv.take<uint32_t>((size_t)G * Cmax);
+    gterm = cv.take<float>((size_t)G * Cmax);
+    if (bf16) p0buf = cv.take<__nv_bfloat16>(((size_t)N + 128) * 128);
+    else sir_fp32_carve(cv, w, N, cin, Cmax, false);
+  });
   if (rc) return rc;
   cudaStream_t st = c->stream;
   const int32_t* order = csr_order;
   if (!order) {
-    int32_t* off = arena_alloc<int32_t>(c, (size_t)G + 2);
-    int32_t* ord = arena_alloc<int32_t>(c, (size_t)N + 1);
-    if (!off || !ord) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
-    rc = group_csr(c, (const long long*)inv, N, G, off, ord);
-    if (rc) return rc;
-    order = ord;
+    if ((rc = sstb_sir_group_csr(c, gc, (const long long*)inv, N, G))) return rc;
+    order = gc.csr.order;
   }
-  uint32_t* gord = arena_alloc<uint32_t>(c, (size_t)G * Cmax);
-  float* gterm = arena_alloc<float>(c, (size_t)G * Cmax);
-  if (!gord || !gterm) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
   if (bf16) {
-    // kernel B reads the pooled layer-0 features back from out_group as float4
-    CHECK_ARG(c, ((uintptr_t)out_group & 15) == 0);
-    __nv_bfloat16* p0buf = arena_alloc<__nv_bfloat16>(c, ((size_t)N + 128) * 128);
-    if (!p0buf) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir: arena");
     rc = sstb_sir_layer_bf16(c, L, in_feats, f_cluster, (const long long*)inv, order, N, G, p0buf, gord, gterm, out_point, out_point_ld, out_group, in_ld, in_gap_at,
                              in_gap);
     if (rc) return rc;
@@ -428,7 +439,7 @@ extern "C" int sstb200_sir_layer_forward_ex(sstb200_ctx* c, const sstb200_sir_la
     LAUNCH_CHECK(c);
     return SSTB_OK;
   }
-  return sir_forward_fp32(c, L, in_feats, f_cluster, (const long long*)inv, N, G, nullptr, order, gord, gterm, out_point, out_group, nullptr);
+  return sir_forward_fp32(c, L, in_feats, f_cluster, (const long long*)inv, N, G, nullptr, order, gord, gterm, w, out_point, out_group, nullptr);
 }
 
 extern "C" int sstb200_sir_layer_forward(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster,

@@ -1,6 +1,6 @@
 // SIRLayer pieces shared by the forward (sir.cu) and the training backward (sir_train.cu).
 #pragma once
-#include "common.cuh"
+#include "index.cuh"
 
 // relation-MLP parameters as the warp-per-point kernels read them
 struct RelDev {
@@ -22,25 +22,31 @@ struct SirState {
   long long* am0;  // [G, C0]
   long long* am1;  // [G, C1] (C1 > 0)
 };
-static inline size_t sir_state_layout(int N, int G, int C0, int C1, void* base, SirState* s) {
-  size_t o0 = 0, o1 = o0 + al256((size_t)N * C0 * 4), o2 = o1 + al256((size_t)N * C1 * 4), o3 = o2 + al256((size_t)G * C0 * 8);
-  size_t end = o3 + al256((size_t)G * C1 * 8);
-  if (s) {
-    char* b = (char*)base;
-    s->t0 = (float*)(b + o0);
-    s->t1 = C1 ? (float*)(b + o1) : nullptr;
-    s->am0 = (long long*)(b + o2);
-    s->am1 = C1 ? (long long*)(b + o3) : nullptr;
-  }
-  return end;
+static inline void sir_state_carve(Carve& cv, SirState& s, int N, int G, int C0, int C1) {
+  s.t0 = cv.take<float>((size_t)N * C0);
+  s.t1 = C1 ? cv.take<float>((size_t)N * C1) : nullptr;
+  s.am0 = cv.take<long long>((size_t)G * C0);
+  s.am1 = C1 ? cv.take<long long>((size_t)G * C1) : nullptr;
+}
+static inline size_t sir_state_bytes(int N, int G, int C0, int C1) {
+  return carve_bytes([&](Carve& cv) {
+    SirState s;
+    sir_state_carve(cv, s, N, G, C0, C1);
+  });
 }
 
 // fills `rd` from the layer and checks the rel-MLP (SSTB_OK or an error code with the message set); *smem = its weight bytes
 int sstb_sir_rel_dev(sstb200_ctx* c, const sstb200_sir_layer* L, RelDev* rd, size_t* smem);
 // x0 = [xyz / xyz_normalizer || rest] * rel_mlp(f_cluster / rel_dist_scaler)   [N, cin]
 int sstb_sir_rel_gate(sstb200_ctx* c, const sstb200_sir_layer* L, const float* in_feats, const float* f_cluster, int N, float* x0);
-// group CSR into caller buffers (offsets [G+2], order [N+1]) from the arena-reserved context, as sstb200_group_csr builds it
-int sstb_sir_group_csr(sstb200_ctx* c, const long long* inv, int N, int G, int32_t* offsets, int32_t* order);
+// group CSR (offsets [G+1] int32 in csr.offsets, order [N] int32 in csr.order) of the points grouped by `inv`, as sstb200_group_csr
+// builds it: carve, then build
+struct SirGroupCsr {
+  int32_t* count;  // [G + 2]: per-group counts, then an error flag
+  Csr csr;
+};
+void sstb_sir_group_csr_carve(Carve& cv, SirGroupCsr& g, int N, int G);
+int sstb_sir_group_csr(sstb200_ctx* c, SirGroupCsr& g, const long long* inv, int N, int G);
 // the range the fp32 training path covers (SSTB_ERR_UNSUPPORTED / SSTB_ERR_ARG with a message otherwise)
 int sstb_sir_train_check(sstb200_ctx* c, const sstb200_sir_layer* L);
 // out[g, col0 + c] = the group max that ord[g, c] holds in order-preserving form (0, an empty group, gives 0)

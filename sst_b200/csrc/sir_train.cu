@@ -424,10 +424,12 @@ extern "C" int sstb200_sir_layer_backward(sstb200_ctx* c, const sstb200_sir_laye
   const int Cg = C0 + C1, Clast = C1 ? C1 : C0;
   for (int l = 0; l < L->num_rel; l++) CHECK_ARG(c, grads->rel_w[l] && grads->rel_ln_w[l] && grads->rel_ln_b[l]);
   for (int l = 0; l < L->num_vfe; l++) CHECK_ARG(c, grads->vfe_w[l] && grads->vfe_ln_w[l] && grads->vfe_ln_b[l] && L->vfe_w[l]);
+  const size_t need = sir_state_bytes(N, G, C0, C1);
+  if (state_bytes < need)
+    return sstb_fail(c, SSTB_ERR_WORKSPACE, "SIRLayer training state: %zu bytes given, %zu needed", state_bytes, need);
   SirState s;
-  if (state_bytes < sir_state_layout(N, G, C0, C1, (void*)state, &s))
-    return sstb_fail(c, SSTB_ERR_WORKSPACE, "SIRLayer training state: %zu bytes given, %zu needed", state_bytes,
-                     sir_state_layout(N, G, C0, C1, nullptr, nullptr));
+  Carve sc{(char*)state, 0};
+  sir_state_carve(sc, s, N, G, C0, C1);
   RelDev rd;
   size_t wsmem = 0;
   if ((rc = sstb_sir_rel_dev(c, L, &rd, &wsmem))) return rc;
@@ -457,33 +459,42 @@ extern "C" int sstb200_sir_layer_backward(sstb200_ctx* c, const sstb200_sir_laye
     for (int l = 0; l < L->num_rel; l++) upd(N, L->rel_dims[l], in), in = L->rel_dims[l];
   }
   const size_t Nf = (size_t)N;
-  size_t need = csr_bytes(N, G) + al256((size_t)G * 4 + 8) + 3 * al256((size_t)256 * 256 * 4) + 2 * al256(Nf * cin * 4) +
-                4 * al256(Nf * C0 * 4) + 2 * al256(Nf * C1 * 4) + 4 * al256((size_t)G * 256 * 4) + al256(Nf * a_tot * 4) +
-                al256(Nf * dz_tot * 4) + al256(dw_part * 8) + al256((size_t)ln_blocks * 512 * 4) + al256((size_t)rel_blocks * ln_tot * 4) + 65536;
   arena_reset(c);
-  if ((rc = arena_reserve(c, need))) return rc;
+  SirGroupCsr gc;
+  float *W0t, *x0, *dx0, *dP0, *dt0, *lnp, *relp, *abuf, *dzbuf;
+  double* part;
+  float *W1at = nullptr, *W1bt = nullptr, *p0 = nullptr, *g0 = nullptr, *dP1 = nullptr, *dt1 = nullptr, *S1 = nullptr, *dg0 = nullptr;
+  rc = arena_carve(c, [&](Carve& cv) {
+    if (!csr_order) sstb_sir_group_csr_carve(cv, gc, N, G);
+    W0t = cv.take<float>((size_t)cin * C0);
+    x0 = cv.take<float>(Nf * cin);
+    dx0 = cv.take<float>(Nf * cin);
+    dP0 = cv.take<float>(Nf * C0);
+    dt0 = cv.take<float>(Nf * C0);
+    part = cv.take<double>(dw_part);
+    lnp = cv.take<float>((size_t)ln_blocks * 2 * 256);
+    relp = cv.take<float>((size_t)rel_blocks * ln_tot);
+    abuf = cv.take<float>(Nf * a_tot);
+    dzbuf = cv.take<float>(Nf * dz_tot);
+    if (C1) {
+      W1at = cv.take<float>((size_t)C0 * C1);
+      W1bt = cv.take<float>((size_t)C0 * C1);
+      p0 = cv.take<float>(Nf * C0);
+      g0 = cv.take<float>((size_t)G * C0);
+      dP1 = cv.take<float>(Nf * C1);
+      dt1 = cv.take<float>(Nf * C1);
+      S1 = cv.take<float>((size_t)G * C1);
+      dg0 = cv.take<float>((size_t)G * C0);
+    }
+  });
+  if (rc) return rc;
   cudaStream_t st = c->stream;
   const int32_t *off = csr_offsets, *order = csr_order;
   if (!order) {
-    int32_t* o = arena_alloc<int32_t>(c, (size_t)G + 2);
-    int32_t* ord = arena_alloc<int32_t>(c, Nf + 1);
-    if (!o || !ord) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir backward: arena");
-    if ((rc = sstb_sir_group_csr(c, inv, N, G, o, ord))) return rc;
-    off = o;
-    order = ord;
+    if ((rc = sstb_sir_group_csr(c, gc, inv, N, G))) return rc;
+    off = (const int32_t*)gc.csr.offsets;
+    order = gc.csr.order;
   }
-  float* W0t = arena_alloc<float>(c, (size_t)cin * C0);
-  float* x0 = arena_alloc<float>(c, Nf * cin);
-  float* dx0 = arena_alloc<float>(c, Nf * cin);
-  float* dP0 = arena_alloc<float>(c, Nf * C0);
-  float* dt0 = arena_alloc<float>(c, Nf * C0);
-  double* part = arena_alloc<double>(c, dw_part);
-  float* lnp = arena_alloc<float>(c, (size_t)ln_blocks * 2 * 256);
-  float* relp = arena_alloc<float>(c, (size_t)rel_blocks * ln_tot);
-  float* abuf = arena_alloc<float>(c, Nf * a_tot);
-  float* dzbuf = arena_alloc<float>(c, Nf * dz_tot);
-  if (!W0t || !x0 || !dx0 || !dP0 || !dt0 || !part || !lnp || !relp || !abuf || !dzbuf)
-    return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir backward: arena");
 
   auto blocks = [](size_t n) { return dim3((unsigned)((n + 255) / 256)); };
   auto ln_bwd = [&](const float* t, const float* dy, int d, int l, float* dt) {
@@ -500,15 +511,6 @@ extern "C" int sstb200_sir_layer_backward(sstb200_ctx* c, const sstb200_sir_laye
 
   // dP1 / dP0: the gradient at each layer's activation output (the shortcut's share goes straight to in_feats below)
   if (C1) {
-    float* W1at = arena_alloc<float>(c, (size_t)C0 * C1);
-    float* W1bt = arena_alloc<float>(c, (size_t)C0 * C1);
-    float* p0 = arena_alloc<float>(c, Nf * C0);
-    float* g0 = arena_alloc<float>(c, (size_t)G * C0);
-    float* dP1 = arena_alloc<float>(c, Nf * C1);
-    float* dt1 = arena_alloc<float>(c, Nf * C1);
-    float* S1 = arena_alloc<float>(c, (size_t)G * C1);
-    float* dg0 = arena_alloc<float>(c, (size_t)G * C0);
-    if (!W1at || !W1bt || !p0 || !g0 || !dP1 || !dt1 || !S1 || !dg0) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sir backward: arena");
     launch_pdl(sirb_transpose_kernel, blocks((size_t)C1 * C0), dim3(256), (size_t)0, st, L->vfe_w[1], 2 * C0, C1, C0, W1at);
     launch_pdl(sirb_transpose_kernel, blocks((size_t)C1 * C0), dim3(256), (size_t)0, st, L->vfe_w[1] + C0, 2 * C0, C1, C0, W1bt);
     // p0 and g0 as the forward had them

@@ -680,11 +680,10 @@ extern "C" int sstb200_spconv_out_coors(sstb200_ctx* c, const int32_t* in_coors,
   rc = sp_extents(c, e, &T, batch_size, g.out_shape);
   if (rc) return rc;
   arena_reset(c);
-  rc = arena_reserve(c, key_index_bytes(1, T) + 4096);
-  if (rc) return rc;
   KeyIndex k;
-  rc = key_index_alloc(c, k, 1, T);
+  rc = arena_carve(c, [&](Carve& cv) { key_index_carve(cv, k, 1, T); });
   if (rc) return rc;
+  if ((rc = key_index_zero(c, k))) return rc;
   const long long work = (long long)n_in * g.KV;
   launch_pdl(sp_mark_out_kernel, dim3((unsigned)((work + 255) / 256)), dim3(256), (size_t)0, c->stream, in_coors, n_in, g, k.bitmap, k.flags);
   key_index_scan(c, k);
@@ -723,15 +722,21 @@ extern "C" int sstb200_spconv_table(sstb200_ctx* c, const int32_t* in_coors, int
   rc = sp_extents(c, eo, &To, batch_size, g.out_shape);
   if (rc) return rc;
   arena_reset(c);
-  rc = arena_reserve(c, key_index_bytes(n_in, Ti) + key_index_bytes(n_out, To) + al256((size_t)n_in * 4) + al256((size_t)n_out * 4) + 8192);
-  if (rc) return rc;
   KeyIndex ki, ko;
   int32_t *perm_i = nullptr, *perm_o = nullptr;
+  rc = arena_carve(c, [&](Carve& cv) {
+    if (nbr) {
+      key_index_carve(cv, ki, n_in, Ti);
+      perm_i = cv.take<int32_t>(n_in);
+    }
+    if (nbr_inv) {
+      key_index_carve(cv, ko, n_out, To);
+      perm_o = cv.take<int32_t>(n_out);
+    }
+  });
+  if (rc) return rc;
   if (nbr) {
-    rc = key_index_alloc(c, ki, n_in, Ti);
-    if (rc) return rc;
-    perm_i = arena_alloc<int32_t>(c, n_in);
-    if (!perm_i) return sstb_fail(c, SSTB_ERR_WORKSPACE, "spconv_table: arena too small");
+    if ((rc = key_index_zero(c, ki))) return rc;
     launch_mark_rows<int32_t>(c, in_coors, n_in, ei, false, ki, nullptr);
     key_index_scan(c, ki);
     launch_pdl(sp_perm_kernel, dim3((n_in + 255) / 256), dim3(256), (size_t)0, c->stream, (const long long*)ki.keys, n_in, (const int32_t*)nullptr,
@@ -741,10 +746,7 @@ extern "C" int sstb200_spconv_table(sstb200_ctx* c, const int32_t* in_coors, int
                (const uint32_t*)ki.word_prefix, (const int32_t*)perm_i, nbr);
   }
   if (nbr_inv) {
-    rc = key_index_alloc(c, ko, n_out, To);
-    if (rc) return rc;
-    perm_o = arena_alloc<int32_t>(c, n_out);
-    if (!perm_o) return sstb_fail(c, SSTB_ERR_WORKSPACE, "spconv_table: arena too small");
+    if ((rc = key_index_zero(c, ko))) return rc;
     launch_mark_rows<int32_t>(c, out_coors, n_out, eo, false, ko, nullptr);
     key_index_scan(c, ko);
     launch_pdl(sp_perm_kernel, dim3((n_out + 255) / 256), dim3(256), (size_t)0, c->stream, (const long long*)ko.keys, n_out, (const int32_t*)nullptr,
@@ -797,10 +799,9 @@ extern "C" int sstb200_spconv_forward(sstb200_ctx* c, const float* feats, int n_
                      "use precision fp32", SPU_MAX_KV, c_in, c_out, kernel_volume);
   // per-row exponents of feats: one small launch (reads feats once; the convolution gathers it kernel_volume times)
   arena_reset(c);
-  int rc = arena_reserve(c, al256((size_t)n_in * 4) + 4096);
+  int32_t* rexp;
+  int rc = arena_carve(c, [&](Carve& cv) { rexp = cv.take<int32_t>((size_t)n_in + 1); });
   if (rc) return rc;
-  int32_t* rexp = arena_alloc<int32_t>(c, (size_t)n_in + 1);
-  if (!rexp) return sstb_fail(c, SSTB_ERR_WORKSPACE, "spconv_forward: arena too small");
   if (n_in) launch_pdl(sp_row_exp_kernel, dim3((n_in + 7) / 8), dim3(256), (size_t)0, c->stream, feats, c_in, c_in, n_in, (const int32_t*)nullptr, rexp);
   SpArgs g;
   g.feats = feats, g.rexp = rexp, g.self_exp = 0, g.wun = weight_h16_unscale;
@@ -820,10 +821,15 @@ int sstb_row_gemm_x3(sstb200_ctx* c, const RowGemm& r) {
   const int N = r.N, K = r.K;
   if ((K & 63) || (N & 63) || (r.lda & 3) || (r.ldo & 3) || (r.ldr & 3) || (r.act == 1 && r.res)) return SSTB_ERR_UNSUPPORTED;
   if ((r.ldw && r.ldw != K) || r.res_index || r.pos.tab) return SSTB_ERR_UNSUPPORTED;   // forms only the FFMA row GEMM takes
-  __half* hi = arena_alloc<__half>(c, (size_t)N * K);
-  __half* lo = arena_alloc<__half>(c, (size_t)N * K);
-  float* wun = arena_alloc<float>(c, (size_t)N);
-  if (!hi || !lo || !wun) return sstb_fail(c, SSTB_ERR_WORKSPACE, "row_gemm_x3: arena too small");
+  // the split weights are carved after what the caller's phase already holds, without a reset
+  __half *hi, *lo;
+  float* wun;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    hi = cv.take<__half>((size_t)N * K);
+    lo = cv.take<__half>((size_t)N * K);
+    wun = cv.take<float>(N);
+  });
+  if (rc) return rc;
   launch_pdl(split_f16_rows_kernel, dim3((unsigned)N), dim3(256), (size_t)0, c->stream, r.W, K, hi, lo, wun);
   SpArgs g;
   g.rexp = nullptr, g.self_exp = 1, g.wun = wun;

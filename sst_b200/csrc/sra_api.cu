@@ -13,9 +13,6 @@ extern "C" int sstb200_sra_layer_forward(sstb200_ctx* c, const sstb200_sra_layer
   CHECK_ARG(c, P->win_offsets && P->tok_perm && P->tok_win);
   CHECK_ARG(c, P->pos_table == nullptr || (P->pos_code && P->pos_L > 0 && P->pos_maxw > 0 && P->pos_ndim >= 1 && P->pos_ndim <= 3));
   arena_reset(c);
-  size_t d = L->d_model, ff = L->dim_ff;
-  int rc = arena_reserve(c, (size_t)n * (6 * d + ff) * 4 + (size_t)n * (6 * d + ff) * 2 + (1 << 20));
-  if (rc) return rc;
   if (precision == SSTB200_PREC_FP32) return sstb_sra_layer_fp32(c, L, P, x, y, n, n_dev);
   if (precision == SSTB200_PREC_BF16) return sstb_sra_layer_bf16(c, L, P, x, y, n, n_dev);
   return sstb_fail(c, SSTB_ERR_ARG, "unknown precision %d", precision);
@@ -42,9 +39,7 @@ extern "C" int sstb200_sra_stack_forward(sstb200_ctx* c, const sstb200_sra_layer
   sstb200_sra_plan plans[2] = {*plan_shift0, *plan_shift1};
   if (precision == SSTB200_PREC_BF16) {
     arena_reset(c);
-    int rc = arena_reserve(c, (size_t)n * 128 * 8 + (size_t)num_layers * 4 * 128 * 4 + (1 << 20));
-    if (rc) return rc;
-    rc = sstb_sra_stack_bf16(c, layers, num_layers, plans, x, y, tmp, n, n_dev);
+    int rc = sstb_sra_stack_bf16(c, layers, num_layers, plans, x, y, tmp, n, n_dev);
     if (rc != SSTB_ERR_UNSUPPORTED) return rc;
   }
   // generic path: layer by layer, ping-pong between tmp and y so that the last layer lands in y

@@ -60,15 +60,18 @@ int sstb_sra_layer_bf16(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb20
     return sstb_fail(c, SSTB_ERR_ARG, "the tensor-core path needs the *_w_f16 weight copies");
   if (P->pos_table && P->pos_L % 8 != 0)
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "bf16 path needs the per-axis positional length (%d) to be a multiple of 8", P->pos_L);
-  __half* qkv = arena_alloc<__half>(c, (size_t)n_cap * 3 * d);
-  __half* att = arena_alloc<__half>(c, (size_t)n_cap * d);
-  if (!qkv || !att) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sra bf16 layer: arena too small");
+  __half *qkv, *att;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    qkv = cv.take<__half>((size_t)n_cap * 3 * d);
+    att = cv.take<__half>((size_t)n_cap * d);
+  });
+  if (rc) return rc;
   // tensor-core attention path: plain scaled-dot-product, 8 heads x 16, windows <= 144 tokens
   const bool tc_attn = L->nhead == 8 && (!L->tau || L->tau_n == 1 || L->tau_n == 8) && P->max_window_tokens > 0 && P->max_window_tokens <= ATT_MAXT &&
                        P->num_windows_dev && P->win_batch;
   // 1. QKV projection, fp16 q/k/v for either attention kernel (softmax logits need the mantissa: with bf16 q,k the logit error
   // would dominate the layer's error budget).
-  int rc = qkv_gemm(c, L, P, x, qkv, n_cap, n_dev, tc_attn);
+  rc = qkv_gemm(c, L, P, x, qkv, n_cap, n_dev, tc_attn);
   if (rc) return rc;
   // 2. ragged window attention (fp32 math on bf16 q/k/v)
   if (tc_attn)
@@ -102,17 +105,18 @@ int sstb_sra_stack_bf16(sstb200_ctx* c, const sstb200_sra_layer* layers, int num
     if (!layer_supported_tc(&layers[l], &plans[l & 1])) return SSTB_ERR_UNSUPPORTED;  // caller falls back to per-layer calls
   const int d = 128;
   if (num_layers > SSTB_MAX_STACK) return SSTB_ERR_UNSUPPORTED;
-  __half* qkv = arena_alloc<__half>(c, (size_t)n_cap * 3 * d);
-  __half* att = arena_alloc<__half>(c, (size_t)n_cap * d);
   bool any_bn = false;
   for (int l = 0; l < num_layers; l++) any_bn |= layers[l].norm1_mean != nullptr;
-  float* bn_fold = any_bn ? arena_alloc<float>(c, (size_t)num_layers * 4 * 128) : nullptr;
-  if (!qkv || !att || (any_bn && !bn_fold)) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sra stack: arena too small");
-  if (any_bn) {
-    int rc = sstb_sra_bn_fold(c, layers, num_layers, bn_fold);
-    if (rc) return rc;
-  }
-  int rc = qkv_gemm(c, &layers[0], &plans[0], x, qkv, n_cap, n_dev, true);
+  __half *qkv, *att;
+  float* bn_fold = nullptr;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    qkv = cv.take<__half>((size_t)n_cap * 3 * d);
+    att = cv.take<__half>((size_t)n_cap * d);
+    if (any_bn) bn_fold = cv.take<float>((size_t)num_layers * 4 * 128);
+  });
+  if (rc) return rc;
+  if (any_bn && (rc = sstb_sra_bn_fold(c, layers, num_layers, bn_fold))) return rc;
+  rc = qkv_gemm(c, &layers[0], &plans[0], x, qkv, n_cap, n_dev, true);
   if (rc) return rc;
   const float* xin = x;
   for (int l = 0; l < num_layers; l++) {

@@ -37,12 +37,16 @@ int sstb_sra_layer_fp32(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb20
                         int n_cap, const int32_t* n_dev) {
   int d = L->d_model, ff = L->dim_ff;
   if (d > 256 || d % 32) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "d_model %d (need multiple of 32, <= 256)", d);
-  float* qkv = arena_alloc<float>(c, (size_t)n_cap * 3 * d);
-  float* att = arena_alloc<float>(c, (size_t)n_cap * d);
-  float* t1 = arena_alloc<float>(c, (size_t)n_cap * d);
-  float* x1 = arena_alloc<float>(c, (size_t)n_cap * d);
-  float* hid = arena_alloc<float>(c, (size_t)n_cap * ff);
-  if (!qkv || !att || !t1 || !x1 || !hid) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sra layer: arena too small");
+  float *qkv, *att, *t1, *x1, *hid, *xpos = nullptr;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    qkv = cv.take<float>((size_t)n_cap * 3 * d);
+    att = cv.take<float>((size_t)n_cap * d);
+    t1 = cv.take<float>((size_t)n_cap * d);
+    x1 = cv.take<float>((size_t)n_cap * d);
+    hid = cv.take<float>((size_t)n_cap * ff);
+    if (d % 64 == 0 && ff % 64 == 0 && P->pos_table) xpos = cv.take<float>((size_t)n_cap * d);  // q|k input of the x3 route
+  });
+  if (rc) return rc;
   cudaStream_t st = c->stream;
   const float* xin = x;
   if (!L->post_norm) {  // pre-norm: src2 = norm1(src)
@@ -53,12 +57,9 @@ int sstb_sra_layer_fp32(sstb200_ctx* c, const sstb200_sra_layer* L, const sstb20
   base.M_cap = n_cap, base.M_dev = n_dev;
   const PosTab pt{P->pos_table, P->pos_code, P->pos_L, P->pos_maxw, P->pos_ndim};
   // q,k from (x + pos); v from x
-  int rc = SSTB_OK;
   if (d % 64 == 0 && ff % 64 == 0) {
     const float* xqk = xin;
     if (P->pos_table) {
-      float* xpos = arena_alloc<float>(c, (size_t)n_cap * d);
-      if (!xpos) return sstb_fail(c, SSTB_ERR_WORKSPACE, "sra layer: arena too small");
       const size_t tot = (size_t)n_cap * d;
       launch_pdl(add_pos_kernel, dim3((unsigned)((tot + 255) / 256)), dim3(256), (size_t)0, st, xin, d, pt, xpos, n_cap, n_dev);
       xqk = xpos;

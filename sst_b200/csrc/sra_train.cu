@@ -27,42 +27,51 @@ namespace {
 
 constexpr int DM = 128, DFF = 256;
 
-struct TrainWs {   // per-layer saved tensors (byte offsets from the layer's base)
-  size_t y, qkv, att, t1, x1, x1b, z, h, t2, layer_bytes;
+struct TrainLayerWs {   // one layer's saved tensors
+  float* y;
+  __half* qkv;
+  __nv_bfloat16* att;
+  float *t1, *x1;
+  __nv_bfloat16 *x1b, *z, *h;
+  float* t2;
+};
+struct TrainWs {
+  std::vector<TrainLayerWs> layer;
   // shared backward temporaries (after all layers)
-  size_t dt, dtb, dzb, dattb, dqkv, dx1, dxa, dxb, stats, total;
+  float* dt;
+  __nv_bfloat16 *dtb, *dzb, *dattb, *dqkv;
+  float *dx1, *dxa, *dxb, *stats;
 };
 
-static TrainWs train_ws(int n, int L) {
-  TrainWs w;
-  size_t o = 0;
-  auto take = [&](size_t bytes) {
-    size_t r = o;
-    o += al256(bytes);
-    return r;
-  };
+static void train_ws_carve(Carve& cv, TrainWs& w, int n, int L) {
   const size_t N = (size_t)n;
-  w.y = take(N * DM * 4);
-  w.qkv = take(N * 3 * DM * 2);
-  w.att = take(N * DM * 2);
-  w.t1 = take(N * DM * 4);
-  w.x1 = take(N * DM * 4);
-  w.x1b = take(N * DM * 2);
-  w.z = take(N * DFF * 2);
-  w.h = take(N * DFF * 2);
-  w.t2 = take(N * DM * 4);
-  w.layer_bytes = o;
-  o = w.layer_bytes * (size_t)L;
-  w.dt = take(N * DM * 4);
-  w.dtb = take(N * DM * 2);
-  w.dzb = take(N * DFF * 2);
-  w.dattb = take(N * DM * 2);
-  w.dqkv = take(N * 3 * DM * 2);
-  w.dx1 = take(N * DM * 4);
-  w.dxa = take(N * DM * 4);
-  w.dxb = take(N * DM * 4);
-  w.stats = take(N * 8 * 3 * 4);
-  w.total = o;
+  w.layer.resize(L);
+  for (TrainLayerWs& l : w.layer) {
+    l.y = cv.take<float>(N * DM);
+    l.qkv = cv.take<__half>(N * 3 * DM);
+    l.att = cv.take<__nv_bfloat16>(N * DM);
+    l.t1 = cv.take<float>(N * DM);
+    l.x1 = cv.take<float>(N * DM);
+    l.x1b = cv.take<__nv_bfloat16>(N * DM);
+    l.z = cv.take<__nv_bfloat16>(N * DFF);
+    l.h = cv.take<__nv_bfloat16>(N * DFF);
+    l.t2 = cv.take<float>(N * DM);
+  }
+  w.dt = cv.take<float>(N * DM);
+  w.dtb = cv.take<__nv_bfloat16>(N * DM);
+  w.dzb = cv.take<__nv_bfloat16>(N * DFF);
+  w.dattb = cv.take<__nv_bfloat16>(N * DM);
+  w.dqkv = cv.take<__nv_bfloat16>(N * 3 * DM);
+  w.dx1 = cv.take<float>(N * DM);
+  w.dxa = cv.take<float>(N * DM);
+  w.dxb = cv.take<float>(N * DM);
+  w.stats = cv.take<float>(N * 8 * 3);
+}
+
+static TrainWs train_ws(void* workspace, int n, int L) {
+  TrainWs w;
+  Carve cv{(char*)workspace, 0};
+  train_ws_carve(cv, w, n, L);
   return w;
 }
 
@@ -156,10 +165,9 @@ static int launch_ln_bwd(sstb200_ctx* c, const float* dy, const float* t, const 
   const int grid = c->num_sms * 2;
   // per-block partials in the arena; the reduce is enqueued before any later arena_reset can hand the memory out again
   arena_reset(c);
-  int rc = arena_reserve(c, (size_t)grid * 3 * DM * 4);
+  float* part;
+  int rc = arena_carve(c, [&](Carve& cv) { part = cv.take<float>((size_t)grid * 3 * DM); });
   if (rc) return rc;
-  float* part = arena_alloc<float>(c, (size_t)grid * 3 * DM);
-  if (!part) return sstb_fail(c, SSTB_ERR_WORKSPACE, "LayerNorm partials: arena");
   CUDA_TRY(c, launch_pdl(ln_bwd_kernel, dim3(grid), dim3(256), (size_t)0, c->stream, dy, t, gamma, eps, n, dt, dtb, part));
   CUDA_TRY(c, launch_pdl(ln_reduce_kernel, dim3(3 * DM / 32), dim3(256), (size_t)0, c->stream, (const float*)part, grid, dgamma, dbeta, dbias));
   return SSTB_OK;
@@ -361,12 +369,12 @@ static int launch_dw(sstb200_ctx* c, const __nv_bfloat16* dY, int ldy, int n_out
   const int max_splits = (n + DW_ROWS - 1) / DW_ROWS;
   if (g.splits > max_splits) g.splits = max_splits < 1 ? 1 : max_splits;
   arena_reset(c);
-  int rc = arena_reserve(c, (size_t)g.splits * blocks * 128 * 128 * 4 + (size_t)g.splits * g.nb * 128 * 4 + 8192);
+  int rc = arena_carve(c, [&](Carve& cv) {
+    g.part = cv.take<float>((size_t)g.splits * blocks * 128 * 128);
+    g.part_b = db ? cv.take<float>((size_t)g.splits * g.nb * 128) : nullptr;
+  });
   if (rc) return rc;
-  g.part = arena_alloc<float>(c, (size_t)g.splits * blocks * 128 * 128);
-  g.part_b = db ? arena_alloc<float>(c, (size_t)g.splits * g.nb * 128) : nullptr;
   g.db = db;
-  if (!g.part || (db && !g.part_b)) return sstb_fail(c, SSTB_ERR_WORKSPACE, "dW partials: arena");
   const size_t smem = (size_t)4 * DW_ROWS * DW_PITCH * 2;
   static SmemAttr sa;
   CUDA_TRY(c, ensure_smem(c, sa, dw_gemm_kernel, smem));
@@ -702,10 +710,9 @@ static int launch_attn_bwd(sstb200_ctx* c, const __half* qkv, const __nv_bfloat1
   }
   // per-CTA temperature partials in the arena; the reduce is enqueued before any later arena_reset can hand the memory out again
   arena_reset(c);
-  int rc = arena_reserve(c, (size_t)grid * 8 * 4);
+  float* part;
+  int rc = arena_carve(c, [&](Carve& cv) { part = cv.take<float>((size_t)grid * 8); });
   if (rc) return rc;
-  float* part = arena_alloc<float>(c, (size_t)grid * 8);
-  if (!part) return sstb_fail(c, SSTB_ERR_WORKSPACE, "tau partials: arena");
   const size_t smem = attn_bwd_smem(true);
   static SmemAttr sb;
   CUDA_TRY(c, ensure_smem(c, sb, win_attn_bwd_kernel<true>, smem));
@@ -742,7 +749,10 @@ static bool layer_ok(const sstb200_sra_layer* L, const sstb200_sra_plan* P) {
 
 }  // namespace
 
-extern "C" size_t sstb200_sra_train_workspace_bytes(int n, int num_layers) { return train_ws(n < 1 ? 1 : n, num_layers).total; }
+extern "C" size_t sstb200_sra_train_workspace_bytes(int n, int num_layers) {
+  TrainWs w;
+  return carve_bytes([&](Carve& cv) { train_ws_carve(cv, w, n < 1 ? 1 : n, num_layers); });
+}
 
 // the 16-bit weight copies in `layers[].*_w_f16` are bf16 for this entry point (see the precision policy above)
 extern "C" int sstb200_sra_stack_forward_train(sstb200_ctx* c, const sstb200_sra_layer* layers, int num_layers,
@@ -756,39 +766,38 @@ extern "C" int sstb200_sra_stack_forward_train(sstb200_ctx* c, const sstb200_sra
       return sstb_fail(c, SSTB_ERR_UNSUPPORTED,
                        "training path is built for d_model=128, dim_ff=256, 8 heads, post-norm LayerNorm, gelu, plain or cosine attention "
                        "(1 or 8 temperatures, tau_min > 0), windows <= 144 tokens");
-  const TrainWs w = train_ws(n, num_layers);
-  uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
+  const TrainWs w = train_ws(workspace, n, num_layers);
   const float* xin = x;
   for (int l = 0; l < num_layers; l++) {
     const sstb200_sra_layer* L = &layers[l];
     const sstb200_sra_plan* P = &plans[l & 1];
-    uint8_t* lw = base + w.layer_bytes * (size_t)l;
-    float* y = l + 1 == num_layers ? y_out : reinterpret_cast<float*>(lw + w.y);
+    const TrainLayerWs& lw = w.layer[l];
+    float* y = l + 1 == num_layers ? y_out : lw.y;
     GemmArgs g;
     int rc;
     // 1. q|k|v (fp16 for the attention kernel) from bf16([x+pos | x])
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = xin, g.lda = DM, g.W = L->in_proj_w_f16, g.bias = L->in_proj_b;
     g.pos_tab = P->pos_table, g.pos_code = P->pos_code, g.posL = P->pos_L, g.pos_maxw = P->pos_maxw, g.pos_ndim = P->pos_ndim, g.pos_ntiles = 2;
-    g.out_h16 = lw + w.qkv, g.ldo = 3 * DM;
+    g.out_h16 = lw.qkv, g.ldo = 3 * DM;
     if ((rc = launch_wgmma_gemm<128, 128, PRO_F32, EPI_F16, FMT_BF16>(c, g, 3))) return rc;
     // 2. attention (bf16 output)
-    if ((rc = sstb_win_attn_batch(c, reinterpret_cast<const __half*>(lw + w.qkv), P->num_windows_dev, P->win_offsets, P->win_batch, n, P->tok_perm,
-                                  lw + w.att, /*out_bf16=*/true, L->tau, L->tau_n, L->tau_min)))
+    if ((rc = sstb_win_attn_batch(c, lw.qkv, P->num_windows_dev, P->win_offsets, P->win_batch, n, P->tok_perm,
+                                  lw.att, /*out_bf16=*/true, L->tau, L->tau_n, L->tau_min)))
       return rc;
     // 3. x1 = LN1(x + att Wo^T + bo), keep t1
     memset(&g, 0, sizeof(g));
-    g.M_cap = n, g.A = lw + w.att, g.lda = DM, g.W = L->out_proj_w_f16, g.bias = L->out_proj_b, g.res = xin, g.gamma = L->norm1_w, g.beta = L->norm1_b;
-    g.eps = L->norm_eps, g.out_f32 = reinterpret_cast<float*>(lw + w.x1), g.out_h16 = lw + w.x1b, g.ldo = DM, g.out_pre = reinterpret_cast<float*>(lw + w.t1);
+    g.M_cap = n, g.A = lw.att, g.lda = DM, g.W = L->out_proj_w_f16, g.bias = L->out_proj_b, g.res = xin, g.gamma = L->norm1_w, g.beta = L->norm1_b;
+    g.eps = L->norm_eps, g.out_f32 = lw.x1, g.out_h16 = lw.x1b, g.ldo = DM, g.out_pre = lw.t1;
     if ((rc = launch_wgmma_gemm<128, 128, PRO_H16, EPI_RES_LN, FMT_BF16>(c, g, 1))) return rc;
     // 4. h = GELU(z), z = x1 W1^T + b1
     memset(&g, 0, sizeof(g));
-    g.M_cap = n, g.A = lw + w.x1b, g.lda = DM, g.W = L->lin1_w_f16, g.bias = L->lin1_b, g.out_h16 = lw + w.h, g.out_pre16 = lw + w.z, g.ldo = DFF;
+    g.M_cap = n, g.A = lw.x1b, g.lda = DM, g.W = L->lin1_w_f16, g.bias = L->lin1_b, g.out_h16 = lw.h, g.out_pre16 = lw.z, g.ldo = DFF;
     if ((rc = launch_wgmma_gemm<128, 128, PRO_H16, EPI_H16_GELU, FMT_BF16>(c, g, 2))) return rc;
     // 5. y = LN2(x1 + h W2^T + b2), keep t2
     memset(&g, 0, sizeof(g));
-    g.M_cap = n, g.A = lw + w.h, g.lda = DFF, g.W = L->lin2_w_f16, g.bias = L->lin2_b, g.res = reinterpret_cast<float*>(lw + w.x1), g.gamma = L->norm2_w;
-    g.beta = L->norm2_b, g.eps = L->norm_eps, g.out_f32 = y, g.out_pre = reinterpret_cast<float*>(lw + w.t2);
+    g.M_cap = n, g.A = lw.h, g.lda = DFF, g.W = L->lin2_w_f16, g.bias = L->lin2_b, g.res = lw.x1, g.gamma = L->norm2_w;
+    g.beta = L->norm2_b, g.eps = L->norm_eps, g.out_f32 = y, g.out_pre = lw.t2;
     if ((rc = launch_wgmma_gemm<256, 128, PRO_H16, EPI_RES_LN, FMT_BF16>(c, g, 1))) return rc;
     xin = y;
   }
@@ -804,54 +813,49 @@ extern "C" int sstb200_sra_stack_backward(sstb200_ctx* c, const sstb200_sra_laye
   for (int l = 0; l < num_layers; l++) CHECK_ARG(c, !layers[l].tau || grads[l].tau);   // cosine layers need their d tau accumulator
   if (n == 0) return SSTB_OK;
   const sstb200_sra_plan plans[2] = {*plan_shift0, *plan_shift1};
-  const TrainWs w = train_ws(n, num_layers);
-  uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
-  uint8_t* tmp = base;   // shared temporaries live after the per-layer blocks (offsets already include them)
-  float* dt = reinterpret_cast<float*>(tmp + w.dt);
-  __nv_bfloat16* dtb = reinterpret_cast<__nv_bfloat16*>(tmp + w.dtb);
-  __nv_bfloat16* dzb = reinterpret_cast<__nv_bfloat16*>(tmp + w.dzb);
-  __nv_bfloat16* dattb = reinterpret_cast<__nv_bfloat16*>(tmp + w.dattb);
-  __nv_bfloat16* dqkv = reinterpret_cast<__nv_bfloat16*>(tmp + w.dqkv);
-  float* dx1 = reinterpret_cast<float*>(tmp + w.dx1);
-  float* dxbuf[2] = {reinterpret_cast<float*>(tmp + w.dxa), reinterpret_cast<float*>(tmp + w.dxb)};
+  const TrainWs w = train_ws(workspace, n, num_layers);
+  float* dt = w.dt;
+  __nv_bfloat16 *dtb = w.dtb, *dzb = w.dzb, *dattb = w.dattb, *dqkv = w.dqkv;
+  float* dx1 = w.dx1;
+  float* dxbuf[2] = {w.dxa, w.dxb};
   const float* dcur = dy;
   for (int l = num_layers - 1; l >= 0; l--) {
     const sstb200_sra_layer* L = &layers[l];
     const sstb200_sra_plan* P = &plans[l & 1];
     const sstb200_sra_layer_wt* T = &wt[l];
     const sstb200_sra_layer_grads* G = &grads[l];
-    uint8_t* lw = base + w.layer_bytes * (size_t)l;
-    const float* xin = l == 0 ? x : reinterpret_cast<const float*>(base + w.layer_bytes * (size_t)(l - 1) + w.y);
+    const TrainLayerWs& lw = w.layer[l];
+    const float* xin = l == 0 ? x : w.layer[l - 1].y;
     float* dxo = l == 0 ? dx : dxbuf[l & 1];
     GemmArgs g;
     int rc;
     // LN2': dt2 (fp32 + bf16), d gamma2, d beta2, d b2
-    if ((rc = launch_ln_bwd(c, dcur, reinterpret_cast<const float*>(lw + w.t2), L->norm2_w, L->norm_eps, n, dt, dtb, G->norm2_w, G->norm2_b,
+    if ((rc = launch_ln_bwd(c, dcur, lw.t2, L->norm2_w, L->norm_eps, n, dt, dtb, G->norm2_w, G->norm2_b,
                             G->lin2_b)))
       return rc;
     // dW2 += dt2^T h
-    if ((rc = launch_dw(c, dtb, DM, DM, reinterpret_cast<const __nv_bfloat16*>(lw + w.h), nullptr, DFF, DFF, nullptr, G->lin2_w, n))) return rc;
+    if ((rc = launch_dw(c, dtb, DM, DM, lw.h, nullptr, DFF, DFF, nullptr, G->lin2_w, n))) return rc;
     // dz = (dt2 W2) * gelu'(z)
     memset(&g, 0, sizeof(g));
-    g.M_cap = n, g.A = dtb, g.lda = DM, g.W = T->lin2_wt, g.out_h16 = dzb, g.aux16 = lw + w.z, g.ldo = DFF;
+    g.M_cap = n, g.A = dtb, g.lda = DM, g.W = T->lin2_wt, g.out_h16 = dzb, g.aux16 = lw.z, g.ldo = DFF;
     if ((rc = launch_wgmma_gemm<128, 128, PRO_H16, EPI_GELUGRAD, FMT_BF16>(c, g, 2))) return rc;
     // dW1 += dz^T x1, d b1 += colsum(dz)
-    if ((rc = launch_dw(c, dzb, DFF, DFF, reinterpret_cast<const __nv_bfloat16*>(lw + w.x1b), nullptr, DM, DM, nullptr, G->lin1_w, n, G->lin1_b))) return rc;
+    if ((rc = launch_dw(c, dzb, DFF, DFF, lw.x1b, nullptr, DM, DM, nullptr, G->lin1_w, n, G->lin1_b))) return rc;
     // dx1 = dt2 + dz W1
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = dzb, g.lda = DFF, g.W = T->lin1_wt, g.res = dt, g.out_f32 = dx1;
     if ((rc = launch_wgmma_gemm<256, 128, PRO_H16, EPI_ADD_F32, FMT_BF16>(c, g, 1))) return rc;
     // LN1': dt1, d gamma1, d beta1, d bo
-    if ((rc = launch_ln_bwd(c, dx1, reinterpret_cast<const float*>(lw + w.t1), L->norm1_w, L->norm_eps, n, dt, dtb, G->norm1_w, G->norm1_b,
+    if ((rc = launch_ln_bwd(c, dx1, lw.t1, L->norm1_w, L->norm_eps, n, dt, dtb, G->norm1_w, G->norm1_b,
                             G->out_proj_b)))
       return rc;
     // dWo += dt1^T att ;  datt = dt1 Wo
-    if ((rc = launch_dw(c, dtb, DM, DM, reinterpret_cast<const __nv_bfloat16*>(lw + w.att), nullptr, DM, DM, nullptr, G->out_proj_w, n))) return rc;
+    if ((rc = launch_dw(c, dtb, DM, DM, lw.att, nullptr, DM, DM, nullptr, G->out_proj_w, n))) return rc;
     memset(&g, 0, sizeof(g));
     g.M_cap = n, g.A = dtb, g.lda = DM, g.W = T->out_proj_wt, g.bias = nullptr, g.out_h16 = dattb, g.ldo = DM;
     if ((rc = launch_wgmma_gemm<128, 128, PRO_H16, EPI_H16, FMT_BF16>(c, g, 1))) return rc;
     // attention'
-    if ((rc = launch_attn_bwd(c, reinterpret_cast<const __half*>(lw + w.qkv), reinterpret_cast<const __nv_bfloat16*>(lw + w.att), dattb, P, L, G->tau,
+    if ((rc = launch_attn_bwd(c, lw.qkv, lw.att, dattb, P, L, G->tau,
                               dqkv)))
       return rc;
     // dWq|k += [dq|dk]^T (x + pos) ;  dWv += dv^T x ;  d bqkv += colsum(dqkv)

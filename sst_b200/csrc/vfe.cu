@@ -709,19 +709,27 @@ __global__ void __launch_bounds__(256) vfe_decorate_wide_kernel(VfeDev v, const 
   }
 }
 
+struct VfeWideWs {
+  float *X, *Y0, *T1, *V0, *G;
+  long long* row64;
+};
+static void vfe_wide_carve(Carve& cv, VfeWideWs& w, int P, int D0, int C0, int C1) {
+  const int Cmax = C0 > C1 ? C0 : C1;
+  w.X = cv.take<float>((size_t)P * D0);
+  w.Y0 = cv.take<float>((size_t)P * C0);
+  w.T1 = C1 ? cv.take<float>((size_t)P * Cmax) : nullptr;
+  w.V0 = C1 ? cv.take<float>((size_t)P * C0) : nullptr;
+  w.G = C1 ? cv.take<float>((size_t)P * C1) : nullptr;
+  w.row64 = cv.take<long long>(P);
+}
+
 template <typename TC, typename TM>
 static int vfe_wide_path(sstb200_ctx* c, const sstb200_vfe_cfg* cfg, const VfeDev& v, const float* pts, const TC* coors, const TM* map,
-                         const Csr& r, int P, const int32_t* num_dev, float* vmean, float* out_feats) {
+                         const Csr& r, const VfeWideWs& w, int P, const int32_t* num_dev, float* vmean, float* out_feats) {
   cudaStream_t st = c->stream;
   const int D0 = v.D0, C0 = v.C0, C1 = v.C1;
-  const int Cmax = C0 > C1 ? C0 : C1;
-  float* X = arena_alloc<float>(c, (size_t)P * D0);
-  float* Y0 = arena_alloc<float>(c, (size_t)P * C0);
-  float* T1 = C1 ? arena_alloc<float>(c, (size_t)P * Cmax) : nullptr;
-  float* V0 = C1 ? arena_alloc<float>(c, (size_t)P * C0) : nullptr;
-  float* G = C1 ? arena_alloc<float>(c, (size_t)P * C1) : nullptr;
-  long long* row64 = arena_alloc<long long>(c, (size_t)P);
-  if (!X || !Y0 || !row64 || (C1 && (!T1 || !V0 || !G))) return sstb_fail(c, SSTB_ERR_WORKSPACE, "vfe (wide): arena");
+  float *X = w.X, *Y0 = w.Y0, *T1 = w.T1, *V0 = w.V0, *G = w.G;
+  long long* row64 = w.row64;
   const int mode = v.mode_max ? SSTB200_REDUCE_MAX : SSTB200_REDUCE_MEAN;
   launch_pdl(vfe_mean_kernel, dim3(c->num_sms * 8), dim3(256), (size_t)0, st, pts, v.F, (const uint32_t*)r.offsets, (const int32_t*)r.order, num_dev,
              vmean);
@@ -772,20 +780,25 @@ static int vfe_forward_impl(sstb200_ctx* c, const sstb200_vfe_cfg* cfg, const fl
   long long T = (long long)cells_pad * B;
   if (T > ((long long)1 << 34)) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "voxel grid too large for bitmap rank (%lld cells)", T);
   arena_reset(c);
-  int rc = arena_reserve(c, key_index_bytes(P, T) + csr_bytes(P, P) + al256((size_t)P * 4) * 3 + al256((size_t)P * 3 * 4) +
-                                al256((size_t)P * C0 * 4) + al256((size_t)P * C0 * 2 + 128) + al256((size_t)(C0 + C1) * 8) + al256((size_t)B * 4) + 8192 +
-                                (wide ? al256((size_t)P * D0 * 4) + 4 * al256((size_t)P * (C0 > C1 ? C0 : C1) * 4) + al256((size_t)P * 8) : 0));
-  if (rc) return rc;
   KeyIndex k;
-  rc = key_index_alloc(c, k, P, T);
+  int32_t *count, *map32 = nullptr;
+  float *vmean, *vf0, *fold;
+  __nv_bfloat16* y0buf;
+  Csr r;
+  VfeWideWs ww{};
+  int rc = arena_carve(c, [&](Carve& cv) {
+    key_index_carve(cv, k, P, T);
+    count = cv.take<int32_t>((size_t)P + 2 + B);  // [P + 2] voxel point counts | [B] per-sample "has invalid" flags
+    if (!inverse) map32 = cv.take<int32_t>(P);
+    vmean = cv.take<float>((size_t)P * 3);
+    vf0 = cv.take<float>((size_t)P * C0);
+    fold = cv.take<float>(2 * (size_t)(C0 + C1) + 8);
+    y0buf = cv.take<__nv_bfloat16>((size_t)P * C0 + 64);  // layer-0 point features (bf16, CSR order) for the tensor-core layer 1
+    csr_carve(cv, r, P, P);
+    if (wide) vfe_wide_carve(cv, ww, P, D0, C0, C1);
+  });
   if (rc) return rc;
-  int32_t* count = arena_alloc<int32_t>(c, (size_t)P + 2 + B);  // [P + 2] voxel point counts | [B] per-sample "has invalid" flags
-  int32_t* map32 = inverse ? nullptr : arena_alloc<int32_t>(c, P);
-  float* vmean = arena_alloc<float>(c, (size_t)P * 3);
-  float* vf0 = arena_alloc<float>(c, (size_t)P * C0);
-  float* fold = arena_alloc<float>(c, 2 * (size_t)(C0 + C1) + 8);
-  __nv_bfloat16* y0buf = arena_alloc<__nv_bfloat16>(c, (size_t)P * C0 + 64);  // layer-0 point features (bf16, CSR order) for the tensor-core layer 1
-  if (!count || !vmean || !vf0 || !fold || !y0buf) return sstb_fail(c, SSTB_ERR_WORKSPACE, "vfe: arena");
+  if ((rc = key_index_zero(c, k))) return rc;
   CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)P + 2 + B) * 4, c->stream));
   int32_t* sample_invalid = count + P + 2;
   int nb = (P + 255) / 256;
@@ -803,7 +816,6 @@ static int vfe_forward_impl(sstb200_ctx* c, const sstb200_vfe_cfg* cfg, const fl
   if (eg > c->num_sms * 32) eg = c->num_sms * 32;
   launch_pdl(vfe_emit_kernel<TC>, dim3(eg), dim3(64), (size_t)(0), c->stream, k.bitmap, k.word_prefix, k.nwords, cells_pad, Y, X, q, out_coors, k.total, num_dev);
   CUDA_TRY(c, cudaEventRecord(c->ev_coords, c->stream));   // voxel_coors / num_dev are final from here on (sstb200_branch_fork)
-  Csr r;
   if (inverse) {
     launch_pdl(vfe_map_kernel<TC>, dim3(nb), dim3(256), (size_t)(0), c->stream, k.keys, P, k.bitmap, k.word_prefix, cells_pad, q, inverse, count);
     rc = csr_build<TC>(c, r, inverse, P, count, P, num_dev);
@@ -836,8 +848,8 @@ static int vfe_forward_impl(sstb200_ctx* c, const sstb200_vfe_cfg* cfg, const fl
   v.s1 = fold + 2 * C0;
   v.t1 = fold + 2 * C0 + C1;
   if (wide) {
-    rc = inverse ? vfe_wide_path<TC, TC>(c, cfg, v, pts, coors, (const TC*)inverse, r, P, num_dev, vmean, out_feats)
-                 : vfe_wide_path<TC, int32_t>(c, cfg, v, pts, coors, (const int32_t*)map32, r, P, num_dev, vmean, out_feats);
+    rc = inverse ? vfe_wide_path<TC, TC>(c, cfg, v, pts, coors, (const TC*)inverse, r, ww, P, num_dev, vmean, out_feats)
+                 : vfe_wide_path<TC, int32_t>(c, cfg, v, pts, coors, (const int32_t*)map32, r, ww, P, num_dev, vmean, out_feats);
     if (rc) return rc;
     if (num_host) return read_back_i32(c, num_dev, num_host);
     return SSTB_OK;

@@ -156,11 +156,14 @@ extern "C" int sstb200_dynamic_point_to_voxel_forward(sstb200_ctx* c, const floa
   int rc = make_extents(c, e, 3, lo, hi, &T);
   if (rc) return rc;
   arena_reset(c);
-  rc = arena_reserve(c, key_index_bytes(P, T) + csr_bytes(P, P) + 4096);
-  if (rc) return rc;
   KeyIndex k;
-  rc = key_index_alloc(c, k, P, T);
+  Csr r;
+  rc = arena_carve(c, [&](Carve& cv) {
+    key_index_carve(cv, k, P, T);
+    csr_carve(cv, r, P, P);
+  });
   if (rc) return rc;
+  if ((rc = key_index_zero(c, k))) return rc;
   CUDA_TRY(c, cudaMemsetAsync(reduce_count, 0, (size_t)P * 4, c->stream));
   int nb = (P + 255) / 256;
   launch_mark_rows<int32_t>(c, coors, P, e, true, k, nullptr);
@@ -168,7 +171,6 @@ extern "C" int sstb200_dynamic_point_to_voxel_forward(sstb200_ctx* c, const floa
   launch_emit_rows<int32_t>(c, k, e, 1, out_coors, num_dev);
   launch_pdl(map_count_kernel<int32_t>, dim3(nb), dim3(256), (size_t)(0), c->stream, k.keys, P, k.bitmap, k.word_prefix, 1, k.flags, coors_map, reduce_count, nullptr);
   LAUNCH_CHECK(c);
-  Csr r;
   rc = csr_build<int32_t>(c, r, coors_map, P, reduce_count, P, num_dev);
   if (rc) return rc;
   launch_segment_reduce(c, feats, C, r.offsets, r.order, P, num_dev, reduce_type,
@@ -250,9 +252,9 @@ extern "C" int sstb200_dynamic_point_to_voxel_backward(sstb200_ctx* c, float* gr
                                                    reduce_type == SSTB200_REDUCE_MEAN);
   } else {
     arena_reset(c);
-    int rc = arena_reserve(c, (size_t)M * C * 4 + 1024);
+    int32_t* from;
+    int rc = arena_carve(c, [&](Carve& cv) { from = cv.take<int32_t>((size_t)M * C); });
     if (rc) return rc;
-    int32_t* from = arena_alloc<int32_t>(c, (size_t)M * C);
     size_t m = (size_t)M * C;
     unsigned mb = (unsigned)((m + 255) / 256);
     launch_pdl(fill_i32_kernel, dim3(mb), dim3(256), (size_t)(0), c->stream, from, m, P);
@@ -282,11 +284,10 @@ extern "C" int sstb200_unique_rows_i64(sstb200_ctx* c, const int64_t* coors, int
   int rc = make_extents(c, e, ndim, (const long long*)lo, (const long long*)hi, &T);
   if (rc) return rc;
   arena_reset(c);
-  rc = arena_reserve(c, key_index_bytes(P, T) + 4096);
-  if (rc) return rc;
   KeyIndex k;
-  rc = key_index_alloc(c, k, P, T);
+  rc = arena_carve(c, [&](Carve& cv) { key_index_carve(cv, k, P, T); });
   if (rc) return rc;
+  if ((rc = key_index_zero(c, k))) return rc;
   if (counts) CUDA_TRY(c, cudaMemsetAsync(counts, 0, (size_t)P * 4, c->stream));
   int nb = (P + 255) / 256;
   launch_mark_rows<long long>(c, (const long long*)coors, P, e, false, k, nullptr);
@@ -308,12 +309,15 @@ extern "C" int sstb200_segment_reduce(sstb200_ctx* c, const float* src, const in
   if (nseg == 0) return SSTB_OK;
   CHECK_ARG(c, out && (P == 0 || (src && index)));
   arena_reset(c);
-  int rc = arena_reserve(c, csr_bytes(P, nseg) + al256((size_t)nseg * 4 + 8) + 4096);
+  int32_t* count;
+  Csr r;
+  int rc = arena_carve(c, [&](Carve& cv) {
+    count = cv.take<int32_t>((size_t)nseg + 2);
+    csr_carve(cv, r, P, nseg);
+  });
   if (rc) return rc;
-  int32_t* count = arena_alloc<int32_t>(c, (size_t)nseg + 2);
   CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)nseg + 2) * 4, c->stream));
   if (P > 0) launch_pdl(count_index_kernel, dim3((P + 255) / 256), dim3(256), (size_t)(0), c->stream, (const long long*)index, P, nseg, count, count + nseg + 1);
-  Csr r;
   rc = csr_build<long long>(c, r, (const long long*)index, P, count, nseg, nullptr);
   if (rc) return rc;
   launch_segment_reduce(c, src, C, r.offsets, r.order, nseg, nullptr, reduce_type, 0.f, out, (long long*)argmax, P);
@@ -334,21 +338,23 @@ extern "C" int sstb200_ingroup_indices(sstb200_ctx* c, const int64_t* group, int
   int rc = make_extents(c, e, 1, &lo, &hi, &T);
   if (rc) return rc;
   arena_reset(c);
-  rc = arena_reserve(c, key_index_bytes(N, T) + csr_bytes(N, N) + al256((size_t)N * 4) * 2 + 4096);
-  if (rc) return rc;
   KeyIndex k;
-  rc = key_index_alloc(c, k, N, T);
+  int32_t *cid, *count;
+  Csr r;
+  rc = arena_carve(c, [&](Carve& cv) {
+    key_index_carve(cv, k, N, T);
+    cid = cv.take<int32_t>(N);
+    count = cv.take<int32_t>((size_t)N + 2);
+    csr_carve(cv, r, N, N);
+  });
   if (rc) return rc;
-  int32_t* cid = arena_alloc<int32_t>(c, N);
-  int32_t* count = arena_alloc<int32_t>(c, (size_t)N + 2);
+  if ((rc = key_index_zero(c, k))) return rc;
   const int32_t* ng = (const int32_t*)k.total;  // #distinct groups, written by the bitmap scan
   CUDA_TRY(c, cudaMemsetAsync(count, 0, ((size_t)N + 2) * 4, c->stream));
   int nb = (N + 255) / 256;
   launch_mark_rows<long long>(c, (const long long*)group, N, e, false, k, nullptr);
   key_index_scan(c, k);
   launch_pdl(map_count_kernel<int32_t>, dim3(nb), dim3(256), (size_t)(0), c->stream, k.keys, N, k.bitmap, k.word_prefix, 0, k.flags, cid, count, nullptr);
-  Csr r;
-  r.offsets = nullptr;
   rc = csr_build<int32_t>(c, r, cid, N, count, N, ng);
   if (rc) return rc;
   launch_pdl(stable_rank_kernel, dim3(c->num_sms * 4), dim3(256), (size_t)(0), c->stream, r.offsets, r.order, ng, nullptr, (long long*)out, nullptr, nullptr);

@@ -255,13 +255,17 @@ static int window_plan_impl(sstb200_ctx* c, const TC* coors, int n, const int32_
   if (T > ((long long)1 << 34)) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "window slot space too large");
   arena_reset(c);
   size_t nwcap = (size_t)n;  // #windows <= #tokens
-  int rc = arena_reserve(c, key_index_bytes(n, T) + csr_bytes(n, nwcap) + al256((nwcap + 2) * 4) + 4096);
-  if (rc) return rc;
   KeyIndex k;
-  rc = key_index_alloc(c, k, n, T);
+  int32_t* count;
+  Csr r;
+  r.offsets = (uint32_t*)o->win_offsets;  // int32 [n+1] caller buffer (only R+1 entries are meaningful): the scan writes it in place
+  int rc = arena_carve(c, [&](Carve& cv) {
+    key_index_carve(cv, k, n, T);
+    count = cv.take<int32_t>(nwcap + 2);
+    csr_carve(cv, r, n, nwcap);
+  });
   if (rc) return rc;
-  int32_t* count = arena_alloc<int32_t>(c, nwcap + 2);
-  if (!count) return sstb_fail(c, SSTB_ERR_WORKSPACE, "window plan: arena");
+  if ((rc = key_index_zero(c, k))) return rc;
   CUDA_TRY(c, cudaMemsetAsync(count, 0, (nwcap + 2) * 4, c->stream));
   int nb = (n + 255) / 256;
   if (k.nwords <= 12 * 1024) {  // <= 48 KB: block-private bitmap
@@ -276,8 +280,6 @@ static int window_plan_impl(sstb200_ctx* c, const TC* coors, int n, const int32_
   key_index_scan(c, k);
   launch_pdl(map_count_kernel<int32_t>, dim3(nb), dim3(256), (size_t)(0), c->stream, k.keys, n, k.bitmap, k.word_prefix, 0, k.flags, o->tok_win, count, n_dev);
   const int32_t* nwin = (const int32_t*)k.total;  // #distinct windows, written by the bitmap scan
-  Csr r;
-  r.offsets = (uint32_t*)o->win_offsets;  // int32 [n+1] caller buffer (only R+1 entries are meaningful): the scan writes it in place
   rc = csr_build<int32_t>(c, r, o->tok_win, n, count, nwcap, nwin, n_dev);
   if (rc) return rc;
   // the reference-layout outputs (drop level, flat2win index, per-level window rank) are only produced on request; the
