@@ -754,6 +754,81 @@ int sstb200_anchor_reg_dir_loss_backward(sstb200_ctx* ctx, const float* bbox_pre
                                          float loss_weight_dir, const float* grad_losses, float* grad_bbox_pred,
                                          float* grad_dir_cls_preds);
 
+/* ---- VoteSegHead training (mmdet3d/models/decode_heads/segmentation_head.py), fp32, stream-ordered, no sync.
+ *
+ * sstb200_voteseg_targets: get_targets (lines 212-283, centroid_offset and extra_width unset) for the whole batch in one launch.
+ *   points [N, >= 3] fp32 with row stride point_stride (floats), the samples concatenated: sample b owns rows
+ *   [point_offsets[b], point_offsets[b + 1]).  gt_boxes [G, 7] bottom-centre LiDAR boxes and gt_labels int64 [G], sample b owning rows
+ *   [gt_offsets[b], gt_offsets[b + 1]).  Both offset arrays are host arrays of batch + 1 entries.
+ *   A point takes the label of the lowest-index box of its own sample that contains it, boxes with a negative label skipped (the
+ *   reference's valid_gt_mask filter, line 229, then points_in_boxes_gpu's first hit).  The in-box test is sstb200_points_in_boxes'
+ *   (box3d.cuh), so it is bit-identical to the reference kernel.  Its vote target is encode_vote_targets(gravity_center - point) with the
+ *   reference's fp32 expressions: centre z = z + h * 0.5, the subtraction, then sign(d) * sqrt(|d|) with an IEEE square root; the
+ *   results are bit-exact.  A point in no box (so every point of a sample with no valid GT, lines 231-234) gets bg_label (num_classes:
+ *   the background column of a sigmoid head, the last of the num_classes + 1 logits of a softmax head), vote target 0 and mask 0.
+ *   Outputs labels int64 [N], vote_targets f32 [N, 3] and vote_mask uint8 [N] (0 / 1), every entry written.  GTs are staged in shared
+ *   memory 256 at a time and a point stops at its first hit.  No temporaries.
+ *   Errors: a NULL pointer, batch < 1, stride < 3, offsets that do not start at 0 or decrease (SSTB_ERR_ARG); more than 256 samples or
+ *   more than 4096 GTs in one sample (SSTB_ERR_UNSUPPORTED).
+ *
+ * sstb200_voteseg_loss_forward: `losses` (lines 107-173) in one read of every point's row.  seg_logits [N, C] (row stride logit_stride)
+ *   and vote_preds [N, 3 C] (row stride vote_stride, class-major: class c owns channels 3 c .. 3 c + 2) are read in place; labels int64
+ *   [N], vote_targets f32 [N, 3] contiguous, vote_mask uint8 [N].  Every logit is first multiplied by cfg->logit_scale (line 116).
+ *   - use_softmax 0: mmdet 2.14 FocalLoss(use_sigmoid=True, gamma, alpha) against one-hot(label) without the background column
+ *     (label C), reduction 'mean' without avg_factor: losses[0] = loss_weight * sum / (N C).  The log-sigmoid is the stable softplus form
+ *     of py_sigmoid_focal_loss, exact for logits of any size; mmcv's CUDA kernel instead clamps log(max(1 - p, FLT_MIN)) and so saturates
+ *     near 87 for logits beyond about +-17.  gamma must be >= 1.
+ *   - use_softmax 1: mmseg CrossEntropyLoss(use_sigmoid=False, class_weight): losses[0] = loss_weight * sum w[y] (logsumexp(x) - x[y]) / N,
+ *     divided by N and not by the sum of the weights (F.cross_entropy(reduction='none') then weight_reduce_loss, mmseg 0.14.1 to 1.0,
+ *     avg_non_ignore False).  class_weight: host [C], NULL for ones.  Labels come from get_targets and are never 255 or -100, so
+ *     ignore_index plays no part.
+ *   - vote loss: mmdet 2.14 L1Loss over the valid points (mask 1): losses[1] = loss_weight_vote * sum |vote_preds[i, 3 y + k] -
+ *     vote_targets[i, k]| / (3 n_valid), n_valid counted and divided on the device and written to *num_valid (int64).  Only the three
+ *     channels of a valid point's own class are read.  With no valid point losses[1] = vote_preds.sum() * 0 as in the reference (line
+ *     142): 0, or NaN when any vote prediction is not finite (an fp32 overflow of the sum of finite predictions is not reproduced).  A
+ *     third launch reads the device n_valid and scans the whole vote tensor for that only when n_valid is 0.
+ *   - training-log counts (lines 146-171), int64 [2 E + 1]: tp[e] (E entries), real[e], then num_fg.  Group g predicts a point when
+ *     its score exceeds group_thresh[g] (compared in fp32); the score is the sum over the classes in group_masks[g] (bit c = class c) of
+ *     sigmoid(x) (use_softmax 0) or of the softmax probabilities (use_softmax 1).  tp[e] counts the points of class entry_class[e]
+ *     that group entry_group[e] predicts, real[e] the points of class entry_class[e], num_fg the sum over groups of the points each
+ *     predicts.  The recall quotients are left to the caller.  The reference's host asserts (lines 124-127, 134-135) are not made.
+ *   - NaN: a NaN logit makes losses[0] NaN, and a NaN vote prediction that is read makes losses[1] NaN.  A label outside [0, C] (sigmoid)
+ *     or [0, C) (softmax), or a valid point whose label is not below C, makes the loss NaN instead of reading out of bounds.
+ *   Block partials (double sums, integer counts) summed in a fixed order: deterministic.  Three launches, partials from the context arena.
+ * sstb200_voteseg_loss_backward: grad_losses (d / d losses[0], d / d losses[1], device) -> grad_logits [N, C] and grad_vote_preds
+ *   [N, 3 C], both contiguous and fully written.  Each point writes only its own row, with no atomics: two calls are bit-identical.
+ *   d logit = logit_scale * loss_weight / (N C) (sigmoid) or loss_weight w[y] / N (softmax) times the element's derivative, recomputed
+ *   from the logits.  A NaN logit makes its own gradient NaN (its whole row in softmax mode) and no other.  The vote gradient is
+ *   loss_weight_vote * sign(pred - target) / (3 n_valid) on the three channels of a valid point's own class, sign(0) = sign(NaN) = 0 as
+ *   torch.abs' gradient, and 0 everywhere else; with no valid point it is all zeros.  One launch.
+ *   Errors (both): a NULL pointer, N < 1, C < 1, a row stride below the row, a group or entry out of range (SSTB_ERR_ARG); more than 64
+ *   classes, 64 groups or 64 entries, a focal gamma below 1 (SSTB_ERR_UNSUPPORTED). */
+typedef struct {
+  int32_t num_classes;           /* C: logit columns (num_classes + 1 for a softmax head) */
+  int32_t use_softmax;           /* 0: sigmoid focal loss, 1: softmax cross-entropy */
+  float gamma, alpha;            /* focal loss */
+  float logit_scale;
+  float loss_weight;             /* loss_decode */
+  float loss_weight_vote;        /* loss_vote */
+  const float* class_weight;     /* host [C] or NULL (softmax) */
+  int32_t num_groups;            /* G <= 64 */
+  const uint64_t* group_masks;   /* host [G] */
+  const float* group_thresh;     /* host [G] */
+  int32_t num_entries;           /* E <= 64 */
+  const int32_t* entry_group;    /* host [E] */
+  const int32_t* entry_class;    /* host [E] */
+} sstb200_voteseg_cfg;
+int sstb200_voteseg_targets(sstb200_ctx* ctx, const float* points, int64_t point_stride, const int32_t* point_offsets,
+                            const float* gt_boxes, const int64_t* gt_labels, const int32_t* gt_offsets, int batch, int bg_label,
+                            int64_t* labels, float* vote_targets, uint8_t* vote_mask);
+int sstb200_voteseg_loss_forward(sstb200_ctx* ctx, const sstb200_voteseg_cfg* cfg, const float* seg_logits, int64_t logit_stride,
+                                 const float* vote_preds, int64_t vote_stride, int64_t num_points, const int64_t* labels,
+                                 const float* vote_targets, const uint8_t* vote_mask, float* losses, int64_t* num_valid, int64_t* counts);
+int sstb200_voteseg_loss_backward(sstb200_ctx* ctx, const sstb200_voteseg_cfg* cfg, const float* seg_logits, int64_t logit_stride,
+                                  const float* vote_preds, int64_t vote_stride, int64_t num_points, const int64_t* labels,
+                                  const float* vote_targets, const uint8_t* vote_mask, const int64_t* num_valid, const float* grad_losses,
+                                  float* grad_logits, float* grad_vote_preds);
+
 #ifdef __cplusplus
 }
 #endif

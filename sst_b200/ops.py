@@ -19,6 +19,7 @@ and error behaviour; no CPU path - CPU tensors raise.
                                       mmcv.ops.deform_conv (1.3.8-1.4.0)    (CenterHead's DCN)
     anchor3d_targets, anchor_focal_loss, anchor_reg_dir_loss
                                       models/dense_heads/anchor3d_head.py, train_mixins.py (Anchor3DHead training)
+    voteseg_targets, voteseg_loss     models/decode_heads/segmentation_head.py:107-283 (VoteSegHead training)
 """
 import ctypes as C
 import math
@@ -1405,3 +1406,200 @@ def anchor_reg_dir_loss(bbox_pred, dir_cls_preds, labels, bbox_targets, bbox_wei
     """(loss_bbox, loss_dir), fp32 device scalars, of AnchorRegDirLossFunction"""
     return AnchorRegDirLossFunction.apply(bbox_pred, dir_cls_preds, labels, bbox_targets, bbox_weights, dir_targets, dir_weights,
                                           num_total_pos, num_classes, code_weight, loss_weight_bbox, loss_weight_dir)
+
+
+# ----------------------------------------------------------------------------------------------
+# VoteSegHead training (mmdet3d/models/decode_heads/segmentation_head.py:107-283)
+# ----------------------------------------------------------------------------------------------
+class _VoteSegCfg(C.Structure):
+    _fields_ = [("num_classes", C.c_int32), ("use_softmax", C.c_int32), ("gamma", C.c_float), ("alpha", C.c_float),
+                ("logit_scale", C.c_float), ("loss_weight", C.c_float), ("loss_weight_vote", C.c_float), ("class_weight", L.P_f32),
+                ("num_groups", C.c_int32), ("group_masks", C.POINTER(C.c_uint64)), ("group_thresh", L.P_f32),
+                ("num_entries", C.c_int32), ("entry_group", L.P_i32), ("entry_class", L.P_i32)]
+
+
+_VS_ARGS = [L.vp, C.POINTER(_VoteSegCfg), L.vp, C.c_int64, L.vp, C.c_int64, C.c_int64, L.vp, L.vp, L.vp]
+L.SIGNATURES["sstb200_voteseg_targets"] = (C.c_int, [L.vp, L.vp, C.c_int64, L.P_i32, L.vp, L.vp, L.P_i32, C.c_int, C.c_int, L.vp, L.vp,
+                                                     L.vp])
+L.SIGNATURES["sstb200_voteseg_loss_forward"] = (C.c_int, _VS_ARGS + [L.vp, L.vp, L.vp])
+L.SIGNATURES["sstb200_voteseg_loss_backward"] = (C.c_int, _VS_ARGS + [L.vp, L.vp, L.vp, L.vp])
+
+
+def _offsets(sizes):
+    out = [0]
+    for n in sizes:
+        out.append(out[-1] + int(n))
+    return out
+
+
+def voteseg_targets(points_list_or_cat, offsets, gt_boxes, gt_labels, num_classes):
+    """VoteSegHead.get_targets for the whole batch in one launch.  points_list_or_cat: a list of [n_b, >= 3] fp32 CUDA tensors (offsets
+    None), or their concatenation [N, >= 3] with offsets = the B + 1 host sample offsets (ints or a CPU tensor; read in place, any row
+    stride).  gt_boxes: a list over samples of [G_b, >= 7] bottom-centre boxes (tensors or objects with `.tensor`, columns 0-6 used),
+    gt_labels: a list of int64 [G_b] (a negative label marks an invalid box).  num_classes: the head's class count, the background label.
+    Returns (labels int64 [N], vote_targets f32 [N, 3], vote_mask bool [N]), the reference's tensors bit for bit.  No host sync."""
+    if isinstance(points_list_or_cat, (list, tuple)):
+        if offsets is not None:
+            raise L.SSTB200Error("voteseg_targets: offsets are given by the list of points; pass None")
+        pts_list = [_fp32_cuda("points", p, 2) for p in points_list_or_cat]
+        offs = _offsets([p.shape[0] for p in pts_list])
+        pts = torch.cat(pts_list) if len(pts_list) > 1 else pts_list[0]
+    else:
+        pts = points_list_or_cat
+        if not isinstance(pts, torch.Tensor) or not pts.is_cuda or pts.dtype != torch.float32 or pts.dim() != 2:
+            raise L.SSTB200Error("voteseg_targets: points must be a float32 [N, >= 3] CUDA tensor or a list of them")
+        if isinstance(offsets, torch.Tensor):
+            if offsets.is_cuda:
+                raise L.SSTB200Error("voteseg_targets: offsets must be host values (reading device offsets would synchronise)")
+            offsets = offsets.tolist()
+        offs = [int(v) for v in offsets]
+    if pts.shape[1] < 3 or pts.stride(1) != 1:
+        if pts.shape[1] < 3:
+            raise L.SSTB200Error(f"voteseg_targets: points need at least 3 columns, got {tuple(pts.shape)}")
+        pts = pts.contiguous()
+    B = len(offs) - 1
+    if B < 1 or offs[0] != 0 or offs[-1] != pts.shape[0] or any(b < a for a, b in zip(offs, offs[1:])):
+        raise L.SSTB200Error(f"voteseg_targets: offsets {offs} do not partition the {pts.shape[0]} points")
+    if len(gt_boxes) != B or len(gt_labels) != B:
+        raise L.SSTB200Error(f"voteseg_targets: {len(gt_boxes)} box and {len(gt_labels)} label lists for {B} samples")
+    dev = pts.device
+    boxes = [getattr(b, "tensor", b) for b in gt_boxes]
+    for b, lab in zip(boxes, gt_labels):
+        if b.dim() != 2 or b.shape[1] < 7 or lab.shape != (b.shape[0],):
+            raise L.SSTB200Error(f"voteseg_targets: boxes {tuple(b.shape)} and labels {tuple(lab.shape)} do not match")
+    gt = torch.cat([b[:, :7] for b in boxes]).to(dev, torch.float32).contiguous()
+    gl = torch.cat([lab.reshape(-1) for lab in gt_labels]).to(dev, torch.int64).contiguous()
+    N = pts.shape[0]
+    labels = torch.empty((N,), dtype=torch.int64, device=dev)
+    vote_targets = torch.empty((N, 3), dtype=torch.float32, device=dev)
+    vote_mask = torch.empty((N,), dtype=torch.bool, device=dev)
+    c = L.ctx(dev)
+    L.check(c, L.lib().sstb200_voteseg_targets(c, L.ptr(pts) if N else None, pts.stride(0), L.arr(C.c_int32, offs),
+                                               L.ptr(gt) if gt.numel() else None, L.ptr(gl) if gl.numel() else None,
+                                               L.arr(C.c_int32, _offsets([b.shape[0] for b in boxes])), B, int(num_classes),
+                                               L.ptr(labels) if N else None, L.ptr(vote_targets) if N else None,
+                                               L.ptr(vote_mask) if N else None))
+    return labels, vote_targets, vote_mask
+
+
+class VoteSegLossConfig:
+    """The constant part of VoteSegHead.losses: the loss settings and the training-log groups.  num_classes = logit columns C.
+    Sigmoid heads: score_thresh[i] / class_names[i] give recall_<name> of class i.  Softmax heads: group_names (lists of class names) with
+    one score_thresh each give the group scores of gather_group_by_names, recall_<name> of every grouped class and num_fg."""
+
+    def __init__(self, num_classes, use_sigmoid, gamma=2.0, alpha=0.25, class_weight=None, logit_scale=1.0, loss_weight=1.0,
+                 loss_weight_vote=1.0, score_thresh=None, class_names=None, group_names=None):
+        self.num_classes, self.use_sigmoid = int(num_classes), bool(use_sigmoid)
+        groups, entries, names = [], [], []   # (mask, thr); (group, class); recall key per entry
+        if score_thresh is not None:
+            if self.use_sigmoid:
+                for i, thr in enumerate(score_thresh):
+                    groups.append((1 << i, float(thr)))
+                    entries.append((i, i))
+                    names.append(class_names[i])
+            else:
+                for gi, g in enumerate(group_names):
+                    idx = [list(class_names).index(n) for n in g]
+                    mask = 0
+                    for k in idx:
+                        mask |= 1 << k
+                    groups.append((mask, float(score_thresh[gi])))
+                    for n, k in zip(g, idx):
+                        entries.append((gi, k))
+                        names.append(n)
+        self.entry_names, self.log_fg = names, score_thresh is not None and not self.use_sigmoid
+        cw = None if class_weight is None else [float(w) for w in class_weight]
+        if cw is not None and len(cw) != self.num_classes:
+            raise L.SSTB200Error(f"voteseg_loss: {len(cw)} class weights for {self.num_classes} classes")
+        self.gamma, self.alpha, self.class_weight, self.logit_scale = float(gamma), float(alpha), cw, float(logit_scale)
+        self.loss_weight, self.loss_weight_vote, self.groups, self.entries = float(loss_weight), float(loss_weight_vote), groups, entries
+
+    def struct(self):
+        """(sstb200_voteseg_cfg, the host arrays it points to: keep both alive over the call)"""
+        keep = (L.arr(C.c_float, self.class_weight) if self.class_weight else None, L.arr(C.c_uint64, [m for m, _ in self.groups]),
+                L.arr(C.c_float, [t for _, t in self.groups]), L.arr(C.c_int32, [g for g, _ in self.entries]),
+                L.arr(C.c_int32, [k for _, k in self.entries]))
+        s = _VoteSegCfg(self.num_classes, int(not self.use_sigmoid), self.gamma, self.alpha, self.logit_scale, self.loss_weight,
+                        self.loss_weight_vote, keep[0], len(self.groups), keep[1], keep[2], len(self.entries), keep[3], keep[4])
+        return s, keep
+
+    def metrics(self, counts):
+        """{recall_<name>: tp / (real + 1e-5)} and, for softmax heads, num_fg [1], as the reference's fp32 device tensors"""
+        E = len(self.entry_names)
+        out = {}
+        if E == 0 and not self.log_fg:
+            return out
+        cf = counts.float()
+        for e, name in enumerate(self.entry_names):
+            out[f"recall_{name}"] = cf[e] / (cf[E + e] + 1e-5)
+        if self.log_fg:
+            out["num_fg"] = cf[2 * E:2 * E + 1]
+        return out
+
+
+def _row_major(name, t, cols):
+    """t as fp32 [N, cols] rows with unit column stride, read in place when it already is"""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise L.SSTB200Error(f"{name} must be a CUDA tensor (there is no CPU path)")
+    if t.dtype == torch.float16:                       # @force_fp32 casts half predictions
+        t = t.float()
+    if t.dtype != torch.float32 or t.dim() != 2 or t.shape[1] != cols:
+        raise L.SSTB200Error(f"{name} must be float32 [N, {cols}], got {t.dtype} {tuple(t.shape)}")
+    if t.stride(1) != 1 or t.stride(0) < cols:
+        t = t.contiguous()
+    return t
+
+
+class VoteSegLossFunction(Function):
+    """VoteSegHead.losses' two losses and training-log counts in one pass over the point rows (sstb200_voteseg_loss_forward): returns
+    (losses [2] = (loss_sem_seg, loss_vote), counts int64 [2 E + 1], non-differentiable).  seg_logits [N, C] and vote_preds [N, 3 C] are
+    read in place with their row strides; labels / vote_targets / vote_mask come from voteseg_targets.  Saves only the two predictions,
+    the targets and the device n_valid; the backward writes each point's own rows with no atomics (bit-identical from run to run).  No
+    host sync.  A NaN logit makes loss_sem_seg NaN and its own gradient NaN (its row's in softmax mode), not the whole gradient."""
+
+    @staticmethod
+    def forward(ctx, seg_logits, vote_preds, labels, vote_targets, vote_mask, cfg):
+        Cn = cfg.num_classes
+        x, v = _row_major("seg_logits", seg_logits, Cn), _row_major("vote_preds", vote_preds, 3 * Cn)
+        N = x.shape[0]
+        t = _fp32_cuda("vote_targets", vote_targets, 2)
+        if v.shape[0] != N or t.shape != (N, 3) or labels.shape != (N,) or vote_mask.shape != (N,) or N == 0:
+            raise L.SSTB200Error(f"voteseg_loss: logits {tuple(x.shape)}, vote_preds {tuple(v.shape)}, labels {tuple(labels.shape)}, "
+                                 f"vote_targets {tuple(t.shape)} and vote_mask {tuple(vote_mask.shape)} do not fit N > 0 points")
+        if labels.dtype != torch.int64 or not labels.is_cuda or vote_mask.dtype not in (torch.bool, torch.uint8) or not vote_mask.is_cuda:
+            raise L.SSTB200Error("voteseg_loss: labels must be int64 and vote_mask bool, on the GPU")
+        lab, m = labels.contiguous(), vote_mask.contiguous().view(torch.uint8)
+        losses = torch.empty((2,), dtype=torch.float32, device=x.device)
+        num_valid = torch.empty((), dtype=torch.int64, device=x.device)
+        counts = torch.empty((2 * len(cfg.entry_names) + 1,), dtype=torch.int64, device=x.device)
+        c = L.ctx(x.device)
+        st, _keep = cfg.struct()
+        L.check(c, L.lib().sstb200_voteseg_loss_forward(c, C.byref(st), L.ptr(x), x.stride(0), L.ptr(v), v.stride(0), N, L.ptr(lab),
+                                                        L.ptr(t), L.ptr(m), L.ptr(losses), L.ptr(num_valid), L.ptr(counts)))
+        ctx.save_for_backward(x, v, lab, t, m, num_valid)
+        ctx.cfg, ctx.dtypes = cfg, (seg_logits.dtype, vote_preds.dtype)
+        ctx.mark_non_differentiable(counts)
+        return losses, counts
+
+    @staticmethod
+    def backward(ctx, grad_losses, _grad_counts=None):
+        x, v, lab, t, m, num_valid = ctx.saved_tensors
+        cfg = ctx.cfg
+        N = x.shape[0]
+        gx = torch.empty((N, cfg.num_classes), dtype=torch.float32, device=x.device)
+        gv = torch.empty((N, 3 * cfg.num_classes), dtype=torch.float32, device=x.device)
+        gl = grad_losses.float().contiguous()
+        c = L.ctx(x.device)
+        st, _keep = cfg.struct()
+        L.check(c, L.lib().sstb200_voteseg_loss_backward(c, C.byref(st), L.ptr(x), x.stride(0), L.ptr(v), v.stride(0), N, L.ptr(lab),
+                                                         L.ptr(t), L.ptr(m), L.ptr(num_valid), L.ptr(gl), L.ptr(gx), L.ptr(gv)))
+        return gx.to(ctx.dtypes[0]), gv.to(ctx.dtypes[1]), None, None, None, None
+
+
+def voteseg_loss(seg_logits, vote_preds, labels, vote_targets, vote_mask, cfg=None, **kwargs):
+    """(loss_sem_seg, loss_vote, metrics) of VoteSegLossFunction: two fp32 device scalars carrying gradients and a dict of
+    non-differentiable device tensors (recall_<name>, num_fg).  cfg: a VoteSegLossConfig, or its keyword arguments."""
+    if cfg is None:
+        cfg = VoteSegLossConfig(**kwargs)
+    losses, counts = VoteSegLossFunction.apply(seg_logits, vote_preds, labels, vote_targets, vote_mask, cfg)
+    return losses[0], losses[1], cfg.metrics(counts)
