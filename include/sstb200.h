@@ -829,6 +829,66 @@ int sstb200_voteseg_loss_backward(sstb200_ctx* ctx, const sstb200_voteseg_cfg* c
                                   const float* vote_targets, const uint8_t* vote_mask, const int64_t* num_valid, const float* grad_losses,
                                   float* grad_logits, float* grad_vote_preds);
 
+/* ---- SparseClusterHeadV2 training (mmdet3d/models/dense_heads/sparse_cluster_head{,_v2}.py), fp32, stream-ordered, no sync.
+ *
+ * sstb200_cluster_head_targets: get_targets of every task (v2 lines 299-405 after modify_gt_for_single_task, assign_single of v1 lines
+ *   364-397 with enlarge_width unset, assign_by_dist unset) for the whole batch in one launch.
+ *   cluster_xyz [M, >= 3] fp32 with row stride xyz_stride (floats); batch_idx int64 [M] with element stride batch_stride (column 1 of
+ *   cluster_inds [M, 3] is batch_idx = cluster_inds + 1, stride 3).  Clusters need not be sorted by sample.  gt_boxes [G, 7] bottom-centre
+ *   LiDAR boxes and gt_labels int64 [G] (global class ids), sample b owning rows [gt_offsets[b], gt_offsets[b + 1]) (host, batch + 1).
+ *   class_task / class_rank (host [num_classes]): the task of each global class and its position in that task's class list, task -1
+ *   for a class in no task.  task_classes (host [num_tasks]): C_t.
+ *   Per task t a cluster takes the GT of its own sample that contains it with the smallest (class rank, GT index): the first hit of
+ *   points_in_boxes_gpu over modify_gt_for_single_task's list, which concatenates the task's classes in order and keeps the input order
+ *   within a class.  A GT with a negative label or a class in no task takes part in no task.  The in-box test is sstb200_points_in_boxes'
+ *   (box3d.cuh), bit-identical to the reference kernel.
+ *   Outputs, per task t: labels[t] int64 [M] = the rank of the hit's class, C_t (background) without a hit; bbox_targets[t] f32 [M, 8] =
+ *   BasePointBBoxCoder.encode (xyz - cluster xyz, exact in fp32; log(dims + 1e-6) with the addition in fp32; sin(yaw), cos(yaw)), the
+ *   three transcendentals in double rounded once, zeros on negatives; num_pos int64 [T] (device) = the positives of each task.
+ *   A cluster whose batch index is outside [0, batch) gets label -1 and NaN targets in every task (the reference's boolean split would
+ *   give it no sample and a zero row), so the classification loss is NaN.  Every entry is written.
+ *   Errors: a NULL pointer, batch < 1, a stride below the row, offsets that do not start at 0 or decrease, a class mapped outside its
+ *   task (SSTB_ERR_ARG); more than 256 samples, 8 tasks, 64 classes or 4096 GTs in one sample (SSTB_ERR_UNSUPPORTED).
+ *
+ * sstb200_cluster_head_loss_forward: loss_single_task of every task (v2 lines 192-297) in one launch sequence.  Per task t,
+ *   cls_logits[t] [M, C_t] and reg_preds[t] [M, 8] are read in place with row strides logit_strides[t] / reg_strides[t]; labels[t],
+ *   bbox_targets[t] and num_pos from sstb200_cluster_head_targets; cls_avg_factor and reg_avg_factor fp32 [T] on the device.
+ *   losses f32 [T, 4] = (cls, center, size, rot) with
+ *   - cls: loss_weight_cls * sum focal / cls_avg_factor[t], mmdet 2.14 FocalLoss(use_sigmoid=True, gamma, alpha) against one-hot(label)
+ *     without the background column C_t, label_weights all ones, in the stable softplus form (see sstb200_voteseg_loss_forward for the
+ *     difference from mmcv's clamped CUDA kernel).  A label outside [0, C_t] makes it NaN.  gamma must be >= 1.
+ *   - center / size / rot: loss_weight_q * sum over the positives (0 <= label < C_t) of L1 |d| or, with smooth_l1, mmdet's SmoothL1
+ *     (|d| < beta ? 0.5 d^2 / beta : |d| - 0.5 beta) on columns [0, 3), [3, 6), [6, 8), over reg_avg_factor[t].  When the local
+ *     num_pos[t] is 0 they are exactly 0 whatever the factor (the reference's `num_pos > 0` branch takes pos_reg_preds.sum() * 0).
+ *   Block partials in double summed in a fixed order: deterministic.  Two launches, partials from the context arena.
+ * sstb200_cluster_head_loss_backward: grad_losses (device [T, 4]) -> grad_logits[t] [M, C_t] and grad_reg_preds[t] [M, 8], contiguous
+ *   and fully written; each cluster writes only its own rows, with no atomics, so two calls are bit-identical.  A NaN logit makes its own
+ *   gradient NaN and no other; the reg gradient is 0 off the positives and for a task with no local positive.  One launch.
+ *   Errors (both): a NULL pointer, M < 1, a row stride below the row, C_t < 1, SmoothL1 with beta <= 0 (SSTB_ERR_ARG); more than 8
+ *   tasks or 64 classes in a task, a gamma below 1 (SSTB_ERR_UNSUPPORTED). */
+typedef struct {
+  float gamma, alpha;                  /* focal loss */
+  int32_t smooth_l1;                   /* 0: L1Loss, 1: SmoothL1Loss(beta) for center, size and rot */
+  float beta;
+  float loss_weight_cls, loss_weight_center, loss_weight_size, loss_weight_rot;
+} sstb200_cluster_head_loss_cfg;
+int sstb200_cluster_head_targets(sstb200_ctx* ctx, const float* cluster_xyz, int64_t xyz_stride, const int64_t* batch_idx,
+                                 int64_t batch_stride, int64_t num_clusters, const float* gt_boxes, const int64_t* gt_labels,
+                                 const int32_t* gt_offsets, int batch, int num_classes, const int32_t* class_task, const int32_t* class_rank,
+                                 int num_tasks, const int32_t* task_classes, int64_t* const* labels, float* const* bbox_targets,
+                                 int64_t* num_pos);
+int sstb200_cluster_head_loss_forward(sstb200_ctx* ctx, const sstb200_cluster_head_loss_cfg* cfg, int num_tasks, int64_t num_clusters,
+                                      const float* const* cls_logits, const int64_t* logit_strides, const int32_t* task_classes,
+                                      const float* const* reg_preds, const int64_t* reg_strides, int64_t* const* labels,
+                                      float* const* bbox_targets, const int64_t* num_pos, const float* cls_avg_factor,
+                                      const float* reg_avg_factor, float* losses);
+int sstb200_cluster_head_loss_backward(sstb200_ctx* ctx, const sstb200_cluster_head_loss_cfg* cfg, int num_tasks, int64_t num_clusters,
+                                       const float* const* cls_logits, const int64_t* logit_strides, const int32_t* task_classes,
+                                       const float* const* reg_preds, const int64_t* reg_strides, int64_t* const* labels,
+                                       float* const* bbox_targets, const int64_t* num_pos, const float* cls_avg_factor,
+                                       const float* reg_avg_factor, const float* grad_losses, float* const* grad_logits,
+                                       float* const* grad_reg_preds);
+
 #ifdef __cplusplus
 }
 #endif

@@ -20,6 +20,8 @@ and error behaviour; no CPU path - CPU tensors raise.
     anchor3d_targets, anchor_focal_loss, anchor_reg_dir_loss
                                       models/dense_heads/anchor3d_head.py, train_mixins.py (Anchor3DHead training)
     voteseg_targets, voteseg_loss     models/decode_heads/segmentation_head.py:107-283 (VoteSegHead training)
+    cluster_head_targets, cluster_head_loss, multiclass_nms_groups
+                                      models/dense_heads/sparse_cluster_head_v2.py (SparseClusterHeadV2 training and proposals)
 """
 import ctypes as C
 import math
@@ -735,6 +737,13 @@ def nms_bev(boxes, seg_offsets, thresh, rotated=True):
     """Segmented greedy NMS (sstb200_nms_bev): boxes [num, 5] grouped into segments [seg_offsets[s], seg_offsets[s+1]), each sorted by
     descending score; thresh[s] per segment (None keeps the whole segment).  Returns int64 positions into `boxes` of the kept boxes,
     segment after segment, in score order; one host sync for their number."""
+    keep, num_dev = _nms_bev_async(boxes, seg_offsets, thresh, rotated)
+    return keep[:int(num_dev.item())]
+
+
+def _nms_bev_async(boxes, seg_offsets, thresh, rotated):
+    """nms_bev without reading the kept count: (keep int64 [num], whose first num_dev entries are valid, num_dev int32 [1] on the
+    device).  No host sync."""
     _need_cuda(boxes)
     b = _bev_boxes(boxes, "nms_bev")
     S = len(seg_offsets) - 1
@@ -748,10 +757,9 @@ def nms_bev(boxes, seg_offsets, thresh, rotated=True):
     ws = torch.empty((nbytes.value,), dtype=torch.uint8, device=b.device)
     keep = torch.empty((b.shape[0],), dtype=torch.int64, device=b.device)
     num_dev = torch.empty((1,), dtype=torch.int32, device=b.device)
-    num = C.c_int32()
     L.check(c, L.lib().sstb200_nms_bev(c, b.data_ptr(), b.shape[0], off, S, th, int(bool(rotated)), ws.data_ptr(), nbytes.value,
-                                       keep.data_ptr(), num_dev.data_ptr(), C.byref(num)))
-    return keep[:num.value]
+                                       keep.data_ptr(), num_dev.data_ptr(), None))
+    return keep, num_dev
 
 
 def nms_gpu(boxes, scores, thresh, pre_maxsize=None, post_max_size=None):
@@ -774,12 +782,70 @@ def nms_normal_gpu(boxes, scores, thresh):
     return order[nms_bev(boxes[order], [0, order.numel()], [thresh], rotated=False)].contiguous()
 
 
+def multiclass_nms_groups(mlvl_bboxes, mlvl_bboxes_for_nms, cls, idx, sc, group, num_groups, num_classes, nms_thrs, max_num, rotated,
+                          extras=()):
+    """box3d_multiclass_nms (box3d_nms.py:10-143) for `num_groups` independent groups of candidates in ONE segmented nms_bev call.
+    Candidate k is box idx[k] of mlvl_bboxes / mlvl_bboxes_for_nms, of class cls[k] in [0, num_classes), with score sc[k], in group
+    group[k] (int64 device tensors; group num_groups drops the candidate); within a (group, class) the candidates come in input order.
+    nms_thrs: one threshold per class,
+    None for no NMS.  Per group, the reference's order: classes in turn; within a class, descending score, or input order for a class
+    whose threshold is None; then, over max_num kept, the reference's own `scores.sort(descending=True)` cut.  Returns a list over
+    groups of (bboxes, scores, labels, *extras[idx of the kept]) or None for a group with nothing kept.  Whatever the number of groups,
+    one host sync for the candidates per (group, class) and, when some class has an NMS threshold, a second for the kept boxes per
+    group; with no threshold every candidate is kept and nms_bev is not called."""
+    _need_cuda(mlvl_bboxes, mlvl_bboxes_for_nms, cls, idx, sc, group, *extras)
+    dev = sc.device
+    seg = group * num_classes + cls
+    none = [t is None for t in nms_thrs]
+    if all(none):                                                      # a class without NMS keeps input order
+        key = torch.zeros_like(sc)
+    elif any(none):
+        key = torch.where(torch.tensor(none, dtype=torch.bool, device=dev)[cls], torch.zeros_like(sc), sc)
+    else:
+        key = sc
+    o = torch.sort(key, descending=True, stable=True).indices
+    o = o[torch.sort(seg[o], stable=True).indices]
+    S = (num_groups + 1) * num_classes
+    counts = torch.zeros((S,), dtype=torch.int64, device=dev).index_add_(0, seg, torch.ones_like(seg))
+    counts = counts.tolist()[:num_groups * num_classes]
+    n = sum(counts)
+    if n == 0:
+        return [None] * num_groups
+    o = o[:n]                                                          # the dropped candidates sort last
+    cls, idx, sc, group = cls[o], idx[o], sc[o], group[o]
+    if all(none):                  # nothing to suppress: every candidate is kept, in the order above, and the counts are known
+        keep = torch.arange(n, device=dev)
+        per = [sum(counts[g * num_classes:(g + 1) * num_classes]) for g in range(num_groups)]
+    else:
+        keep, num_dev = _nms_bev_async(mlvl_bboxes_for_nms[idx], _offsets(counts), list(nms_thrs) * num_groups, rotated)
+        K = keep.shape[0]
+        live = torch.arange(K, device=dev) < num_dev
+        keep = torch.where(live, keep, torch.zeros_like(keep))
+        kept_group = torch.where(live, group[keep], torch.full_like(keep, num_groups))
+        per = torch.zeros((num_groups + 1,), dtype=torch.int64, device=dev).index_add_(0, kept_group, torch.ones_like(kept_group))
+        per = per.tolist()[:num_groups]
+    out = []
+    for g, (a, b) in enumerate(zip(_offsets(per), _offsets(per)[1:])):
+        if a == b:
+            out.append(None)
+            continue
+        k = keep[a:b]
+        sel = idx[k]
+        res = [mlvl_bboxes[sel], sc[k], cls[k]] + [e[sel] for e in extras]
+        if b - a > max_num:
+            _, inds = res[1].sort(descending=True)
+            inds = inds[:max_num]
+            res = [r[inds] for r in res]
+        out.append(tuple(res))
+    return out
+
+
 def box3d_multiclass_nms(mlvl_bboxes, mlvl_bboxes_for_nms, mlvl_scores, score_thr, max_num, cfg, mlvl_dir_scores=None,
                          mlvl_attr_scores=None, mlvl_bboxes2d=None):
-    """box3d_nms.py:10-143 with every class in ONE segmented NMS call.  Same arguments, outputs and order: classes in turn, each
-    class's kept boxes by descending score (boxes in input order for a class whose nms_thr is None), then the reference's own
-    `scores.sort(descending=True)` when more than max_num remain.  Within a class, equal scores are taken in input order; the reference
-    takes them in torch's sort order, so the two agree whenever a class has no tied scores."""
+    """box3d_nms.py:10-143 with every class in ONE segmented NMS call (the one-group case of multiclass_nms_groups).  Same arguments,
+    outputs and order: classes in turn, each class's kept boxes by descending score (boxes in input order for a class whose nms_thr is
+    None), then the reference's own `scores.sort(descending=True)` when more than max_num remain.  Within a class, equal scores are
+    taken in input order; the reference takes them in torch's sort order, so the two agree whenever a class has no tied scores."""
     _need_cuda(mlvl_bboxes, mlvl_bboxes_for_nms, mlvl_scores, mlvl_dir_scores, mlvl_attr_scores, mlvl_bboxes2d)
     num_classes = mlvl_scores.shape[1] - 1
     dev = mlvl_scores.device
@@ -797,42 +863,13 @@ def box3d_multiclass_nms(mlvl_bboxes, mlvl_bboxes_for_nms, mlvl_scores, score_th
     cls_scores = mlvl_scores[:, :num_classes]
     thr = torch.tensor([float(t) for t in score_thrs], dtype=mlvl_scores.dtype, device=dev)
     cls, idx = (cls_scores > thr).t().nonzero(as_tuple=True)           # class-major, input order within a class
-    sc = cls_scores[idx, cls]
-    no_nms = torch.tensor([t is None for t in nms_thrs], dtype=torch.bool, device=dev)
-    key = torch.where(no_nms[cls], torch.zeros_like(sc), sc)           # a class without NMS keeps input order
-    o = torch.sort(key, descending=True, stable=True).indices
-    o = o[torch.sort(cls[o], stable=True).indices]
-    cls, idx, sc = cls[o], idx[o], sc[o]
-    counts = torch.bincount(cls, minlength=num_classes).tolist()
-    if sum(counts) == 0:
-        bboxes = mlvl_scores.new_zeros((0, mlvl_bboxes.size(-1)))
-        scores = mlvl_scores.new_zeros((0,))
-        labels = mlvl_scores.new_zeros((0,), dtype=torch.long)
-        dir_scores = mlvl_scores.new_zeros((0,)) if mlvl_dir_scores is not None else None
-        attr_scores = mlvl_scores.new_zeros((0,)) if mlvl_attr_scores is not None else None
-        bboxes2d = mlvl_scores.new_zeros((0, 4)) if mlvl_bboxes2d is not None else None
-    else:
-        offsets = [0]
-        for n in counts:
-            offsets.append(offsets[-1] + n)
-        keep = nms_bev(mlvl_bboxes_for_nms[idx], offsets, nms_thrs, rotated=cfg.use_rotate_nms)
-        sel = idx[keep]
-        bboxes, scores, labels = mlvl_bboxes[sel], sc[keep], cls[keep]
-        dir_scores = mlvl_dir_scores[sel] if mlvl_dir_scores is not None else None
-        attr_scores = mlvl_attr_scores[sel] if mlvl_attr_scores is not None else None
-        bboxes2d = mlvl_bboxes2d[sel] if mlvl_bboxes2d is not None else None
-        if bboxes.shape[0] > max_num:
-            _, inds = scores.sort(descending=True)
-            inds = inds[:max_num]
-            bboxes, labels, scores = bboxes[inds, :], labels[inds], scores[inds]
-            dir_scores = dir_scores[inds] if dir_scores is not None else None
-            attr_scores = attr_scores[inds] if attr_scores is not None else None
-            bboxes2d = bboxes2d[inds] if bboxes2d is not None else None
-    results = (bboxes, scores, labels)
-    for extra, given in ((dir_scores, mlvl_dir_scores), (attr_scores, mlvl_attr_scores), (bboxes2d, mlvl_bboxes2d)):
-        if given is not None:
-            results = results + (extra,)
-    return results
+    given = [e for e in (mlvl_dir_scores, mlvl_attr_scores, mlvl_bboxes2d) if e is not None]
+    res = multiclass_nms_groups(mlvl_bboxes, mlvl_bboxes_for_nms, cls, idx, cls_scores[idx, cls], torch.zeros_like(cls), 1,
+                                num_classes, nms_thrs, max_num, cfg.use_rotate_nms, given)[0]
+    if res is None:
+        res = (mlvl_scores.new_zeros((0, mlvl_bboxes.size(-1))), mlvl_scores.new_zeros((0,)), mlvl_scores.new_zeros((0,), dtype=torch.long))
+        res = res + tuple(mlvl_scores.new_zeros((0, 4) if e is mlvl_bboxes2d else (0,)) for e in given)
+    return res
 
 
 # ----------------------------------------------------------------------------------------------
@@ -1603,3 +1640,194 @@ def voteseg_loss(seg_logits, vote_preds, labels, vote_targets, vote_mask, cfg=No
         cfg = VoteSegLossConfig(**kwargs)
     losses, counts = VoteSegLossFunction.apply(seg_logits, vote_preds, labels, vote_targets, vote_mask, cfg)
     return losses[0], losses[1], cfg.metrics(counts)
+
+
+# ----------------------------------------------------------------------------------------------
+# SparseClusterHeadV2 training (mmdet3d/models/dense_heads/sparse_cluster_head{,_v2}.py)
+# ----------------------------------------------------------------------------------------------
+class _ClusterHeadCfg(C.Structure):
+    _fields_ = [("gamma", C.c_float), ("alpha", C.c_float), ("smooth_l1", C.c_int32), ("beta", C.c_float),
+                ("loss_weight_cls", C.c_float), ("loss_weight_center", C.c_float), ("loss_weight_size", C.c_float),
+                ("loss_weight_rot", C.c_float)]
+
+
+_CH_ARGS = [L.vp, C.POINTER(_ClusterHeadCfg), C.c_int, C.c_int64, _PP, L.P_i64, L.P_i32, _PP, L.P_i64, _PP, _PP, L.vp, L.vp, L.vp]
+L.SIGNATURES["sstb200_cluster_head_targets"] = (C.c_int, [L.vp, L.vp, C.c_int64, L.vp, C.c_int64, C.c_int64, L.vp, L.vp, L.P_i32, C.c_int,
+                                                          C.c_int, L.P_i32, L.P_i32, C.c_int, L.P_i32, _PP, _PP, L.vp])
+L.SIGNATURES["sstb200_cluster_head_loss_forward"] = (C.c_int, _CH_ARGS + [L.vp])
+L.SIGNATURES["sstb200_cluster_head_loss_backward"] = (C.c_int, _CH_ARGS + [L.vp, _PP, _PP])
+
+CLUSTER_HEAD_CODE_SIZE = 8
+
+
+def _batch_index(cluster_inds, M):
+    """the cluster batch index read in place: column 1 of int64 cluster_inds [M, 3], or a 1-D int64 index -> (tensor, element stride)"""
+    if not isinstance(cluster_inds, torch.Tensor) or not cluster_inds.is_cuda or cluster_inds.dtype != torch.int64:
+        raise L.SSTB200Error("cluster_head_targets: cluster_inds must be an int64 CUDA tensor")
+    if cluster_inds.dim() == 2:
+        if cluster_inds.shape[1] < 2 or cluster_inds.shape[0] != M:
+            raise L.SSTB200Error(f"cluster_head_targets: cluster_inds {tuple(cluster_inds.shape)} for {M} clusters")
+        col = cluster_inds[:, 1]
+    elif cluster_inds.dim() == 1 and cluster_inds.shape[0] == M:
+        col = cluster_inds
+    else:
+        raise L.SSTB200Error(f"cluster_head_targets: cluster_inds {tuple(cluster_inds.shape)} for {M} clusters")
+    if M and col.stride(0) < 1:
+        col = col.contiguous()
+    return col, max(col.stride(0), 1)
+
+
+def cluster_head_targets(cluster_xyz, cluster_inds, gt_boxes, gt_labels, tasks, class_names):
+    """SparseClusterHeadV2.get_targets of every task for the whole batch in one launch.  cluster_xyz fp32 [M, >= 3] (read in place, any
+    row stride); cluster_inds int64 [M, 3] (column 1 is the sample) or [M]; gt_boxes: a list over samples of [G_b, >= 7] bottom-centre
+    boxes (tensors or objects with `.tensor`), gt_labels: a list of int64 [G_b] global class ids; tasks: lists of class names per task,
+    class_names: the global class list.  Returns (labels, bbox_targets, num_pos): lists over tasks of int64 [M] (background = the task's
+    class count), fp32 [M, 8] (zeros on negatives) and an int64 [T] device tensor of the positives.  A cluster whose sample index is
+    outside [0, B) gets label -1 and NaN targets.  No host sync."""
+    xyz = cluster_xyz
+    if not isinstance(xyz, torch.Tensor) or not xyz.is_cuda or xyz.dtype != torch.float32 or xyz.dim() != 2 or xyz.shape[1] < 3:
+        raise L.SSTB200Error("cluster_head_targets: cluster_xyz must be a float32 [M, >= 3] CUDA tensor")
+    if xyz.stride(1) != 1 or xyz.stride(0) < 3:
+        xyz = xyz.contiguous()
+    M = xyz.shape[0]
+    bidx, bstride = _batch_index(cluster_inds, M)
+    if bidx.device != xyz.device:
+        raise L.SSTB200Error(f"cluster_head_targets: cluster_inds on {bidx.device}, cluster_xyz on {xyz.device}")
+    B = len(gt_boxes)
+    if B < 1 or len(gt_labels) != B:
+        raise L.SSTB200Error(f"cluster_head_targets: {len(gt_boxes)} box and {len(gt_labels)} label lists")
+    names = list(class_names)
+    class_task, class_rank = [-1] * len(names), [0] * len(names)
+    for t, task in enumerate(tasks):
+        for r, n in enumerate(task):
+            k = names.index(n)
+            class_task[k], class_rank[k] = t, r
+    T = len(tasks)
+    dev = xyz.device
+    boxes = [getattr(b, "tensor", b) for b in gt_boxes]
+    for b, lab in zip(boxes, gt_labels):
+        if b.dim() != 2 or b.shape[1] < 7 or lab.shape != (b.shape[0],):
+            raise L.SSTB200Error(f"cluster_head_targets: boxes {tuple(b.shape)} and labels {tuple(lab.shape)} do not match")
+    gt = torch.cat([b[:, :7] for b in boxes]).to(dev, torch.float32).contiguous()
+    gl = torch.cat([lab.reshape(-1) for lab in gt_labels]).to(dev, torch.int64).contiguous()
+    labels = [torch.empty((M,), dtype=torch.int64, device=dev) for _ in range(T)]
+    targets = [torch.empty((M, CLUSTER_HEAD_CODE_SIZE), dtype=torch.float32, device=dev) for _ in range(T)]
+    num_pos = torch.empty((T,), dtype=torch.int64, device=dev)
+    c = L.ctx(dev)
+    L.check(c, L.lib().sstb200_cluster_head_targets(
+        c, L.ptr(xyz) if M else None, xyz.stride(0), L.ptr(bidx) if M else None, bstride, M, L.ptr(gt) if gt.numel() else None,
+        L.ptr(gl) if gl.numel() else None, L.arr(C.c_int32, _offsets([b.shape[0] for b in boxes])), B, len(names),
+        L.arr(C.c_int32, class_task), L.arr(C.c_int32, class_rank), T, L.arr(C.c_int32, [len(t) for t in tasks]), _ptrs(labels),
+        _ptrs(targets), L.ptr(num_pos)))
+    return labels, targets, num_pos
+
+
+class ClusterHeadLossConfig:
+    """The constant part of SparseClusterHeadV2.loss_single_task: the focal settings of loss_cls and the L1 / SmoothL1 settings and
+    weights of loss_center / loss_size / loss_rot (the three must share their type and beta).  Built once per head."""
+
+    def __init__(self, gamma=2.0, alpha=0.25, loss_weight_cls=1.0, loss_weight_center=1.0, loss_weight_size=1.0, loss_weight_rot=1.0,
+                 smooth_l1=False, beta=1.0):
+        self.gamma, self.alpha, self.smooth_l1, self.beta = float(gamma), float(alpha), bool(smooth_l1), float(beta)
+        self.weights = (float(loss_weight_cls), float(loss_weight_center), float(loss_weight_size), float(loss_weight_rot))
+
+    def struct(self):
+        return _ClusterHeadCfg(self.gamma, self.alpha, int(self.smooth_l1), self.beta, *self.weights)
+
+
+def _cluster_head_loss_inputs(labels, targets, num_pos, cls_avg, reg_avg, preds):
+    """every tensor the loss kernels read as a raw device array, checked: the T cls_logits [M, C_t] and T reg_preds [M, 8] fp32 rows
+    with unit column stride, labels int64 [M] and bbox_targets fp32 [M, 8] per task, num_pos int64 [T] and the fp32 avg factors [T],
+    all CUDA tensors on the predictions' device.  Shapes and dtypes are checked before devices.  Returns them contiguous where the
+    kernels need it."""
+    T = len(labels)
+    if T < 1 or len(targets) != T or len(preds) != 2 * T:
+        raise L.SSTB200Error(f"cluster_head_loss: {len(preds)} predictions, {len(labels)} labels and {len(targets)} bbox_targets; "
+                             "one cls_logits, reg_preds, labels and bbox_targets per task")
+    for name, t in [("num_pos", num_pos), ("cls_avg_factor", cls_avg), ("reg_avg_factor", reg_avg)] + \
+            [(f"labels[{k}]", a) for k, a in enumerate(labels)] + [(f"bbox_targets[{k}]", a) for k, a in enumerate(targets)] + \
+            [(f"prediction {k}", a) for k, a in enumerate(preds)]:
+        if not isinstance(t, torch.Tensor):
+            raise L.SSTB200Error(f"cluster_head_loss: {name} must be a tensor, got {type(t).__name__}")
+    M = preds[0].shape[0] if preds[0].dim() == 2 else -1
+    if M < 1:
+        raise L.SSTB200Error(f"cluster_head_loss: cls_logits[0] must be [M, C] with M > 0, got {tuple(preds[0].shape)}")
+    for k in range(T):
+        x, r = preds[k], preds[T + k]
+        if x.dim() != 2 or x.shape[0] != M or x.shape[1] < 1 or r.shape != (M, CLUSTER_HEAD_CODE_SIZE):
+            raise L.SSTB200Error(f"cluster_head_loss: task {k}: cls_logits {tuple(x.shape)} and reg_preds {tuple(r.shape)} do not fit "
+                                 f"[{M}, C] and [{M}, {CLUSTER_HEAD_CODE_SIZE}]")
+        if labels[k].dtype != torch.int64 or labels[k].shape != (M,):
+            raise L.SSTB200Error(f"cluster_head_loss: labels[{k}] must be int64 [{M}], got {labels[k].dtype} {tuple(labels[k].shape)}")
+        if targets[k].dtype != torch.float32 or targets[k].shape != (M, CLUSTER_HEAD_CODE_SIZE):
+            raise L.SSTB200Error(f"cluster_head_loss: bbox_targets[{k}] must be float32 [{M}, {CLUSTER_HEAD_CODE_SIZE}], got "
+                                 f"{targets[k].dtype} {tuple(targets[k].shape)}")
+    if num_pos.dtype != torch.int64 or num_pos.shape != (T,):
+        raise L.SSTB200Error(f"cluster_head_loss: num_pos must be int64 [{T}], got {num_pos.dtype} {tuple(num_pos.shape)}")
+    for name, f in (("cls_avg_factor", cls_avg), ("reg_avg_factor", reg_avg)):
+        if f.dtype not in (torch.float32, torch.float16) or f.shape != (T,):
+            raise L.SSTB200Error(f"cluster_head_loss: {name} must be float32 [{T}], got {f.dtype} {tuple(f.shape)}")
+    xs = [_row_major(f"cls_logits[{k}]", x, x.shape[1]) for k, x in enumerate(preds[:T])]
+    rs = [_row_major(f"reg_preds[{k}]", r, CLUSTER_HEAD_CODE_SIZE) for k, r in enumerate(preds[T:])]
+    dev = xs[0].device
+    named = [(f"cls_logits[{k}]", a) for k, a in enumerate(xs)] + [(f"reg_preds[{k}]", a) for k, a in enumerate(rs)] + \
+        [(f"labels[{k}]", a) for k, a in enumerate(labels)] + [(f"bbox_targets[{k}]", a) for k, a in enumerate(targets)] + \
+        [("num_pos", num_pos), ("cls_avg_factor", cls_avg), ("reg_avg_factor", reg_avg)]
+    for name, t in named:
+        if not t.is_cuda or t.device != dev:
+            raise L.SSTB200Error(f"cluster_head_loss: {name} is on {t.device}; every input must be a CUDA tensor on {dev}")
+    labels = [a.contiguous() for a in labels]
+    targets = [_fp32_cuda(f"bbox_targets[{k}]", a, 2) for k, a in enumerate(targets)]
+    return (xs, rs, labels, targets, num_pos.contiguous(), _fp32_cuda("cls_avg_factor", cls_avg, 1),
+            _fp32_cuda("reg_avg_factor", reg_avg, 1))
+
+
+class ClusterHeadLossFunction(Function):
+    """loss_single_task of every task in one launch sequence (sstb200_cluster_head_loss_forward): returns losses [T, 4] = (cls, center,
+    size, rot) per task.  Inputs: cfg, the targets of cluster_head_targets, the device avg factors cls_avg [T] and reg_avg [T], then the
+    T cls_logits [M, C_t] and the T reg_preds [M, 8], read in place with their row strides.  Saves the predictions, targets and factors
+    only; the backward writes each cluster's own rows with no atomics (bit-identical from run to run).  No host sync."""
+
+    @staticmethod
+    def forward(ctx, cfg, labels, targets, num_pos, cls_avg, reg_avg, *preds):
+        T = len(labels)
+        xs, rs, labels, targets, num_pos, ca, ra = _cluster_head_loss_inputs(labels, targets, num_pos, cls_avg, reg_avg, preds)
+        M = xs[0].shape[0]
+        losses = torch.empty((T, 4), dtype=torch.float32, device=xs[0].device)
+        c = L.ctx(xs[0].device)
+        st = cfg.struct()
+        args = (c, C.byref(st), T, M, _ptrs(xs), L.arr(C.c_int64, [x.stride(0) for x in xs]), L.arr(C.c_int32, [x.shape[1] for x in xs]),
+                _ptrs(rs), L.arr(C.c_int64, [r.stride(0) for r in rs]), _ptrs(labels), _ptrs(targets), L.ptr(num_pos), L.ptr(ca), L.ptr(ra))
+        L.check(c, L.lib().sstb200_cluster_head_loss_forward(*args, L.ptr(losses)))
+        ctx.save_for_backward(num_pos, ca, ra, *xs, *rs, *labels, *targets)
+        ctx.cfg, ctx.T, ctx.dtypes = cfg, T, [p.dtype for p in preds]
+        return losses
+
+    @staticmethod
+    def backward(ctx, grad_losses):
+        T = ctx.T
+        saved = ctx.saved_tensors
+        num_pos, ca, ra = saved[:3]
+        xs, rs, labels, targets = saved[3:3 + T], saved[3 + T:3 + 2 * T], saved[3 + 2 * T:3 + 3 * T], saved[3 + 3 * T:]
+        M = xs[0].shape[0]
+        gx = [torch.empty((M, x.shape[1]), dtype=torch.float32, device=x.device) for x in xs]
+        gr = [torch.empty((M, CLUSTER_HEAD_CODE_SIZE), dtype=torch.float32, device=x.device) for x in xs]
+        gl = grad_losses.float().contiguous()
+        c = L.ctx(xs[0].device)
+        st = ctx.cfg.struct()
+        L.check(c, L.lib().sstb200_cluster_head_loss_backward(
+            c, C.byref(st), T, M, _ptrs(xs), L.arr(C.c_int64, [x.stride(0) for x in xs]), L.arr(C.c_int32, [x.shape[1] for x in xs]),
+            _ptrs(rs), L.arr(C.c_int64, [r.stride(0) for r in rs]), _ptrs(labels), _ptrs(targets), L.ptr(num_pos), L.ptr(ca), L.ptr(ra),
+            L.ptr(gl), _ptrs(gx), _ptrs(gr)))
+        grads = [g.to(d) for g, d in zip(gx + gr, ctx.dtypes)]
+        return (None, None, None, None, None, None, *grads)
+
+
+def cluster_head_loss(cls_logits, reg_preds, labels, bbox_targets, num_pos, cls_avg_factor, reg_avg_factor, cfg):
+    """losses [T, 4] = (loss_cls, loss_center, loss_size, loss_rot) per task of ClusterHeadLossFunction, an fp32 device tensor carrying
+    gradients to the T cls_logits and T reg_preds.  cls_avg_factor / reg_avg_factor: fp32 device [T] (see SparseClusterHeadV2.loss for
+    how the head forms them).  A misshapen, mistyped or off-device input raises SSTB200Error."""
+    if len(cls_logits) != len(labels) or len(reg_preds) != len(labels) or len(bbox_targets) != len(labels):
+        raise L.SSTB200Error("cluster_head_loss: one cls_logits, reg_preds, labels and bbox_targets per task")
+    return ClusterHeadLossFunction.apply(cfg, list(labels), list(bbox_targets), num_pos, cls_avg_factor, reg_avg_factor, *cls_logits,
+                                         *reg_preds)
