@@ -20,11 +20,11 @@
 #include <stdarg.h>
 #include <algorithm>
 #include <climits>
-#include "common.cuh"
+#include "heads.cuh"
 
 namespace {
 
-#define A3_THREADS 256
+#define A3_THREADS 256  // targets block
 #define A3_MAX_BATCH 256
 #define A3_MAX_SIZES 8
 #define A3_MAX_ROTS 8
@@ -268,34 +268,8 @@ __global__ void a3_total_kernel(const int* npos, int B, int64_t* num_total_pos) 
 }
 
 // ---- losses -------------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ double a3_block_sum(double v, double* sh) {
-#pragma unroll
-  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += sh[w];
-  __syncthreads();
-  return s;  // valid in thread 0
-}
-
-// sigmoid focal loss, gamma 2, alpha 0.25, on the stable form: softplus(+-x) = max(+-x, 0) + log1p(exp(-|x|)), s = sigmoid(x),
-// q = 1 - s = sigmoid(-x) from the same exp(-|x|)
-struct Sig {
-  float s, q, sp_pos, sp_neg;
-};
-
-__device__ __forceinline__ Sig sig(float x) {
-  const float e = expf(-fabsf(x)), inv = 1.f / (1.f + e), l1p = log1pf(e);
-  Sig r;
-  r.s = x >= 0.f ? inv : e * inv;
-  r.q = x >= 0.f ? e * inv : inv;
-  r.sp_pos = fmaxf(x, 0.f) + l1p;
-  r.sp_neg = fmaxf(-x, 0.f) + l1p;
-  return r;
-}
-
+// sigmoid focal loss, gamma 2, alpha 0.25, on heads.cuh's sig.  Not heads.cuh's sigmoid_focal: q * q is other arithmetic than
+// powf(q, 2.f).
 #define FOCAL_ALPHA 0.25f
 
 __device__ __forceinline__ float focal_loss(float x, bool t) {
@@ -328,8 +302,8 @@ __device__ __forceinline__ void focal_elem(const FocalArgs& a, long long i, bool
   w = __ldg(a.label_w + slot);
 }
 
-__global__ void __launch_bounds__(A3_THREADS) focal_forward_kernel(const FocalArgs a, double* part) {
-  __shared__ double sh[A3_THREADS / 32];
+__global__ void __launch_bounds__(LOSS_THREADS) focal_forward_kernel(const FocalArgs a, double* part) {
+  __shared__ double sh[LOSS_THREADS / 32];
   double acc = 0.0;
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) {
@@ -338,12 +312,12 @@ __global__ void __launch_bounds__(A3_THREADS) focal_forward_kernel(const FocalAr
     focal_elem(a, i, t, w);
     acc += (double)(focal_loss(__ldg(a.x + i), t) * w);
   }
-  acc = a3_block_sum(acc, sh);
+  acc = thread0_block_sum(acc, sh);
   if (threadIdx.x == 0) part[blockIdx.x] = acc;
 }
 
-__global__ void __launch_bounds__(A3_THREADS) focal_backward_kernel(const FocalArgs a, float loss_weight, const int64_t* num_total_pos,
-                                                                    const float* grad_loss, float* grad_x) {
+__global__ void __launch_bounds__(LOSS_THREADS) focal_backward_kernel(const FocalArgs a, float loss_weight, const int64_t* num_total_pos,
+                                                                      const float* grad_loss, float* grad_x) {
   const float scale = (float)((double)grad_loss[0] * loss_weight / (double)*num_total_pos);
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) {
@@ -355,13 +329,11 @@ __global__ void __launch_bounds__(A3_THREADS) focal_backward_kernel(const FocalA
 }
 
 // sum of nparts partials (per output k: part[k * nparts + i]) in a fixed order -> out[k] = weight[k] * sum / num_total_pos
-__global__ void __launch_bounds__(A3_THREADS) a3_final_kernel(const double* part, int nparts, int nout, float w0, float w1,
-                                                              const int64_t* num_total_pos, float* out0, float* out1) {
-  __shared__ double sh[A3_THREADS / 32];
+__global__ void __launch_bounds__(LOSS_THREADS) a3_final_kernel(const double* part, int nparts, int nout, float w0, float w1,
+                                                                const int64_t* num_total_pos, float* out0, float* out1) {
+  __shared__ double sh[LOSS_THREADS / 32];
   for (int k = 0; k < nout; k++) {
-    double acc = 0.0;
-    for (int i = threadIdx.x; i < nparts; i += blockDim.x) acc += part[(size_t)k * nparts + i];
-    acc = a3_block_sum(acc, sh);
+    const double acc = sum_partials(part, nparts, k, sh);
     if (threadIdx.x == 0) *(k ? out1 : out0) = (float)((double)(k ? w1 : w0) * (acc / (double)*num_total_pos));
   }
 }
@@ -392,8 +364,8 @@ __device__ __forceinline__ bool is_pos(const RegArgs& a, long long slot) {
   return l >= 0 && l < a.C;
 }
 
-__global__ void __launch_bounds__(A3_THREADS) reg_forward_kernel(const RegArgs a, double* part, int nparts) {
-  __shared__ double sh[A3_THREADS / 32];
+__global__ void __launch_bounds__(LOSS_THREADS) reg_forward_kernel(const RegArgs a, double* part, int nparts) {
+  __shared__ double sh[LOSS_THREADS / 32];
   double l1 = 0.0, ce = 0.0;
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) {
@@ -414,14 +386,18 @@ __global__ void __launch_bounds__(A3_THREADS) reg_forward_kernel(const RegArgs a
     const float lse = fmaxf(z0, z1) + log1pf(expf(-fabsf(z0 - z1)));
     ce += (double)((lse - (a.dir_t[slot] ? z1 : z0)) * a.dir_w[slot]);
   }
-  l1 = a3_block_sum(l1, sh);
-  ce = a3_block_sum(ce, sh);
+  l1 = thread0_block_sum(l1, sh);
+  ce = thread0_block_sum(ce, sh);
   if (threadIdx.x == 0) part[blockIdx.x] = l1, part[nparts + blockIdx.x] = ce;
 }
 
+// sign(d) with NaN passed through; torch.abs' gradient (heads.cuh's abs_grad) is 0 at NaN, a behaviour change kept for a separate fix
+__device__ __forceinline__ float sign_nan(float d) { return d > 0.f ? 1.f : (d < 0.f ? -1.f : (d == d ? 0.f : d)); }
+
 // every (b, anchor, cell) owns its 7 + 2 channels: the gradients are written in full, zero off the positives
-__global__ void __launch_bounds__(A3_THREADS) reg_backward_kernel(const RegArgs a, float w_bbox, float w_dir, const int64_t* num_total_pos,
-                                                                  const float* grad_loss, float* grad_bbox, float* grad_dir) {
+__global__ void __launch_bounds__(LOSS_THREADS) reg_backward_kernel(const RegArgs a, float w_bbox, float w_dir,
+                                                                    const int64_t* num_total_pos, const float* grad_loss, float* grad_bbox,
+                                                                    float* grad_dir) {
   const double inv = 1.0 / (double)*num_total_pos;
   const float sb = (float)((double)grad_loss[0] * w_bbox * inv), sd = (float)((double)grad_loss[1] * w_dir * inv);
   const long long stride = (long long)gridDim.x * blockDim.x;
@@ -444,14 +420,14 @@ __global__ void __launch_bounds__(A3_THREADS) reg_backward_kernel(const RegArgs 
 #pragma unroll
     for (int k = 0; k < 6; k++) {
       const float df = p[k * a.HW] - t[k];
-      gb[k * a.HW] = sb * (w[k] * a.cw[k]) * (df > 0.f ? 1.f : (df < 0.f ? -1.f : (df == df ? 0.f : df)));
+      gb[k * a.HW] = sb * (w[k] * a.cw[k]) * sign_nan(df);
     }
     const float p6 = p[6 * a.HW], t6 = t[6];
     float sp, cp, st, ct;
     sincosf(p6, &sp, &cp);
     sincosf(t6, &st, &ct);
     const float df = sp * ct - cp * st;
-    const float sgn = df > 0.f ? 1.f : (df < 0.f ? -1.f : (df == df ? 0.f : df));
+    const float sgn = sign_nan(df);
     gb[6 * a.HW] = sb * (w[6] * a.cw[6]) * sgn * (cp * ct + sp * st);
     const float* d = a.dir + ba * 2 * a.HW + hw;
     const float z0 = d[0], z1 = d[a.HW];
@@ -461,11 +437,6 @@ __global__ void __launch_bounds__(A3_THREADS) reg_backward_kernel(const RegArgs 
     gd[0] = g * (p0 - (t1 ? 0.f : 1.f));
     gd[a.HW] = g * (p1 - (t1 ? 1.f : 0.f));
   }
-}
-
-int loss_grid(sstb200_ctx* c, long long n) {
-  const long long want = (n + A3_THREADS * 8 - 1) / (A3_THREADS * 8);
-  return (int)std::max(1LL, std::min(want, (long long)c->num_sms * 8));
 }
 
 int focal_args(sstb200_ctx* c, const float* cls_score, int batch, int num_anchors, int num_classes, int height, int width,
@@ -508,13 +479,8 @@ extern "C" int sstb200_anchor3d_targets(sstb200_ctx* c, const float* x_centers, 
   if (batch > A3_MAX_BATCH || num_sizes > A3_MAX_SIZES || num_rots > A3_MAX_ROTS)
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "anchor3d_targets: %d samples / %d sizes / %d rotations, at most %d / %d / %d", batch,
                      num_sizes, num_rots, A3_MAX_BATCH, A3_MAX_SIZES, A3_MAX_ROTS);
-  CHECK_ARG(c, sample_offsets[0] == 0);
-  for (int b = 0; b < batch; b++) {
-    CHECK_ARG(c, sample_offsets[b + 1] >= sample_offsets[b]);
-    if (sample_offsets[b + 1] - sample_offsets[b] > A3_MAX_GT)
-      return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "anchor3d_targets: sample %d has %d GT boxes, at most %d", b,
-                       sample_offsets[b + 1] - sample_offsets[b], A3_MAX_GT);
-  }
+  int rc = check_offsets(c, "anchor3d_targets", sample_offsets, batch, A3_MAX_GT);
+  if (rc) return rc;
   const int N = sample_offsets[batch];
   CHECK_ARG(c, N == 0 || (gt_boxes && gt_labels));
   const long long per_size = (long long)height * width * num_rots;
@@ -534,7 +500,7 @@ extern "C" int sstb200_anchor3d_targets(sstb200_ctx* c, const float* x_centers, 
   a.dir_w = dir_weights, a.num_total_pos = num_total_pos;
   const size_t SN = std::max<size_t>(1, (size_t)num_sizes * N), BA = (size_t)batch * A;
   arena_reset(c);
-  int rc = arena_carve(c, [&](Carve& cv) {
+  rc = arena_carve(c, [&](Carve& cv) {
     a.gt_max = cv.take<unsigned>(SN);
     a.gt_arg = cv.take<int>(SN);
     a.nvalid = cv.take<int>((size_t)batch * num_sizes);
@@ -576,9 +542,9 @@ extern "C" int sstb200_anchor_focal_loss_forward(sstb200_ctx* c, const float* cl
   double* part;
   rc = arena_carve(c, [&](Carve& cv) { part = cv.take<double>(nb); });
   if (rc) return rc;
-  focal_forward_kernel<<<nb, A3_THREADS, 0, c->stream>>>(a, part);
+  focal_forward_kernel<<<nb, LOSS_THREADS, 0, c->stream>>>(a, part);
   LAUNCH_CHECK(c);
-  a3_final_kernel<<<1, A3_THREADS, 0, c->stream>>>(part, nb, 1, loss_weight, 0.f, num_total_pos, loss, nullptr);
+  a3_final_kernel<<<1, LOSS_THREADS, 0, c->stream>>>(part, nb, 1, loss_weight, 0.f, num_total_pos, loss, nullptr);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }
@@ -591,7 +557,7 @@ extern "C" int sstb200_anchor_focal_loss_backward(sstb200_ctx* c, const float* c
   int rc = focal_args(c, cls_score, batch, num_anchors, num_classes, height, width, labels, label_weights, num_total_pos, a);
   if (rc) return rc;
   CHECK_ARG(c, grad_loss && grad_cls_score);
-  focal_backward_kernel<<<loss_grid(c, a.n), A3_THREADS, 0, c->stream>>>(a, loss_weight, num_total_pos, grad_loss, grad_cls_score);
+  focal_backward_kernel<<<loss_grid(c, a.n), LOSS_THREADS, 0, c->stream>>>(a, loss_weight, num_total_pos, grad_loss, grad_cls_score);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }
@@ -611,9 +577,9 @@ extern "C" int sstb200_anchor_reg_dir_loss_forward(sstb200_ctx* c, const float* 
   double* part;
   rc = arena_carve(c, [&](Carve& cv) { part = cv.take<double>(2 * nb); });
   if (rc) return rc;
-  reg_forward_kernel<<<nb, A3_THREADS, 0, c->stream>>>(a, part, nb);
+  reg_forward_kernel<<<nb, LOSS_THREADS, 0, c->stream>>>(a, part, nb);
   LAUNCH_CHECK(c);
-  a3_final_kernel<<<1, A3_THREADS, 0, c->stream>>>(part, nb, 2, loss_weight_bbox, loss_weight_dir, num_total_pos, loss_bbox, loss_dir);
+  a3_final_kernel<<<1, LOSS_THREADS, 0, c->stream>>>(part, nb, 2, loss_weight_bbox, loss_weight_dir, num_total_pos, loss_bbox, loss_dir);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }
@@ -629,8 +595,8 @@ extern "C" int sstb200_anchor_reg_dir_loss_backward(sstb200_ctx* c, const float*
                     dir_targets, dir_weights, code_weight, num_total_pos, a);
   if (rc) return rc;
   CHECK_ARG(c, grad_losses && grad_bbox_pred && grad_dir_cls_preds);
-  reg_backward_kernel<<<loss_grid(c, a.n), A3_THREADS, 0, c->stream>>>(a, loss_weight_bbox, loss_weight_dir, num_total_pos, grad_losses,
-                                                                       grad_bbox_pred, grad_dir_cls_preds);
+  reg_backward_kernel<<<loss_grid(c, a.n), LOSS_THREADS, 0, c->stream>>>(a, loss_weight_bbox, loss_weight_dir, num_total_pos, grad_losses,
+                                                                         grad_bbox_pred, grad_dir_cls_preds);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }

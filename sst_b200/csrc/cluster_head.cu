@@ -4,7 +4,7 @@
 // rot columns, forward and backward.  fp32, stream-ordered, no host sync.
 //
 // Targets: one thread per cluster, one grid row per sample; a block row stages its sample's GTs in shared memory CH_CHUNK at a time and
-// only the clusters whose batch index is that sample test them, with box3d.cuh's make_box / to_local / in_box (the test of
+// only the clusters whose batch index is that sample test them, with in_box.cuh's make_box / to_local / in_box (the test of
 // points_in_boxes_gpu, so a hit is bit-identical to the reference's).  modify_gt_for_single_task orders a task's GTs class by class in
 // the task's class order and by input index within a class, and points_in_boxes_gpu takes the first box of that list: so a cluster
 // takes, per task, the hit with the smallest (class rank, GT index).  Every GT is tested once for all tasks.
@@ -14,11 +14,12 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
-#include "box3d.cuh"
+#include "heads.cuh"
+#include "in_box.cuh"
 
 namespace {
 
-#define CH_THREADS 256
+#define CH_THREADS 256       // targets block
 #define CH_CHUNK 256         // GTs staged in shared memory per step
 #define CH_MAX_BATCH 256
 #define CH_MAX_GT 4096       // GTs per sample
@@ -134,30 +135,7 @@ struct ChLossArgs {
   const int64_t* num_pos;    // [T] device, the local positives
 };
 
-// stable form: softplus(+-x) = max(+-x, 0) + log1p(exp(-|x|)); s = sigmoid(x) and q = 1 - s from the same exp(-|x|)
-__device__ __forceinline__ void ch_sig(float x, float& s, float& q, float& sp_pos, float& sp_neg) {
-  const float e = expf(-fabsf(x)), inv = 1.f / (1.f + e), l1p = log1pf(e);
-  s = x >= 0.f ? inv : e * inv;
-  q = x >= 0.f ? e * inv : inv;
-  sp_pos = fmaxf(x, 0.f) + l1p;
-  sp_neg = fmaxf(-x, 0.f) + l1p;
-}
-
-// mmdet 2.14 sigmoid focal element: t = 1: alpha q^gamma softplus(-x); t = 0: (1 - alpha) s^gamma softplus(x)
-__device__ __forceinline__ float ch_focal(const ChLossArgs& a, float x, bool t) {
-  float s, q, pp, pn;
-  ch_sig(x, s, q, pp, pn);
-  return t ? a.alpha * powf(q, a.gamma) * pn : (1.f - a.alpha) * powf(s, a.gamma) * pp;
-}
-
-// d/dx: t = 1: -alpha q^gamma (gamma s softplus(-x) + q); t = 0: (1 - alpha) s^gamma (gamma q softplus(x) + s)
-__device__ __forceinline__ float ch_focal_grad(const ChLossArgs& a, float x, bool t) {
-  float s, q, pp, pn;
-  ch_sig(x, s, q, pp, pn);
-  return t ? -a.alpha * powf(q, a.gamma) * (a.gamma * s * pn + q) : (1.f - a.alpha) * powf(s, a.gamma) * (a.gamma * q * pp + s);
-}
-
-// mmdet 2.14 l1_loss / smooth_l1_loss element of d = pred - target, and its derivative (torch.abs' gradient: sign, 0 at 0 and NaN)
+// mmdet 2.14 l1_loss / smooth_l1_loss element of d = pred - target, and its derivative
 __device__ __forceinline__ float ch_reg(const ChLossArgs& a, float d) {
   const float ad = fabsf(d);
   if (!a.smooth) return ad;
@@ -165,29 +143,17 @@ __device__ __forceinline__ float ch_reg(const ChLossArgs& a, float d) {
 }
 
 __device__ __forceinline__ float ch_reg_grad(const ChLossArgs& a, float d) {
-  const float sg = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);
+  const float sg = abs_grad(d);
   if (!a.smooth) return sg;
   const float ad = fabsf(d);
   return ad < a.beta ? ad / a.beta * sg : sg;
 }
 
-__device__ __forceinline__ double ch_block_sum(double v, double* sh) {
-#pragma unroll
-  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += sh[w];
-  __syncthreads();
-  return s;  // valid in thread 0
-}
-
 // column groups of the reg code: center [0, 3), size [3, 6), rot [6, 8)
 __device__ __forceinline__ int ch_group(int k) { return k < 3 ? 1 : (k < 6 ? 2 : 3); }
 
-__global__ void __launch_bounds__(CH_THREADS) ch_loss_forward_kernel(const __grid_constant__ ChLossArgs a, double* part, int nb) {
-  __shared__ double sh[CH_THREADS / 32];
+__global__ void __launch_bounds__(LOSS_THREADS) ch_loss_forward_kernel(const __grid_constant__ ChLossArgs a, double* part, int nb) {
+  __shared__ double sh[LOSS_THREADS / 32];
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (int t = 0; t < a.T; t++) {
     double acc[4] = {0.0, 0.0, 0.0, 0.0};
@@ -195,7 +161,7 @@ __global__ void __launch_bounds__(CH_THREADS) ch_loss_forward_kernel(const __gri
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < a.M; i += stride) {
       const float* xr = a.x[t] + i * a.xs[t];
       const int64_t y = __ldg(a.labels[t] + i);
-      for (int c = 0; c < C; c++) acc[0] += (double)ch_focal(a, __ldg(xr + c), y == c);
+      for (int c = 0; c < C; c++) acc[0] += (double)sigmoid_focal(__ldg(xr + c), y == c, a.alpha, a.gamma);
       if (!(y >= 0 && y <= C)) acc[0] += (double)NAN;  // an out-of-range batch index (label -1)
       if (y >= 0 && y < C) {
         const float* rr = a.r[t] + i * a.rs[t];
@@ -204,20 +170,18 @@ __global__ void __launch_bounds__(CH_THREADS) ch_loss_forward_kernel(const __gri
       }
     }
     for (int q = 0; q < 4; q++) {
-      const double s = ch_block_sum(acc[q], sh);
+      const double s = thread0_block_sum(acc[q], sh);
       if (threadIdx.x == 0) part[(size_t)(t * 4 + q) * nb + blockIdx.x] = s;
     }
   }
 }
 
 // fixed-order sums of the partials -> losses [T, 4]
-__global__ void __launch_bounds__(CH_THREADS) ch_loss_final_kernel(const __grid_constant__ ChLossArgs a, const double* part, int nb,
-                                                                   float* losses) {
-  __shared__ double sh[CH_THREADS / 32];
+__global__ void __launch_bounds__(LOSS_THREADS) ch_loss_final_kernel(const __grid_constant__ ChLossArgs a, const double* part, int nb,
+                                                                     float* losses) {
+  __shared__ double sh[LOSS_THREADS / 32];
   for (int k = 0; k < 4 * a.T; k++) {
-    double acc = 0.0;
-    for (int i = threadIdx.x; i < nb; i += blockDim.x) acc += part[(size_t)k * nb + i];
-    const double s = ch_block_sum(acc, sh);
+    const double s = sum_partials(part, nb, k, sh);
     if (threadIdx.x == 0) {
       const int t = k / 4, q = k % 4;
       if (q == 0)
@@ -233,8 +197,8 @@ struct ChGradPtrs {
   float* gr[CH_MAX_TASKS];  // [M, 8] contiguous
 };
 
-__global__ void __launch_bounds__(CH_THREADS) ch_loss_backward_kernel(const __grid_constant__ ChLossArgs a, const float* grad_losses,
-                                                                      const __grid_constant__ ChGradPtrs p) {
+__global__ void __launch_bounds__(LOSS_THREADS) ch_loss_backward_kernel(const __grid_constant__ ChLossArgs a, const float* grad_losses,
+                                                                        const __grid_constant__ ChGradPtrs p) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (int t = 0; t < a.T; t++) {
     const int C = a.C[t];
@@ -248,7 +212,7 @@ __global__ void __launch_bounds__(CH_THREADS) ch_loss_backward_kernel(const __gr
       const float* xr = a.x[t] + i * a.xs[t];
       const int64_t y = __ldg(a.labels[t] + i);
       const bool ok = y >= 0 && y <= C;
-      for (int c = 0; c < C; c++) gxt[i * C + c] = ok ? gc * ch_focal_grad(a, __ldg(xr + c), y == c) : NAN;
+      for (int c = 0; c < C; c++) gxt[i * C + c] = ok ? gc * sigmoid_focal_grad(__ldg(xr + c), y == c, a.alpha, a.gamma) : NAN;
       float* g = grt + i * CH_CODE;
       if (y >= 0 && y < C) {
         const float* rr = a.r[t] + i * a.rs[t];
@@ -259,11 +223,6 @@ __global__ void __launch_bounds__(CH_THREADS) ch_loss_backward_kernel(const __gr
       }
     }
   }
-}
-
-int ch_grid(sstb200_ctx* c, long long n) {
-  const long long want = (n + CH_THREADS * 8 - 1) / (CH_THREADS * 8);
-  return (int)std::max(1LL, std::min(want, (long long)c->num_sms * 8));
 }
 
 int ch_loss_args(sstb200_ctx* c, const sstb200_cluster_head_loss_cfg* cfg, int num_tasks, int64_t num_clusters, const float* const* cls_logits,
@@ -304,13 +263,8 @@ extern "C" int sstb200_cluster_head_targets(sstb200_ctx* c, const float* cluster
   if (num_tasks > CH_MAX_TASKS || num_classes > CH_MAX_CLASSES)
     return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "cluster_head_targets: %d tasks / %d classes, at most %d / %d", num_tasks, num_classes,
                      CH_MAX_TASKS, CH_MAX_CLASSES);
-  CHECK_ARG(c, gt_offsets[0] == 0);
-  for (int b = 0; b < batch; b++) {
-    CHECK_ARG(c, gt_offsets[b + 1] >= gt_offsets[b]);
-    if (gt_offsets[b + 1] - gt_offsets[b] > CH_MAX_GT)
-      return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "cluster_head_targets: sample %d has %d GT boxes, at most %d", b,
-                       gt_offsets[b + 1] - gt_offsets[b], CH_MAX_GT);
-  }
+  const int rc = check_offsets(c, "cluster_head_targets", gt_offsets, batch, CH_MAX_GT);
+  if (rc) return rc;
   ChTargetArgs a;
   for (int t = 0; t < num_tasks; t++) {
     CHECK_ARG(c, task_classes[t] >= 1 && task_classes[t] <= CH_MAX_CLASSES);
@@ -348,14 +302,14 @@ extern "C" int sstb200_cluster_head_loss_forward(sstb200_ctx* c, const sstb200_c
                         bbox_targets, num_pos, cls_avg_factor, reg_avg_factor, a);
   if (rc) return rc;
   CHECK_ARG(c, losses);
-  const int nb = ch_grid(c, a.M);
+  const int nb = loss_grid(c, a.M);
   arena_reset(c);
   double* part;
   rc = arena_carve(c, [&](Carve& cv) { part = cv.take<double>((size_t)4 * num_tasks * nb); });
   if (rc) return rc;
-  ch_loss_forward_kernel<<<nb, CH_THREADS, 0, c->stream>>>(a, part, nb);
+  ch_loss_forward_kernel<<<nb, LOSS_THREADS, 0, c->stream>>>(a, part, nb);
   LAUNCH_CHECK(c);
-  ch_loss_final_kernel<<<1, CH_THREADS, 0, c->stream>>>(a, part, nb, losses);
+  ch_loss_final_kernel<<<1, LOSS_THREADS, 0, c->stream>>>(a, part, nb, losses);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }
@@ -376,7 +330,7 @@ extern "C" int sstb200_cluster_head_loss_backward(sstb200_ctx* c, const sstb200_
     CHECK_ARG(c, grad_logits[t] && grad_reg_preds[t]);
     p.gx[t] = grad_logits[t], p.gr[t] = grad_reg_preds[t];
   }
-  ch_loss_backward_kernel<<<ch_grid(c, a.M), CH_THREADS, 0, c->stream>>>(a, grad_losses, p);
+  ch_loss_backward_kernel<<<loss_grid(c, a.M), LOSS_THREADS, 0, c->stream>>>(a, grad_losses, p);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }

@@ -3,7 +3,7 @@
 // training-log counts, forward and backward.  fp32, stream-ordered, no host sync.
 //
 // Targets: one thread per point, one grid row per sample.  The sample's GTs are staged in shared memory VS_CHUNK at a time and tested
-// with box3d.cuh's make_box / to_local / in_box, the test sstb200_points_in_boxes uses, so the hit is bit-identical to the reference's
+// with in_box.cuh's make_box / to_local / in_box, the test sstb200_points_in_boxes uses, so the hit is bit-identical to the reference's
 // points_in_boxes_gpu (first hit wins); a point stops scanning at its first hit.  GTs with a negative label are skipped, which is the
 // reference's valid_gt_mask filter followed by points_in_boxes on the survivors.
 //
@@ -13,11 +13,12 @@
 #include <stdarg.h>
 #include <algorithm>
 #include <cmath>
-#include "box3d.cuh"
+#include "heads.cuh"
+#include "in_box.cuh"
 
 namespace {
 
-#define VS_THREADS 256
+#define VS_THREADS 256      // targets block
 #define VS_CHUNK 256         // GTs staged in shared memory per step
 #define VS_MAX_BATCH 256
 #define VS_MAX_GT 4096       // GTs per sample
@@ -112,34 +113,6 @@ struct VsLossArgs {
   int eg[VS_MAX_ENTRIES], ec[VS_MAX_ENTRIES];
 };
 
-// stable form: softplus(+-x) = max(+-x, 0) + log1p(exp(-|x|)), s = sigmoid(x), q = 1 - s = sigmoid(-x) from the same exp(-|x|)
-struct Sig {
-  float s, q, sp_pos, sp_neg;
-};
-
-__device__ __forceinline__ Sig sig(float x) {
-  const float e = expf(-fabsf(x)), inv = 1.f / (1.f + e), l1p = log1pf(e);
-  Sig r;
-  r.s = x >= 0.f ? inv : e * inv;
-  r.q = x >= 0.f ? e * inv : inv;
-  r.sp_pos = fmaxf(x, 0.f) + l1p;
-  r.sp_neg = fmaxf(-x, 0.f) + l1p;
-  return r;
-}
-
-// mmdet 2.14 py_sigmoid_focal_loss element: t = 1: alpha q^gamma softplus(-x); t = 0: (1 - alpha) s^gamma softplus(x)
-__device__ __forceinline__ float focal_loss(const VsLossArgs& a, float x, bool t) {
-  const Sig g = sig(x);
-  return t ? a.alpha * powf(g.q, a.gamma) * g.sp_neg : (1.f - a.alpha) * powf(g.s, a.gamma) * g.sp_pos;
-}
-
-// d/dx: t = 1: -alpha q^gamma (gamma s softplus(-x) + q); t = 0: (1 - alpha) s^gamma (gamma q softplus(x) + s)
-__device__ __forceinline__ float focal_grad(const VsLossArgs& a, float x, bool t) {
-  const Sig g = sig(x);
-  return t ? -a.alpha * powf(g.q, a.gamma) * (a.gamma * g.s * g.sp_neg + g.q)
-           : (1.f - a.alpha) * powf(g.s, a.gamma) * (a.gamma * g.q * g.sp_pos + g.s);
-}
-
 __device__ __forceinline__ float logit(const VsLossArgs& a, const float* xr, int c) { return __fmul_rn(__ldg(xr + c), a.scale); }
 
 // softmax statistics of a row: max and sum of exp(x - max); NaN anywhere in the row makes both NaN
@@ -158,23 +131,12 @@ __device__ __forceinline__ void row_softmax(const VsLossArgs& a, const float* xr
 
 __device__ __forceinline__ bool label_ok(const VsLossArgs& a, int64_t y) { return y >= 0 && y < (a.softmax ? a.C : a.C + 1); }
 
-__device__ __forceinline__ double vs_block_sum(double v, double* sh) {
-#pragma unroll
-  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += sh[w];
-  __syncthreads();
-  return s;  // valid in thread 0
-}
-
 // integer partials per block: n_valid, num_fg, then tp[E], real[E]
 #define VS_NINT(E) (2 + 2 * (E))
 
-__global__ void __launch_bounds__(VS_THREADS) vs_loss_forward_kernel(const __grid_constant__ VsLossArgs a, double* part, int* ipart, int nb) {
-  __shared__ double sh[VS_THREADS / 32];
+__global__ void __launch_bounds__(LOSS_THREADS) vs_loss_forward_kernel(const __grid_constant__ VsLossArgs a, double* part, int* ipart,
+                                                                        int nb) {
+  __shared__ double sh[LOSS_THREADS / 32];
   __shared__ int scnt[VS_NINT(VS_MAX_ENTRIES)];
   const int K = VS_NINT(a.E);
   for (int k = threadIdx.x; k < K; k += blockDim.x) scnt[k] = 0;
@@ -190,7 +152,7 @@ __global__ void __launch_bounds__(VS_THREADS) vs_loss_forward_kernel(const __gri
     float m = 0.f, se = 1.f;
     // segmentation loss (lines 116-118)
     if (!a.softmax) {
-      for (int c = 0; c < a.C; c++) seg += (double)focal_loss(a, logit(a, xr, c), y == c);
+      for (int c = 0; c < a.C; c++) seg += (double)sigmoid_focal(logit(a, xr, c), y == c, a.alpha, a.gamma);
     } else {
       row_softmax(a, xr, m, se);
       if (ok) seg += (double)(a.cw[y] * (m + logf(se) - logit(a, xr, (int)y)));
@@ -224,8 +186,8 @@ __global__ void __launch_bounds__(VS_THREADS) vs_loss_forward_kernel(const __gri
     for (int e = 0; e < a.E; e++)
       if (y == a.ec[e]) atomicAdd(scnt + 2 + a.E + e, 1);
   }
-  seg = vs_block_sum(seg, sh);
-  vote = vs_block_sum(vote, sh);
+  seg = thread0_block_sum(seg, sh);
+  vote = thread0_block_sum(vote, sh);
 #pragma unroll
   for (int o = 16; o; o >>= 1) {
     nvalid += __shfl_xor_sync(0xffffffffu, nvalid, o);
@@ -241,16 +203,12 @@ __global__ void __launch_bounds__(VS_THREADS) vs_loss_forward_kernel(const __gri
 }
 
 // fixed-order sums of the partials -> losses[0..1], the device n_valid and the counts (tp[E], real[E], num_fg)
-__global__ void __launch_bounds__(VS_THREADS) vs_loss_final_kernel(const double* part, const int* ipart, int nb, int E, long long n, int C,
-                                                                   int softmax, float w_seg, float w_vote, float* losses,
-                                                                   int64_t* num_valid, int64_t* counts) {
-  __shared__ double sh[VS_THREADS / 32];
+__global__ void __launch_bounds__(LOSS_THREADS) vs_loss_final_kernel(const double* part, const int* ipart, int nb, int E, long long n,
+                                                                     int C, int softmax, float w_seg, float w_vote, float* losses,
+                                                                     int64_t* num_valid, int64_t* counts) {
+  __shared__ double sh[LOSS_THREADS / 32];
   double s[2];
-  for (int k = 0; k < 2; k++) {
-    double acc = 0.0;
-    for (int i = threadIdx.x; i < nb; i += blockDim.x) acc += part[(size_t)k * nb + i];
-    s[k] = vs_block_sum(acc, sh);
-  }
+  for (int k = 0; k < 2; k++) s[k] = sum_partials(part, nb, k, sh);
   // the integer partials: one warp per count, its lanes striding over the blocks (integer sums do not depend on the order)
   __shared__ long long v[VS_NINT(VS_MAX_ENTRIES)];
   const int lane = threadIdx.x & 31;
@@ -274,8 +232,8 @@ __global__ void __launch_bounds__(VS_THREADS) vs_loss_final_kernel(const double*
 
 // The no-valid-point case of the vote loss: vote_preds.sum() * 0 is NaN when any vote prediction is not finite.  Every block returns at
 // once unless the device n_valid is 0, so the whole [N, 3 C] vote tensor is read only in that case.
-__global__ void __launch_bounds__(VS_THREADS) vs_vote_nonfinite_kernel(const __grid_constant__ VsLossArgs a, const int64_t* num_valid,
-                                                                       float* losses) {
+__global__ void __launch_bounds__(LOSS_THREADS) vs_vote_nonfinite_kernel(const __grid_constant__ VsLossArgs a,
+                                                                         const int64_t* num_valid, float* losses) {
   if (*num_valid > 0) return;
   const int W = 3 * a.C;
   bool bad = false;
@@ -287,9 +245,9 @@ __global__ void __launch_bounds__(VS_THREADS) vs_vote_nonfinite_kernel(const __g
   if (bad) losses[1] = NAN;  // every writer stores the same value
 }
 
-__global__ void __launch_bounds__(VS_THREADS) vs_loss_backward_kernel(const __grid_constant__ VsLossArgs a, float w_seg, float w_vote,
-                                                                      const int64_t* num_valid, const float* grad_losses, float* gx,
-                                                                      float* gv) {
+__global__ void __launch_bounds__(LOSS_THREADS) vs_loss_backward_kernel(const __grid_constant__ VsLossArgs a, float w_seg,
+                                                                        float w_vote, const int64_t* num_valid, const float* grad_losses,
+                                                                        float* gx, float* gv) {
   const float gs = (float)((double)grad_losses[0] * w_seg * a.scale / (double)(a.softmax ? a.n : a.n * a.C));
   const long long nv = *num_valid;
   const float gvs = nv > 0 ? (float)((double)grad_losses[1] * w_vote / (double)(3 * nv)) : 0.f;
@@ -302,7 +260,7 @@ __global__ void __launch_bounds__(VS_THREADS) vs_loss_backward_kernel(const __gr
     const int64_t y = __ldg(a.labels + i);
     const bool ok = label_ok(a, y);
     if (!a.softmax) {
-      for (int c = 0; c < a.C; c++) gxr[c] = ok ? gs * focal_grad(a, logit(a, xr, c), y == c) : NAN;
+      for (int c = 0; c < a.C; c++) gxr[c] = ok ? gs * sigmoid_focal_grad(logit(a, xr, c), y == c, a.alpha, a.gamma) : NAN;
     } else {
       float m, se;
       row_softmax(a, xr, m, se);
@@ -315,15 +273,10 @@ __global__ void __launch_bounds__(VS_THREADS) vs_loss_backward_kernel(const __gr
       const float* t = a.vt + i * 3;
       for (int k = 0; k < 3; k++) {
         const float d = __ldg(vr + 3 * y + k) - __ldg(t + k);
-        gvr[3 * y + k] = gvs * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f));  // torch's abs gradient: sign, 0 at 0 and NaN
+        gvr[3 * y + k] = gvs * abs_grad(d);
       }
     }
   }
-}
-
-int vs_grid(sstb200_ctx* c, long long n) {
-  const long long want = (n + VS_THREADS * 8 - 1) / (VS_THREADS * 8);
-  return (int)std::max(1LL, std::min(want, (long long)c->num_sms * 8));
 }
 
 int vs_loss_args(sstb200_ctx* c, const sstb200_voteseg_cfg* cfg, const float* seg_logits, int64_t logit_stride, const float* vote_preds,
@@ -364,15 +317,11 @@ extern "C" int sstb200_voteseg_targets(sstb200_ctx* c, const float* points, int6
                                        int64_t* labels, float* vote_targets, uint8_t* vote_mask) {
   CHECK_ARG(c, point_offsets && gt_offsets && batch >= 1 && point_stride >= 3);
   if (batch > VS_MAX_BATCH) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "voteseg_targets: %d samples, at most %d", batch, VS_MAX_BATCH);
-  CHECK_ARG(c, point_offsets[0] == 0 && gt_offsets[0] == 0);
+  int rc = check_offsets(c, "voteseg_targets", point_offsets, batch, INT_MAX);
+  if (!rc) rc = check_offsets(c, "voteseg_targets", gt_offsets, batch, VS_MAX_GT);
+  if (rc) return rc;
   int max_pts = 0;
-  for (int b = 0; b < batch; b++) {
-    CHECK_ARG(c, point_offsets[b + 1] >= point_offsets[b] && gt_offsets[b + 1] >= gt_offsets[b]);
-    max_pts = std::max(max_pts, point_offsets[b + 1] - point_offsets[b]);
-    if (gt_offsets[b + 1] - gt_offsets[b] > VS_MAX_GT)
-      return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "voteseg_targets: sample %d has %d GT boxes, at most %d", b, gt_offsets[b + 1] - gt_offsets[b],
-                       VS_MAX_GT);
-  }
+  for (int b = 0; b < batch; b++) max_pts = std::max(max_pts, point_offsets[b + 1] - point_offsets[b]);
   const int N = point_offsets[batch], G = gt_offsets[batch];
   CHECK_ARG(c, N == 0 || (points && labels && vote_targets && vote_mask));
   CHECK_ARG(c, G == 0 || (gt_boxes && gt_labels));
@@ -395,7 +344,7 @@ extern "C" int sstb200_voteseg_loss_forward(sstb200_ctx* c, const sstb200_votese
   int rc = vs_loss_args(c, cfg, seg_logits, logit_stride, vote_preds, vote_stride, num_points, labels, vote_targets, vote_mask, a);
   if (rc) return rc;
   CHECK_ARG(c, losses && num_valid && counts);
-  const int nb = vs_grid(c, a.n);
+  const int nb = loss_grid(c, a.n);
   arena_reset(c);
   double* part;
   int* ipart;
@@ -404,12 +353,12 @@ extern "C" int sstb200_voteseg_loss_forward(sstb200_ctx* c, const sstb200_votese
     ipart = cv.take<int>((size_t)VS_NINT(a.E) * nb);
   });
   if (rc) return rc;
-  vs_loss_forward_kernel<<<nb, VS_THREADS, 0, c->stream>>>(a, part, ipart, nb);
+  vs_loss_forward_kernel<<<nb, LOSS_THREADS, 0, c->stream>>>(a, part, ipart, nb);
   LAUNCH_CHECK(c);
-  vs_loss_final_kernel<<<1, VS_THREADS, 0, c->stream>>>(part, ipart, nb, a.E, a.n, a.C, a.softmax, cfg->loss_weight, cfg->loss_weight_vote,
-                                                        losses, num_valid, counts);
+  vs_loss_final_kernel<<<1, LOSS_THREADS, 0, c->stream>>>(part, ipart, nb, a.E, a.n, a.C, a.softmax, cfg->loss_weight,
+                                                          cfg->loss_weight_vote, losses, num_valid, counts);
   LAUNCH_CHECK(c);
-  vs_vote_nonfinite_kernel<<<vs_grid(c, a.n * 3 * a.C), VS_THREADS, 0, c->stream>>>(a, num_valid, losses);
+  vs_vote_nonfinite_kernel<<<loss_grid(c, a.n * 3 * a.C), LOSS_THREADS, 0, c->stream>>>(a, num_valid, losses);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }
@@ -422,8 +371,8 @@ extern "C" int sstb200_voteseg_loss_backward(sstb200_ctx* c, const sstb200_votes
   int rc = vs_loss_args(c, cfg, seg_logits, logit_stride, vote_preds, vote_stride, num_points, labels, vote_targets, vote_mask, a);
   if (rc) return rc;
   CHECK_ARG(c, num_valid && grad_losses && grad_logits && grad_vote_preds);
-  vs_loss_backward_kernel<<<vs_grid(c, a.n), VS_THREADS, 0, c->stream>>>(a, cfg->loss_weight, cfg->loss_weight_vote, num_valid, grad_losses,
-                                                                         grad_logits, grad_vote_preds);
+  vs_loss_backward_kernel<<<loss_grid(c, a.n), LOSS_THREADS, 0, c->stream>>>(a, cfg->loss_weight, cfg->loss_weight_vote, num_valid,
+                                                                             grad_losses, grad_logits, grad_vote_preds);
   LAUNCH_CHECK(c);
   return SSTB_OK;
 }

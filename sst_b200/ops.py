@@ -1126,6 +1126,31 @@ def _fp32_cuda(name, t, dim=None):
     return t.contiguous()
 
 
+def _offsets(sizes):
+    out = [0]
+    for n in sizes:
+        out.append(out[-1] + int(n))
+    return out
+
+
+def _sample_offsets(fn, sample_sizes, n):
+    sizes = [int(v) for v in sample_sizes]
+    if sum(sizes) != n or min(sizes, default=-1) < 0:
+        raise L.SSTB200Error(f"{fn}: sample sizes {sizes} do not add up to the {n} boxes")
+    return _offsets(sizes)
+
+
+def _cat_gt(fn, gt_boxes, gt_labels, dev):
+    """per-sample boxes (columns 0-6 of tensors or of their `.tensor`) and labels -> fp32 [G, 7], int64 [G] on dev, B + 1 offsets"""
+    boxes = [getattr(b, "tensor", b) for b in gt_boxes]
+    for b, lab in zip(boxes, gt_labels):
+        if b.dim() != 2 or b.shape[1] < 7 or lab.shape != (b.shape[0],):
+            raise L.SSTB200Error(f"{fn}: boxes {tuple(b.shape)} and labels {tuple(lab.shape)} do not match")
+    gt = torch.cat([b[:, :7] for b in boxes]).to(dev, torch.float32).contiguous()
+    gl = torch.cat([lab.reshape(-1) for lab in gt_labels]).to(dev, torch.int64).contiguous()
+    return gt, gl, _offsets([b.shape[0] for b in boxes])
+
+
 def centerpoint_targets(boxes, labels, sample_sizes, task_num_classes, pc_min, voxel_size, out_size_factor, feature_map_size,
                         gaussian_overlap, min_radius, max_objs, norm_bbox=True):
     """CenterHead.get_targets for the whole batch: boxes [N, 7|9] fp32 gravity-centred, labels int64 [N], the samples' boxes
@@ -1141,17 +1166,11 @@ def centerpoint_targets(boxes, labels, sample_sizes, task_num_classes, pc_min, v
         raise L.SSTB200Error(f"centerpoint_targets: boxes must be [N, 7] or [N, 9], got {tuple(boxes.shape)}")
     if labels.dim() != 1 or labels.shape[0] != boxes.shape[0]:
         raise L.SSTB200Error(f"centerpoint_targets: labels {tuple(labels.shape)} do not match boxes {tuple(boxes.shape)}")
-    sizes = [int(n) for n in sample_sizes]
-    if sum(sizes) != boxes.shape[0] or min(sizes, default=-1) < 0:
-        raise L.SSTB200Error(f"centerpoint_targets: sample sizes {sizes} do not add up to the {boxes.shape[0]} boxes")
+    offsets = _sample_offsets("centerpoint_targets", sample_sizes, boxes.shape[0])
     W, H = (int(v) for v in feature_map_size)
-    B, dev = len(sizes), boxes.device
+    B, dev = len(offsets) - 1, boxes.device
     boxes, labels = boxes.contiguous(), labels.long().contiguous()
-    offsets, task_off = [0], [0]
-    for n in sizes:
-        offsets.append(offsets[-1] + n)
-    for n in task_num_classes:
-        task_off.append(task_off[-1] + int(n))
+    task_off = _offsets(task_num_classes)
     hm = [torch.empty((B, int(n), H, W), dtype=torch.float32, device=dev) for n in task_num_classes]
     ab = [torch.empty((B, max_objs, 10), dtype=torch.float32, device=dev) for _ in task_num_classes]
     ind = [torch.empty((B, max_objs), dtype=torch.int64, device=dev) for _ in task_num_classes]
@@ -1295,9 +1314,7 @@ def anchor3d_targets(x_centers, y_centers, size_z, size_wlh, rotations, gt_boxes
         raise L.SSTB200Error(f"anchor3d_targets: gt_boxes must be float32 [N, 7], got {gt_boxes.dtype} {tuple(gt_boxes.shape)}")
     if gt_labels.dim() != 1 or gt_labels.shape[0] != gt_boxes.shape[0]:
         raise L.SSTB200Error(f"anchor3d_targets: gt_labels {tuple(gt_labels.shape)} do not match gt_boxes {tuple(gt_boxes.shape)}")
-    sizes = [int(n) for n in sample_sizes]
-    if sum(sizes) != gt_boxes.shape[0] or min(sizes, default=-1) < 0:
-        raise L.SSTB200Error(f"anchor3d_targets: sample sizes {sizes} do not add up to the {gt_boxes.shape[0]} boxes")
+    offsets = _sample_offsets("anchor3d_targets", sample_sizes, gt_boxes.shape[0])
 
     def per_size(name, v, ctype):
         vals = list(v) if isinstance(v, (list, tuple)) else [v] * S
@@ -1305,11 +1322,8 @@ def anchor3d_targets(x_centers, y_centers, size_z, size_wlh, rotations, gt_boxes
             raise L.SSTB200Error(f"anchor3d_targets: {name} needs {S} values, got {len(vals)}")
         return L.arr(ctype, [ctype(x).value if ctype is C.c_float else int(bool(x)) for x in vals])
 
-    B, A, dev = len(sizes), H * W * S * R, xc.device
+    B, A, dev = len(offsets) - 1, H * W * S * R, xc.device
     gt, gl = gt_boxes.contiguous(), gt_labels.long().contiguous()
-    offsets = [0]
-    for n in sizes:
-        offsets.append(offsets[-1] + n)
     labels = torch.empty((B, A), dtype=torch.int64, device=dev)
     label_weights = torch.empty((B, A), dtype=torch.float32, device=dev)
     bbox_targets = torch.empty((B, A, 7), dtype=torch.float32, device=dev)
@@ -1462,13 +1476,6 @@ L.SIGNATURES["sstb200_voteseg_loss_forward"] = (C.c_int, _VS_ARGS + [L.vp, L.vp,
 L.SIGNATURES["sstb200_voteseg_loss_backward"] = (C.c_int, _VS_ARGS + [L.vp, L.vp, L.vp, L.vp])
 
 
-def _offsets(sizes):
-    out = [0]
-    for n in sizes:
-        out.append(out[-1] + int(n))
-    return out
-
-
 def voteseg_targets(points_list_or_cat, offsets, gt_boxes, gt_labels, num_classes):
     """VoteSegHead.get_targets for the whole batch in one launch.  points_list_or_cat: a list of [n_b, >= 3] fp32 CUDA tensors (offsets
     None), or their concatenation [N, >= 3] with offsets = the B + 1 host sample offsets (ints or a CPU tensor; read in place, any row
@@ -1500,12 +1507,7 @@ def voteseg_targets(points_list_or_cat, offsets, gt_boxes, gt_labels, num_classe
     if len(gt_boxes) != B or len(gt_labels) != B:
         raise L.SSTB200Error(f"voteseg_targets: {len(gt_boxes)} box and {len(gt_labels)} label lists for {B} samples")
     dev = pts.device
-    boxes = [getattr(b, "tensor", b) for b in gt_boxes]
-    for b, lab in zip(boxes, gt_labels):
-        if b.dim() != 2 or b.shape[1] < 7 or lab.shape != (b.shape[0],):
-            raise L.SSTB200Error(f"voteseg_targets: boxes {tuple(b.shape)} and labels {tuple(lab.shape)} do not match")
-    gt = torch.cat([b[:, :7] for b in boxes]).to(dev, torch.float32).contiguous()
-    gl = torch.cat([lab.reshape(-1) for lab in gt_labels]).to(dev, torch.int64).contiguous()
+    gt, gl, gt_offs = _cat_gt("voteseg_targets", gt_boxes, gt_labels, dev)
     N = pts.shape[0]
     labels = torch.empty((N,), dtype=torch.int64, device=dev)
     vote_targets = torch.empty((N, 3), dtype=torch.float32, device=dev)
@@ -1513,7 +1515,7 @@ def voteseg_targets(points_list_or_cat, offsets, gt_boxes, gt_labels, num_classe
     c = L.ctx(dev)
     L.check(c, L.lib().sstb200_voteseg_targets(c, L.ptr(pts) if N else None, pts.stride(0), L.arr(C.c_int32, offs),
                                                L.ptr(gt) if gt.numel() else None, L.ptr(gl) if gl.numel() else None,
-                                               L.arr(C.c_int32, _offsets([b.shape[0] for b in boxes])), B, int(num_classes),
+                                               L.arr(C.c_int32, gt_offs), B, int(num_classes),
                                                L.ptr(labels) if N else None, L.ptr(vote_targets) if N else None,
                                                L.ptr(vote_mask) if N else None))
     return labels, vote_targets, vote_mask
@@ -1704,19 +1706,14 @@ def cluster_head_targets(cluster_xyz, cluster_inds, gt_boxes, gt_labels, tasks, 
             class_task[k], class_rank[k] = t, r
     T = len(tasks)
     dev = xyz.device
-    boxes = [getattr(b, "tensor", b) for b in gt_boxes]
-    for b, lab in zip(boxes, gt_labels):
-        if b.dim() != 2 or b.shape[1] < 7 or lab.shape != (b.shape[0],):
-            raise L.SSTB200Error(f"cluster_head_targets: boxes {tuple(b.shape)} and labels {tuple(lab.shape)} do not match")
-    gt = torch.cat([b[:, :7] for b in boxes]).to(dev, torch.float32).contiguous()
-    gl = torch.cat([lab.reshape(-1) for lab in gt_labels]).to(dev, torch.int64).contiguous()
+    gt, gl, gt_offs = _cat_gt("cluster_head_targets", gt_boxes, gt_labels, dev)
     labels = [torch.empty((M,), dtype=torch.int64, device=dev) for _ in range(T)]
     targets = [torch.empty((M, CLUSTER_HEAD_CODE_SIZE), dtype=torch.float32, device=dev) for _ in range(T)]
     num_pos = torch.empty((T,), dtype=torch.int64, device=dev)
     c = L.ctx(dev)
     L.check(c, L.lib().sstb200_cluster_head_targets(
         c, L.ptr(xyz) if M else None, xyz.stride(0), L.ptr(bidx) if M else None, bstride, M, L.ptr(gt) if gt.numel() else None,
-        L.ptr(gl) if gl.numel() else None, L.arr(C.c_int32, _offsets([b.shape[0] for b in boxes])), B, len(names),
+        L.ptr(gl) if gl.numel() else None, L.arr(C.c_int32, gt_offs), B, len(names),
         L.arr(C.c_int32, class_task), L.arr(C.c_int32, class_rank), T, L.arr(C.c_int32, [len(t) for t in tasks]), _ptrs(labels),
         _ptrs(targets), L.ptr(num_pos)))
     return labels, targets, num_pos
