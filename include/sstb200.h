@@ -889,6 +889,54 @@ int sstb200_cluster_head_loss_backward(sstb200_ctx* ctx, const sstb200_cluster_h
                                        const float* reg_avg_factor, const float* grad_losses, float* const* grad_logits,
                                        float* const* grad_reg_preds);
 
+/* ---- FSDV2Head training (mmdet3d/models/dense_heads/fsd_v2_head.py): the cluster-head kernels above with centroid assignment and
+ * velocity.  The three functions above are these with assign_xyz NULL, gt_width 7 and code_size 8, and give the same results bit for bit.
+ *
+ * sstb200_cluster_head_targets_ex: sstb200_cluster_head_targets plus
+ *   - assign_xyz (NULL, or [M, >= 3] fp32 with row stride assign_stride): the points of the in-box test, train_cfg centroid_assign's
+ *     aux_xyz (lines 359-362); the encode still subtracts cluster_xyz (line 382).  NULL tests cluster_xyz.
+ *   - gt_width: the row width of gt_boxes, 7, 9 (with velocity, columns 7-8) or 10 (plus the copy-paste flag, column 9).
+ *   - code_size 8 or 10.  With 10, bbox_targets[t] is f32 [M, 11]: columns 0-7 as above, 8-9 = the hit's GT columns 7-8, and column 10 =
+ *     the velocity loss weight, GT column 9 for gt_width 10 (lines 383-388) and 1 for gt_width 9; all 11 are 0 on negatives and NaN for
+ *     an out-of-range batch index.  With 8, bbox_targets[t] is [M, 8].
+ *   Errors: those of sstb200_cluster_head_targets; code_size other than 8 / 10, code_size 10 with gt_width 7 (the reference's encode
+ *   has no velocity to copy), code_size 8 with gt_width 9 / 10 (its encode asserts code_size == 10), assign_stride < 3 (SSTB_ERR_ARG).
+ *
+ * sstb200_cluster_head_loss_forward_ex / _backward_ex: sstb200_cluster_head_loss_forward / _backward with cfg->code_size.  With 8 they
+ *   are those functions.  With 10, reg_preds[t] is [M, >= 10], bbox_targets[t] [M, 11] from sstb200_cluster_head_targets_ex, and losses
+ *   f32 [T, 5] = (cls, center, size, rot, vel) with
+ *   - vel: loss_weight_vel * sum over the positives of the L1 / SmoothL1 element (the type and beta of the other three) of columns
+ *     [8, 10) times the target's column 10, over 2 * num_pos[t], the local count: loss_vel is called without avg_factor (lines 243-248),
+ *     mmdet's reduction 'mean' over the [num_pos, 2] elements.  Exactly 0 when num_pos[t] is 0.
+ *   The backward takes grad_losses [T, 5] and writes grad_reg_preds[t] [M, 10], contiguous; columns 8-9 are 0 where the weight is 0.
+ *   Block partials in double summed in a fixed order as above; no atomics; deterministic.
+ *   Errors: those of the functions above, and code_size other than 8 / 10 or a reg row stride below code_size (SSTB_ERR_ARG). */
+typedef struct {
+  float gamma, alpha;                  /* focal loss */
+  int32_t smooth_l1;                   /* 0: L1Loss, 1: SmoothL1Loss(beta) for center, size, rot and vel */
+  float beta;
+  float loss_weight_cls, loss_weight_center, loss_weight_size, loss_weight_rot;
+  float loss_weight_vel;               /* code_size 10 only */
+  int32_t code_size;                   /* 8 or 10 */
+} sstb200_cluster_head_loss_cfg_ex;
+int sstb200_cluster_head_targets_ex(sstb200_ctx* ctx, const float* cluster_xyz, int64_t xyz_stride, const float* assign_xyz,
+                                    int64_t assign_stride, const int64_t* batch_idx, int64_t batch_stride, int64_t num_clusters,
+                                    const float* gt_boxes, int gt_width, const int64_t* gt_labels, const int32_t* gt_offsets, int batch,
+                                    int num_classes, const int32_t* class_task, const int32_t* class_rank, int num_tasks,
+                                    const int32_t* task_classes, int code_size, int64_t* const* labels, float* const* bbox_targets,
+                                    int64_t* num_pos);
+int sstb200_cluster_head_loss_forward_ex(sstb200_ctx* ctx, const sstb200_cluster_head_loss_cfg_ex* cfg, int num_tasks, int64_t num_clusters,
+                                         const float* const* cls_logits, const int64_t* logit_strides, const int32_t* task_classes,
+                                         const float* const* reg_preds, const int64_t* reg_strides, int64_t* const* labels,
+                                         float* const* bbox_targets, const int64_t* num_pos, const float* cls_avg_factor,
+                                         const float* reg_avg_factor, float* losses);
+int sstb200_cluster_head_loss_backward_ex(sstb200_ctx* ctx, const sstb200_cluster_head_loss_cfg_ex* cfg, int num_tasks,
+                                          int64_t num_clusters, const float* const* cls_logits, const int64_t* logit_strides,
+                                          const int32_t* task_classes, const float* const* reg_preds, const int64_t* reg_strides,
+                                          int64_t* const* labels, float* const* bbox_targets, const int64_t* num_pos,
+                                          const float* cls_avg_factor, const float* reg_avg_factor, const float* grad_losses,
+                                          float* const* grad_logits, float* const* grad_reg_preds);
+
 #ifdef __cplusplus
 }
 #endif

@@ -36,10 +36,15 @@ def voxelize_with_batch_idx(points, batch_idx, voxel_size, point_cloud_range):
 
 class VirtualVoxelFront(nn.Module):
     """Constructor kwargs = the corresponding kwargs of SingleStageFSDV2 (configs/fsdv2/*.py): `voxel_encoder` (a DynamicScatterVFE
-    config), `virtual_point_projector`, `multiscale_cfg`, `point_cloud_range`."""
+    config), `virtual_point_projector`, `multiscale_cfg`, `point_cloud_range`, `train_cfg`.  In training mode `finish` also returns
+    `virtual_centroid`, the mean of each virtual voxel's points (FSDV2Head's centroid_assign); train_cfg centroid_alpha, which no
+    config sets, raises ValueError."""
 
-    def __init__(self, voxel_encoder, virtual_point_projector, point_cloud_range=None, multiscale_cfg=None, as_rpn=False, backbone=None):
+    def __init__(self, voxel_encoder, virtual_point_projector, point_cloud_range=None, multiscale_cfg=None, as_rpn=False, backbone=None,
+                 train_cfg=None):
         super().__init__()
+        if train_cfg is not None and train_cfg.get("centroid_alpha", None) is not None:
+            raise ValueError(f"VirtualVoxelFront: train_cfg centroid_alpha is not supported, got {train_cfg.get('centroid_alpha')}")
         self.voxel_encoder = build_voxel_encoder(voxel_encoder)
         self.backbone = build_backbone(backbone) if backbone is not None else None   # VirtualVoxelMixer (spconv_modules.py)
         self.virtual_voxel_size = voxel_encoder["voxel_size"]
@@ -118,7 +123,8 @@ class VirtualVoxelFront(nn.Module):
                                              new_coors=voxel_coors)
         virtual_mask = voxel_indicators.squeeze(1) > 0
         out = dict(voxel_feats=voxel_feats, voxel_coors=voxel_coors, unq_inv=unq_inv, virtual_mask=virtual_mask, coors=coors,
-                   cat_pts=cat_pts, cat_batch_idx=cat_batch_idx, pts_indicators=pts_indicators, singlescale_mask=None)
+                   cat_pts=cat_pts, cat_batch_idx=cat_batch_idx, pts_indicators=pts_indicators, singlescale_mask=None,
+                   encoder_coors=voxel_coors)   # the voxels unq_inv indexes, before multiscale fusion and only_virtual
         if multiscale_features is not None:
             out["voxel_feats"], out["voxel_coors"], out["singlescale_mask"] = self.multiscale_fusion(multiscale_features, voxel_feats,
                                                                                                       voxel_coors)
@@ -150,6 +156,12 @@ class VirtualVoxelFront(nn.Module):
         else:
             vf, vc, ce = out_voxel_feats[virtual_mask], out_coors[virtual_mask], voxel_centers[virtual_mask]
         out = dict(virtual_feats=vf, virtual_coors=vc, virtual_centers=ce, sparse_shape=sparse_shape)
+        if self.training:
+            # single_stage_fsd_v2.py:246-261 without centroid_alpha: the mean of each voxel's points over the front's voxel index; the
+            # reference's `.all()` assert that it lies in its voxel is dropped (a host sync)
+            centroid, _ = ops.scatter_v2(front_out["cat_pts"][:, :3], front_out["coors"], mode="avg", return_inv=False,
+                                         unq_inv=front_out["unq_inv"], new_coors=front_out["encoder_coors"])
+            out["virtual_centroid"] = centroid[virtual_mask]
         if self.as_rpn:
             out["pts_feats"] = self.recover_point_features(out_voxel_feats, out_coors, front_out["cat_pts"], front_out["voxel_coors"]
                                                            if ssm is None else front_out["voxel_coors"][ssm], front_out["unq_inv"])

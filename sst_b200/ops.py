@@ -21,7 +21,8 @@ and error behaviour; no CPU path - CPU tensors raise.
                                       models/dense_heads/anchor3d_head.py, train_mixins.py (Anchor3DHead training)
     voteseg_targets, voteseg_loss     models/decode_heads/segmentation_head.py:107-283 (VoteSegHead training)
     cluster_head_targets, cluster_head_loss, multiclass_nms_groups
-                                      models/dense_heads/sparse_cluster_head_v2.py (SparseClusterHeadV2 training and proposals)
+                                      models/dense_heads/sparse_cluster_head_v2.py (SparseClusterHeadV2 training and proposals),
+                                      fsd_v2_head.py (FSDV2Head: centroid assignment, velocity)
 """
 import ctypes as C
 import math
@@ -1140,13 +1141,15 @@ def _sample_offsets(fn, sample_sizes, n):
     return _offsets(sizes)
 
 
-def _cat_gt(fn, gt_boxes, gt_labels, dev):
-    """per-sample boxes (columns 0-6 of tensors or of their `.tensor`) and labels -> fp32 [G, 7], int64 [G] on dev, B + 1 offsets"""
+def _cat_gt(fn, gt_boxes, gt_labels, dev, cols=7):
+    """per-sample boxes (columns 0 to cols - 1 of tensors or of their `.tensor`) and labels -> fp32 [G, cols], int64 [G] on dev, B + 1
+    offsets.  A sample without boxes may have any width."""
     boxes = [getattr(b, "tensor", b) for b in gt_boxes]
     for b, lab in zip(boxes, gt_labels):
-        if b.dim() != 2 or b.shape[1] < 7 or lab.shape != (b.shape[0],):
+        if b.dim() != 2 or (b.shape[1] < cols and b.shape[0] > 0) or b.shape[1] < 7 or lab.shape != (b.shape[0],):
             raise L.SSTB200Error(f"{fn}: boxes {tuple(b.shape)} and labels {tuple(lab.shape)} do not match")
-    gt = torch.cat([b[:, :7] for b in boxes]).to(dev, torch.float32).contiguous()
+    boxes = [b if b.shape[1] >= cols else b.new_zeros((0, cols)) for b in boxes]
+    gt = torch.cat([b[:, :cols] for b in boxes]).to(dev, torch.float32).contiguous()
     gl = torch.cat([lab.reshape(-1) for lab in gt_labels]).to(dev, torch.int64).contiguous()
     return gt, gl, _offsets([b.shape[0] for b in boxes])
 
@@ -1659,7 +1662,24 @@ L.SIGNATURES["sstb200_cluster_head_targets"] = (C.c_int, [L.vp, L.vp, C.c_int64,
 L.SIGNATURES["sstb200_cluster_head_loss_forward"] = (C.c_int, _CH_ARGS + [L.vp])
 L.SIGNATURES["sstb200_cluster_head_loss_backward"] = (C.c_int, _CH_ARGS + [L.vp, _PP, _PP])
 
+
+class _ClusterHeadCfgEx(C.Structure):
+    _fields_ = _ClusterHeadCfg._fields_ + [("loss_weight_vel", C.c_float), ("code_size", C.c_int32)]
+
+
+_CH_ARGS_EX = [L.vp, C.POINTER(_ClusterHeadCfgEx)] + _CH_ARGS[2:]
+L.SIGNATURES["sstb200_cluster_head_targets_ex"] = (C.c_int, [L.vp, L.vp, C.c_int64, L.vp, C.c_int64, L.vp, C.c_int64, C.c_int64, L.vp,
+                                                             C.c_int, L.vp, L.P_i32, C.c_int, C.c_int, L.P_i32, L.P_i32, C.c_int, L.P_i32,
+                                                             C.c_int, _PP, _PP, L.vp])
+L.SIGNATURES["sstb200_cluster_head_loss_forward_ex"] = (C.c_int, _CH_ARGS_EX + [L.vp])
+L.SIGNATURES["sstb200_cluster_head_loss_backward_ex"] = (C.c_int, _CH_ARGS_EX + [L.vp, _PP, _PP])
+
 CLUSTER_HEAD_CODE_SIZE = 8
+
+
+def _target_cols(code_size):
+    """bbox_targets columns for a code size: 8, or 10 plus the velocity loss weight"""
+    return 11 if code_size == 10 else 8
 
 
 def _batch_index(cluster_inds, M):
@@ -1679,13 +1699,19 @@ def _batch_index(cluster_inds, M):
     return col, max(col.stride(0), 1)
 
 
-def cluster_head_targets(cluster_xyz, cluster_inds, gt_boxes, gt_labels, tasks, class_names):
+def cluster_head_targets(cluster_xyz, cluster_inds, gt_boxes, gt_labels, tasks, class_names, assign_xyz=None, code_size=8):
     """SparseClusterHeadV2.get_targets of every task for the whole batch in one launch.  cluster_xyz fp32 [M, >= 3] (read in place, any
     row stride); cluster_inds int64 [M, 3] (column 1 is the sample) or [M]; gt_boxes: a list over samples of [G_b, >= 7] bottom-centre
     boxes (tensors or objects with `.tensor`), gt_labels: a list of int64 [G_b] global class ids; tasks: lists of class names per task,
     class_names: the global class list.  Returns (labels, bbox_targets, num_pos): lists over tasks of int64 [M] (background = the task's
     class count), fp32 [M, 8] (zeros on negatives) and an int64 [T] device tensor of the positives.  A cluster whose sample index is
-    outside [0, B) gets label -1 and NaN targets.  No host sync."""
+    outside [0, B) gets label -1 and NaN targets.  No host sync.
+    FSDV2Head: assign_xyz fp32 [M, >= 3] (read in place) is tested against the boxes instead of cluster_xyz, which the encode still
+    subtracts (train_cfg centroid_assign).  code_size 10 reads the boxes' velocity (columns 7-8; every sample with boxes must have 9 or
+    10 columns, the 10th the copy-paste flag) and returns bbox_targets fp32 [M, 11]: the 10 code columns, then the velocity loss weight
+    (the flag, or 1 for 9-column boxes; 0 on negatives)."""
+    if code_size not in (8, 10):
+        raise L.SSTB200Error(f"cluster_head_targets: code_size must be 8 or 10, got {code_size}")
     xyz = cluster_xyz
     if not isinstance(xyz, torch.Tensor) or not xyz.is_cuda or xyz.dtype != torch.float32 or xyz.dim() != 2 or xyz.shape[1] < 3:
         raise L.SSTB200Error("cluster_head_targets: cluster_xyz must be a float32 [M, >= 3] CUDA tensor")
@@ -1706,7 +1732,11 @@ def cluster_head_targets(cluster_xyz, cluster_inds, gt_boxes, gt_labels, tasks, 
             class_task[k], class_rank[k] = t, r
     T = len(tasks)
     dev = xyz.device
-    gt, gl, gt_offs = _cat_gt("cluster_head_targets", gt_boxes, gt_labels, dev)
+    if assign_xyz is None and code_size == 8:
+        gt, gl, gt_offs = _cat_gt("cluster_head_targets", gt_boxes, gt_labels, dev)
+    else:
+        return _cluster_head_targets_ex(xyz, bidx, bstride, gt_boxes, gt_labels, B, names, class_task, class_rank, tasks, assign_xyz,
+                                        code_size)
     labels = [torch.empty((M,), dtype=torch.int64, device=dev) for _ in range(T)]
     targets = [torch.empty((M, CLUSTER_HEAD_CODE_SIZE), dtype=torch.float32, device=dev) for _ in range(T)]
     num_pos = torch.empty((T,), dtype=torch.int64, device=dev)
@@ -1719,25 +1749,67 @@ def cluster_head_targets(cluster_xyz, cluster_inds, gt_boxes, gt_labels, tasks, 
     return labels, targets, num_pos
 
 
+def _cluster_head_targets_ex(xyz, bidx, bstride, gt_boxes, gt_labels, B, names, class_task, class_rank, tasks, assign_xyz, code_size):
+    """cluster_head_targets with assignment points and / or code size 10 (sstb200_cluster_head_targets_ex)"""
+    fn = "cluster_head_targets"
+    M, dev, T = xyz.shape[0], xyz.device, len(tasks)
+    axyz = xyz
+    if assign_xyz is not None:
+        axyz = assign_xyz
+        if not isinstance(axyz, torch.Tensor) or not axyz.is_cuda or axyz.dtype != torch.float32 or axyz.dim() != 2 or \
+                axyz.shape[0] != M or axyz.shape[1] < 3:
+            raise L.SSTB200Error(f"{fn}: assign_xyz must be a float32 [{M}, >= 3] CUDA tensor")
+        if axyz.device != dev:
+            raise L.SSTB200Error(f"{fn}: assign_xyz on {axyz.device}, cluster_xyz on {dev}")
+        if axyz.stride(1) != 1 or axyz.stride(0) < 3:
+            axyz = axyz.contiguous()
+    width = 7
+    if code_size == 10:
+        widths = {getattr(b, "tensor", b).shape[-1] for b in gt_boxes if getattr(b, "tensor", b).shape[0] > 0}
+        if len(widths) > 1 or not widths <= {9, 10}:
+            raise L.SSTB200Error(f"{fn}: code_size 10 needs boxes of 9 or 10 columns in every sample, got widths {sorted(widths)}")
+        width = widths.pop() if widths else 9
+    gt, gl, gt_offs = _cat_gt(fn, gt_boxes, gt_labels, dev, cols=width)
+    labels = [torch.empty((M,), dtype=torch.int64, device=dev) for _ in range(T)]
+    targets = [torch.empty((M, _target_cols(code_size)), dtype=torch.float32, device=dev) for _ in range(T)]
+    num_pos = torch.empty((T,), dtype=torch.int64, device=dev)
+    c = L.ctx(dev)
+    L.check(c, L.lib().sstb200_cluster_head_targets_ex(
+        c, L.ptr(xyz) if M else None, xyz.stride(0), L.ptr(axyz) if M and assign_xyz is not None else None,
+        axyz.stride(0) if assign_xyz is not None else 0, L.ptr(bidx) if M else None, bstride, M, L.ptr(gt) if gt.numel() else None,
+        width, L.ptr(gl) if gl.numel() else None, L.arr(C.c_int32, gt_offs), B, len(names), L.arr(C.c_int32, class_task),
+        L.arr(C.c_int32, class_rank), T, L.arr(C.c_int32, [len(t) for t in tasks]), code_size, _ptrs(labels), _ptrs(targets),
+        L.ptr(num_pos)))
+    return labels, targets, num_pos
+
+
 class ClusterHeadLossConfig:
     """The constant part of SparseClusterHeadV2.loss_single_task: the focal settings of loss_cls and the L1 / SmoothL1 settings and
-    weights of loss_center / loss_size / loss_rot (the three must share their type and beta).  Built once per head."""
+    weights of loss_center / loss_size / loss_rot (the three must share their type and beta).  Built once per head.
+    loss_weight_vel (FSDV2Head's loss_vel, of the same type and beta) makes the code size 10: the losses gain a fifth column, vel."""
 
     def __init__(self, gamma=2.0, alpha=0.25, loss_weight_cls=1.0, loss_weight_center=1.0, loss_weight_size=1.0, loss_weight_rot=1.0,
-                 smooth_l1=False, beta=1.0):
+                 smooth_l1=False, beta=1.0, loss_weight_vel=None):
         self.gamma, self.alpha, self.smooth_l1, self.beta = float(gamma), float(alpha), bool(smooth_l1), float(beta)
         self.weights = (float(loss_weight_cls), float(loss_weight_center), float(loss_weight_size), float(loss_weight_rot))
+        self.loss_weight_vel = None if loss_weight_vel is None else float(loss_weight_vel)
+        self.code_size = 8 if loss_weight_vel is None else 10
 
     def struct(self):
         return _ClusterHeadCfg(self.gamma, self.alpha, int(self.smooth_l1), self.beta, *self.weights)
 
+    def struct_ex(self):
+        return _ClusterHeadCfgEx(self.gamma, self.alpha, int(self.smooth_l1), self.beta, *self.weights, self.loss_weight_vel or 0.0,
+                                 self.code_size)
 
-def _cluster_head_loss_inputs(labels, targets, num_pos, cls_avg, reg_avg, preds):
+
+def _cluster_head_loss_inputs(labels, targets, num_pos, cls_avg, reg_avg, preds, code=CLUSTER_HEAD_CODE_SIZE):
     """every tensor the loss kernels read as a raw device array, checked: the T cls_logits [M, C_t] and T reg_preds [M, 8] fp32 rows
     with unit column stride, labels int64 [M] and bbox_targets fp32 [M, 8] per task, num_pos int64 [T] and the fp32 avg factors [T],
     all CUDA tensors on the predictions' device.  Shapes and dtypes are checked before devices.  Returns them contiguous where the
-    kernels need it."""
+    kernels need it.  Code size 10: reg_preds [M, 10] and bbox_targets [M, 11]."""
     T = len(labels)
+    tc = _target_cols(code)
     if T < 1 or len(targets) != T or len(preds) != 2 * T:
         raise L.SSTB200Error(f"cluster_head_loss: {len(preds)} predictions, {len(labels)} labels and {len(targets)} bbox_targets; "
                              "one cls_logits, reg_preds, labels and bbox_targets per task")
@@ -1751,13 +1823,13 @@ def _cluster_head_loss_inputs(labels, targets, num_pos, cls_avg, reg_avg, preds)
         raise L.SSTB200Error(f"cluster_head_loss: cls_logits[0] must be [M, C] with M > 0, got {tuple(preds[0].shape)}")
     for k in range(T):
         x, r = preds[k], preds[T + k]
-        if x.dim() != 2 or x.shape[0] != M or x.shape[1] < 1 or r.shape != (M, CLUSTER_HEAD_CODE_SIZE):
+        if x.dim() != 2 or x.shape[0] != M or x.shape[1] < 1 or r.shape != (M, code):
             raise L.SSTB200Error(f"cluster_head_loss: task {k}: cls_logits {tuple(x.shape)} and reg_preds {tuple(r.shape)} do not fit "
-                                 f"[{M}, C] and [{M}, {CLUSTER_HEAD_CODE_SIZE}]")
+                                 f"[{M}, C] and [{M}, {code}]")
         if labels[k].dtype != torch.int64 or labels[k].shape != (M,):
             raise L.SSTB200Error(f"cluster_head_loss: labels[{k}] must be int64 [{M}], got {labels[k].dtype} {tuple(labels[k].shape)}")
-        if targets[k].dtype != torch.float32 or targets[k].shape != (M, CLUSTER_HEAD_CODE_SIZE):
-            raise L.SSTB200Error(f"cluster_head_loss: bbox_targets[{k}] must be float32 [{M}, {CLUSTER_HEAD_CODE_SIZE}], got "
+        if targets[k].dtype != torch.float32 or targets[k].shape != (M, tc):
+            raise L.SSTB200Error(f"cluster_head_loss: bbox_targets[{k}] must be float32 [{M}, {tc}], got "
                                  f"{targets[k].dtype} {tuple(targets[k].shape)}")
     if num_pos.dtype != torch.int64 or num_pos.shape != (T,):
         raise L.SSTB200Error(f"cluster_head_loss: num_pos must be int64 [{T}], got {num_pos.dtype} {tuple(num_pos.shape)}")
@@ -1765,7 +1837,7 @@ def _cluster_head_loss_inputs(labels, targets, num_pos, cls_avg, reg_avg, preds)
         if f.dtype not in (torch.float32, torch.float16) or f.shape != (T,):
             raise L.SSTB200Error(f"cluster_head_loss: {name} must be float32 [{T}], got {f.dtype} {tuple(f.shape)}")
     xs = [_row_major(f"cls_logits[{k}]", x, x.shape[1]) for k, x in enumerate(preds[:T])]
-    rs = [_row_major(f"reg_preds[{k}]", r, CLUSTER_HEAD_CODE_SIZE) for k, r in enumerate(preds[T:])]
+    rs = [_row_major(f"reg_preds[{k}]", r, code) for k, r in enumerate(preds[T:])]
     dev = xs[0].device
     named = [(f"cls_logits[{k}]", a) for k, a in enumerate(xs)] + [(f"reg_preds[{k}]", a) for k, a in enumerate(rs)] + \
         [(f"labels[{k}]", a) for k, a in enumerate(labels)] + [(f"bbox_targets[{k}]", a) for k, a in enumerate(targets)] + \
@@ -1781,21 +1853,30 @@ def _cluster_head_loss_inputs(labels, targets, num_pos, cls_avg, reg_avg, preds)
 
 class ClusterHeadLossFunction(Function):
     """loss_single_task of every task in one launch sequence (sstb200_cluster_head_loss_forward): returns losses [T, 4] = (cls, center,
-    size, rot) per task.  Inputs: cfg, the targets of cluster_head_targets, the device avg factors cls_avg [T] and reg_avg [T], then the
+    size, rot) per task, [T, 5] with vel for a code-size-10 cfg (the _ex entry points).  Inputs: cfg, the targets of cluster_head_targets, the device avg factors cls_avg [T] and reg_avg [T], then the
     T cls_logits [M, C_t] and the T reg_preds [M, 8], read in place with their row strides.  Saves the predictions, targets and factors
     only; the backward writes each cluster's own rows with no atomics (bit-identical from run to run).  No host sync."""
 
     @staticmethod
     def forward(ctx, cfg, labels, targets, num_pos, cls_avg, reg_avg, *preds):
         T = len(labels)
-        xs, rs, labels, targets, num_pos, ca, ra = _cluster_head_loss_inputs(labels, targets, num_pos, cls_avg, reg_avg, preds)
+        code = getattr(cfg, "code_size", CLUSTER_HEAD_CODE_SIZE)
+        xs, rs, labels, targets, num_pos, ca, ra = _cluster_head_loss_inputs(labels, targets, num_pos, cls_avg, reg_avg, preds, code)
         M = xs[0].shape[0]
-        losses = torch.empty((T, 4), dtype=torch.float32, device=xs[0].device)
+        losses = torch.empty((T, 4 if code == 8 else 5), dtype=torch.float32, device=xs[0].device)
         c = L.ctx(xs[0].device)
-        st = cfg.struct()
-        args = (c, C.byref(st), T, M, _ptrs(xs), L.arr(C.c_int64, [x.stride(0) for x in xs]), L.arr(C.c_int32, [x.shape[1] for x in xs]),
-                _ptrs(rs), L.arr(C.c_int64, [r.stride(0) for r in rs]), _ptrs(labels), _ptrs(targets), L.ptr(num_pos), L.ptr(ca), L.ptr(ra))
-        L.check(c, L.lib().sstb200_cluster_head_loss_forward(*args, L.ptr(losses)))
+        if code == 8:
+            st = cfg.struct()
+            args = (c, C.byref(st), T, M, _ptrs(xs), L.arr(C.c_int64, [x.stride(0) for x in xs]),
+                    L.arr(C.c_int32, [x.shape[1] for x in xs]), _ptrs(rs), L.arr(C.c_int64, [r.stride(0) for r in rs]), _ptrs(labels),
+                    _ptrs(targets), L.ptr(num_pos), L.ptr(ca), L.ptr(ra))
+            L.check(c, L.lib().sstb200_cluster_head_loss_forward(*args, L.ptr(losses)))
+        else:
+            st = cfg.struct_ex()
+            L.check(c, L.lib().sstb200_cluster_head_loss_forward_ex(c, C.byref(st), T, M, _ptrs(xs),
+                                L.arr(C.c_int64, [x.stride(0) for x in xs]), L.arr(C.c_int32, [x.shape[1] for x in xs]), _ptrs(rs),
+                                L.arr(C.c_int64, [r.stride(0) for r in rs]), _ptrs(labels), _ptrs(targets), L.ptr(num_pos), L.ptr(ca),
+                                L.ptr(ra), L.ptr(losses)))
         ctx.save_for_backward(num_pos, ca, ra, *xs, *rs, *labels, *targets)
         ctx.cfg, ctx.T, ctx.dtypes = cfg, T, [p.dtype for p in preds]
         return losses
@@ -1808,21 +1889,29 @@ class ClusterHeadLossFunction(Function):
         xs, rs, labels, targets = saved[3:3 + T], saved[3 + T:3 + 2 * T], saved[3 + 2 * T:3 + 3 * T], saved[3 + 3 * T:]
         M = xs[0].shape[0]
         gx = [torch.empty((M, x.shape[1]), dtype=torch.float32, device=x.device) for x in xs]
-        gr = [torch.empty((M, CLUSTER_HEAD_CODE_SIZE), dtype=torch.float32, device=x.device) for x in xs]
+        gr = [torch.empty((M, rs[0].shape[1]), dtype=torch.float32, device=x.device) for x in xs]
         gl = grad_losses.float().contiguous()
         c = L.ctx(xs[0].device)
-        st = ctx.cfg.struct()
-        L.check(c, L.lib().sstb200_cluster_head_loss_backward(
-            c, C.byref(st), T, M, _ptrs(xs), L.arr(C.c_int64, [x.stride(0) for x in xs]), L.arr(C.c_int32, [x.shape[1] for x in xs]),
-            _ptrs(rs), L.arr(C.c_int64, [r.stride(0) for r in rs]), _ptrs(labels), _ptrs(targets), L.ptr(num_pos), L.ptr(ca), L.ptr(ra),
-            L.ptr(gl), _ptrs(gx), _ptrs(gr)))
+        if getattr(ctx.cfg, "code_size", CLUSTER_HEAD_CODE_SIZE) == 8:
+            st = ctx.cfg.struct()
+            L.check(c, L.lib().sstb200_cluster_head_loss_backward(
+                c, C.byref(st), T, M, _ptrs(xs), L.arr(C.c_int64, [x.stride(0) for x in xs]), L.arr(C.c_int32, [x.shape[1] for x in xs]),
+                _ptrs(rs), L.arr(C.c_int64, [r.stride(0) for r in rs]), _ptrs(labels), _ptrs(targets), L.ptr(num_pos), L.ptr(ca), L.ptr(ra),
+                L.ptr(gl), _ptrs(gx), _ptrs(gr)))
+        else:
+            st = ctx.cfg.struct_ex()
+            L.check(c, L.lib().sstb200_cluster_head_loss_backward_ex(c, C.byref(st), T, M, _ptrs(xs),
+                                    L.arr(C.c_int64, [x.stride(0) for x in xs]), L.arr(C.c_int32, [x.shape[1] for x in xs]), _ptrs(rs),
+                                    L.arr(C.c_int64, [r.stride(0) for r in rs]), _ptrs(labels), _ptrs(targets), L.ptr(num_pos), L.ptr(ca),
+                                    L.ptr(ra), L.ptr(gl), _ptrs(gx), _ptrs(gr)))
         grads = [g.to(d) for g, d in zip(gx + gr, ctx.dtypes)]
         return (None, None, None, None, None, None, *grads)
 
 
 def cluster_head_loss(cls_logits, reg_preds, labels, bbox_targets, num_pos, cls_avg_factor, reg_avg_factor, cfg):
     """losses [T, 4] = (loss_cls, loss_center, loss_size, loss_rot) per task of ClusterHeadLossFunction, an fp32 device tensor carrying
-    gradients to the T cls_logits and T reg_preds.  cls_avg_factor / reg_avg_factor: fp32 device [T] (see SparseClusterHeadV2.loss for
+    gradients to the T cls_logits and T reg_preds; [T, 5] with loss_vel when cfg has loss_weight_vel (reg_preds [M, 10], bbox_targets
+    [M, 11] from cluster_head_targets(code_size=10)).  cls_avg_factor / reg_avg_factor: fp32 device [T] (see SparseClusterHeadV2.loss for
     how the head forms them).  A misshapen, mistyped or off-device input raises SSTB200Error."""
     if len(cls_logits) != len(labels) or len(reg_preds) != len(labels) or len(bbox_targets) != len(labels):
         raise L.SSTB200Error("cluster_head_loss: one cls_logits, reg_preds, labels and bbox_targets per task")
