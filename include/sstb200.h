@@ -717,8 +717,10 @@ int sstb200_centerpoint_l1_loss_backward(sstb200_ctx* ctx, const float* const he
  *   place; element (b, y, x, a, c) is channel a C + c, anchor (y W + x) A_loc + a) against one-hot(labels) [B, A] with background
  *   num_classes, weighted by label_weights [B, A]: *loss = loss_weight * sum / num_total_pos (device int64).  Log-sigmoid is the stable
  *   softplus form of mmdet's py_sigmoid_focal_loss: it stays exact for logits of any size, where mmcv's CUDA kernel clamps
- *   log(max(1 - p, FLT_MIN)) and so saturates near 87 for logits beyond about +-17.  A NaN logit makes the loss NaN.  Block partials in
- *   double summed in a fixed order: deterministic.  Two launches, partials from the context arena.
+ *   log(max(1 - p, FLT_MIN)) and so saturates near 87 for logits beyond about +-17.  A NaN logit makes the loss NaN.  An infinite logit
+ *   follows the closed form: on its label's side (+inf for the target class, -inf otherwise) loss 0 and gradient 0, on the other side
+ *   loss inf and gradient NaN; mmdet's Python path gives NaN for both.  Block partials in double summed in a fixed order:
+ *   deterministic.  Two launches, partials from the context arena.
  * sstb200_anchor_focal_loss_backward: grad_cls_score (same shape) = grad_loss[0] * loss_weight / num_total_pos * label_weight * d loss /
  *   d logit, recomputed from the logits in one elementwise pass; NaN only at a NaN logit.
  *
@@ -727,8 +729,10 @@ int sstb200_centerpoint_l1_loss_backward(sstb200_ctx* ctx, const float* const he
  *   num_total_pos, channel 6 compared as sin(p) cos(t) against cos(p) sin(t) (add_sin_difference); loss_dir = loss_weight_dir *
  *   sum dir_weight * (logsumexp(z) - z[dir_target]) / num_total_pos.  No positives: both 0.  Two launches.
  * sstb200_anchor_reg_dir_loss_backward: grad_losses = (d / d loss_bbox, d / d loss_dir) on the device; grad_bbox_pred / grad_dir_cls_preds
- *   fully written, zero off the positives: each positive owns its cells' channels, so there are no atomics.  sign(0) = 0, as torch.abs'
- *   gradient; the yaw channel's derivative goes through both sin(p) cos(t) and cos(p) sin(t).  One launch.
+ *   fully written, zero off the positives: each positive owns its cells' channels, so there are no atomics.  sign(0) = sign(NaN) = 0, as
+ *   torch.abs' gradient: a NaN box coordinate gets gradient 0.  The yaw channel's derivative goes through both sin(p) cos(t) and cos(p)
+ *   sin(t), their products rounded apart as torch rounds them: a yaw equal to its target gets gradient 0, a NaN yaw a NaN gradient.  One
+ *   launch.
  *   Errors (all four): a NULL pointer or a size < 1 (SSTB_ERR_ARG). */
 int sstb200_anchor3d_targets(sstb200_ctx* ctx, const float* x_centers, int width, const float* y_centers, int height, const float* size_z,
                              const float* size_wlh, int num_sizes, const float* rotations, int num_rots, const float* gt_boxes,
@@ -777,7 +781,8 @@ int sstb200_anchor_reg_dir_loss_backward(sstb200_ctx* ctx, const float* bbox_pre
  *   - use_softmax 0: mmdet 2.14 FocalLoss(use_sigmoid=True, gamma, alpha) against one-hot(label) without the background column
  *     (label C), reduction 'mean' without avg_factor: losses[0] = loss_weight * sum / (N C).  The log-sigmoid is the stable softplus form
  *     of py_sigmoid_focal_loss, exact for logits of any size; mmcv's CUDA kernel instead clamps log(max(1 - p, FLT_MIN)) and so saturates
- *     near 87 for logits beyond about +-17.  gamma must be >= 1.
+ *     near 87 for logits beyond about +-17.  An infinite logit follows the closed form: on its label's side loss 0 and gradient 0, on
+ *     the other loss inf and gradient NaN, where mmdet's Python path gives NaN for both.  gamma must be >= 1.
  *   - use_softmax 1: mmseg CrossEntropyLoss(use_sigmoid=False, class_weight): losses[0] = loss_weight * sum w[y] (logsumexp(x) - x[y]) / N,
  *     divided by N and not by the sum of the weights (F.cross_entropy(reduction='none') then weight_reduce_loss, mmseg 0.14.1 to 1.0,
  *     avg_non_ignore False).  class_weight: host [C], NULL for ones.  Labels come from get_targets and are never 255 or -100, so
@@ -856,7 +861,7 @@ int sstb200_voteseg_loss_backward(sstb200_ctx* ctx, const sstb200_voteseg_cfg* c
  *   losses f32 [T, 4] = (cls, center, size, rot) with
  *   - cls: loss_weight_cls * sum focal / cls_avg_factor[t], mmdet 2.14 FocalLoss(use_sigmoid=True, gamma, alpha) against one-hot(label)
  *     without the background column C_t, label_weights all ones, in the stable softplus form (see sstb200_voteseg_loss_forward for the
- *     difference from mmcv's clamped CUDA kernel).  A label outside [0, C_t] makes it NaN.  gamma must be >= 1.
+ *     difference from mmcv's clamped CUDA kernel, and for its infinite logits).  A label outside [0, C_t] makes it NaN.  gamma must be >= 1.
  *   - center / size / rot: loss_weight_q * sum over the positives (0 <= label < C_t) of L1 |d| or, with smooth_l1, mmdet's SmoothL1
  *     (|d| < beta ? 0.5 d^2 / beta : |d| - 0.5 beta) on columns [0, 3), [3, 6), [6, 8), over reg_avg_factor[t].  When the local
  *     num_pos[t] is 0 they are exactly 0 whatever the factor (the reference's `num_pos > 0` branch takes pos_reg_preds.sum() * 0).

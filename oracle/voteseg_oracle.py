@@ -78,6 +78,22 @@ def losses(seg_logits, vote_preds, labels, vote_targets, vote_mask, use_sigmoid,
     return seg, vote
 
 
+def sigmoid_focal64(x, t, alpha, gamma):
+    """(loss, d loss / d x) of each sigmoid focal element in float64, x float64 logits and t bool targets, with s and q = 1 - s both
+    formed from exp(-|x|): the same function as `losses`' sigmoid branch (and the Anchor3D / cluster heads' focal terms), but with no
+    1 - p, so that every element keeps its relative precision out to logits of several hundred.  Autograd through 1 - p loses it beyond
+    |x| of about 15 and gives 0 beyond about 37; the error model of the native kernels is relative per element and needs this form."""
+    e = torch.exp(-x.abs())
+    inv = 1 / (1 + e)
+    s = torch.where(x >= 0, inv, e * inv)
+    q = torch.where(x >= 0, e * inv, inv)
+    l1p = torch.log1p(e)
+    sp_pos, sp_neg = x.clamp(min=0) + l1p, (-x).clamp(min=0) + l1p
+    loss = torch.where(t, alpha * q.pow(gamma) * sp_neg, (1 - alpha) * s.pow(gamma) * sp_pos)
+    grad = torch.where(t, -alpha * q.pow(gamma) * (gamma * s * sp_neg + q), (1 - alpha) * s.pow(gamma) * (gamma * q * sp_pos + s))
+    return loss, grad
+
+
 def scores(seg_logits, use_sigmoid, logit_scale=1.0, class_names=None, group_names=None, **_):
     """[N, G] float64 scores the training log thresholds: sigmoid per class, or the group sums of the softmax (background excluded)"""
     x = seg_logits.double() * logit_scale

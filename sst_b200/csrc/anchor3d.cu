@@ -378,9 +378,9 @@ __global__ void __launch_bounds__(LOSS_THREADS) reg_forward_kernel(const RegArgs
     const float* w = a.bbox_w + slot * 7;
 #pragma unroll
     for (int k = 0; k < 6; k++) l1 += (double)(fabsf(p[k * a.HW] - t[k]) * (w[k] * a.cw[k]));
-    // add_sin_difference: sin(p) cos(t) against cos(p) sin(t)
+    // add_sin_difference: sin(p) cos(t) against cos(p) sin(t), each product rounded as torch rounds it (no FMA contraction)
     const float p6 = p[6 * a.HW], t6 = t[6];
-    l1 += (double)(fabsf(sinf(p6) * cosf(t6) - cosf(p6) * sinf(t6)) * (w[6] * a.cw[6]));
+    l1 += (double)(fabsf(__fsub_rn(__fmul_rn(sinf(p6), cosf(t6)), __fmul_rn(cosf(p6), sinf(t6)))) * (w[6] * a.cw[6]));
     const float* d = a.dir + ba * 2 * a.HW + hw;
     const float z0 = d[0], z1 = d[a.HW];
     const float lse = fmaxf(z0, z1) + log1pf(expf(-fabsf(z0 - z1)));
@@ -390,9 +390,6 @@ __global__ void __launch_bounds__(LOSS_THREADS) reg_forward_kernel(const RegArgs
   ce = thread0_block_sum(ce, sh);
   if (threadIdx.x == 0) part[blockIdx.x] = l1, part[nparts + blockIdx.x] = ce;
 }
-
-// sign(d) with NaN passed through; torch.abs' gradient (heads.cuh's abs_grad) is 0 at NaN, a behaviour change kept for a separate fix
-__device__ __forceinline__ float sign_nan(float d) { return d > 0.f ? 1.f : (d < 0.f ? -1.f : (d == d ? 0.f : d)); }
 
 // every (b, anchor, cell) owns its 7 + 2 channels: the gradients are written in full, zero off the positives
 __global__ void __launch_bounds__(LOSS_THREADS) reg_backward_kernel(const RegArgs a, float w_bbox, float w_dir,
@@ -420,15 +417,17 @@ __global__ void __launch_bounds__(LOSS_THREADS) reg_backward_kernel(const RegArg
 #pragma unroll
     for (int k = 0; k < 6; k++) {
       const float df = p[k * a.HW] - t[k];
-      gb[k * a.HW] = sb * (w[k] * a.cw[k]) * sign_nan(df);
+      gb[k * a.HW] = sb * (w[k] * a.cw[k]) * abs_grad(df);
     }
     const float p6 = p[6 * a.HW], t6 = t[6];
     float sp, cp, st, ct;
     sincosf(p6, &sp, &cp);
     sincosf(t6, &st, &ct);
-    const float df = sp * ct - cp * st;
-    const float sgn = sign_nan(df);
-    gb[6 * a.HW] = sb * (w[6] * a.cw[6]) * sgn * (cp * ct + sp * st);
+    // rounded products: a predicted yaw equal to its target gives df = 0 exactly, and so a zero gradient, as in torch; a contracted
+    // sp * ct - cp * st would leave the rounding residual of one product and a full-size gradient of either sign
+    const float df = __fsub_rn(__fmul_rn(sp, ct), __fmul_rn(cp, st));
+    // torch.abs' gradient is 0 at a NaN difference; a NaN yaw still makes its own gradient NaN through cos(p) cos(t) + sin(p) sin(t)
+    gb[6 * a.HW] = sb * (w[6] * a.cw[6]) * abs_grad(df) * (cp * ct + sp * st);
     const float* d = a.dir + ba * 2 * a.HW + hw;
     const float z0 = d[0], z1 = d[a.HW];
     const float p1 = 1.f / (1.f + expf(z0 - z1)), p0 = 1.f / (1.f + expf(z1 - z0));
