@@ -942,6 +942,83 @@ int sstb200_cluster_head_loss_backward_ex(sstb200_ctx* ctx, const sstb200_cluste
                                           const float* cls_avg_factor, const float* reg_avg_factor, const float* grad_losses,
                                           float* const* grad_logits, float* const* grad_reg_preds);
 
+/* ---- FSD's second stage (mmdet3d/models/roi_heads/fsd_roi_head.py, bbox_heads/fsd_bbox_head.py,
+ * core/bbox/samplers/iou_neg_piecewise_sampler.py), fp32, stream-ordered, no host sync.
+ *
+ * sstb200_roi_assign_sample: GroupCorrectionHead._assign_and_sample for every sample in one launch (one CTA per sample).
+ *   proposals [P, prop_width] (7 or 9 columns, LiDAR bottom-centre) with predicted labels int64 [P], sample b owning rows
+ *   [prop_offsets[b], prop_offsets[b + 1]) (host, batch + 1; every sample needs a proposal: the caller adds the reference's fake box);
+ *   keys fp32 [P], one per proposal; gt_boxes [G, gt_width] (7, 9 or 10; columns 0-6 are used) and gt_labels int64 [G] with host
+ *   gt_offsets.  per_class: proposal i is matched only against the GTs labelled plab[i] by assigner plab[i] (a label outside
+ *   [0, num_classes) leaves it negative with IoU 0); otherwise one assigner over every GT.  Each assigner is mmdet 2.14
+ *   MaxIoUAssigner.assign_wrt_overlaps with match_low_quality and gt_max_assign_all, over the 3-D IoU of
+ *   LiDARInstance3DBoxes.overlaps (fp32, the BEV overlap of sstb200_boxes_overlap_bev).  The sampler is IoUNegPiecewiseSampler with
+ *   neg_pos_ub < 0 and no GT proposals: at most num_pos (= int(num * pos_fraction)) positives, then num - positives negatives split
+ *   into IoU pieces [piece_thrs[q + 1], piece_thrs[q]) (the last [0, piece_thrs[last])) with the reference's carry-over.  Where the
+ *   reference calls random_choice(gallery, k) this keeps the k members with the smallest keys, ties to the lower index.
+ *   Outputs: sample b's rows at [b * num, b * num + counts[2 b + 1]), positives (counts[2 b] of them) by ascending proposal index, then
+ *   negatives by ascending index: out_inds (global proposal row), out_iou (max_overlaps), out_gt (global GT row, -1 on negatives),
+ *   out_labels (the GT's label, -1 on negatives); counts int32 [batch, 2] on the device.  Temporaries from the context arena.
+ *   Errors: a NULL pointer, a width other than the above, offsets that do not start at 0 or decrease, a sample without proposals
+ *   (SSTB_ERR_ARG); more than 4096 proposals or GTs in a sample, more than 8 assigners or IoU pieces (SSTB_ERR_UNSUPPORTED).
+ *
+ * sstb200_roi_head_targets: FullySparseBboxHead.get_targets for all num_rows sampled rows in one launch.  rois [R, roi_width] the
+ *   sampled proposals, iou / gt_rows / labels the rows of sstb200_roi_assign_sample (gt_rows index gt_boxes).  Outputs per row:
+ *   soft_labels fp32 (get_multi_class_soft_label with cls_pos_thr / cls_neg_thr, host double [num_classes]: the compares take them
+ *   in fp32 and the divisor is (float)(pos - neg) formed in double, as torch does with Python floats; 0 on negatives), reg_mask int64
+ *   (1 on positives), bbox_targets fp32 [R, 7] (the canonical transform into the RoI's frame and DeltaXYZWLHRBBoxCoder.encode against
+ *   the zero-centred RoI, in double, rounded once; 0 on negatives) and pos_gt_bboxes fp32 [R, 7] (the GT's columns 0-6; 0 on negatives).
+ *
+ * sstb200_roi_head_loss_forward: FullySparseBboxHead.loss in one launch sequence.  cls_score [R] and bbox_pred [R, 7] read with row
+ *   strides; nonempty uint8 [R]; the targets above; labels the rows' GT labels; rois [R, roi_width] without the batch column;
+ *   cls_avg_factor / reg_avg_factor fp32 [1] on the device.  losses fp32 [3] = (cls, bbox, corner):
+ *   - cls: loss_weight_cls * sum over non-empty rows of the sigmoid BCE against the soft label, over cls_avg_factor;
+ *   - bbox: loss_weight_bbox * sum over positives on non-empty RoIs of L1 / SmoothL1(beta) times code_weights, over reg_avg_factor;
+ *   - corner: corner_loss_weight * the mean over those positives (of class corner_class, or all with -1) and their 8 corners of the
+ *     Huber (delta 1) distance from the prediction decoded against its RoI to the nearer of the GT's and the heading-flipped GT's.
+ *   A term without rows is exactly 0.  counts fp32 [2] = (positives on non-empty RoIs, corner rows), for the backward.  Block partials
+ *   in double summed in a fixed order: deterministic.  Two launches, partials from the context arena.
+ * sstb200_roi_head_loss_backward: grad_losses (device [3]) -> grad_cls [R] and grad_pred [R, 7], contiguous, each row writing only its
+ *   own entries (no atomics).  One launch.
+ *   Errors (both): a NULL pointer, R < 1, a row stride below the row, roi_width other than 7 / 9, SmoothL1 with beta <= 0 (SSTB_ERR_ARG). */
+typedef struct {
+  int32_t per_class;                   /* 1: one assigner per predicted class; 0: one assigner over every GT */
+  int32_t num_classes;                 /* assigners when per_class */
+  float pos_iou_thr[8], neg_iou_thr[8], min_pos_iou[8];
+  int32_t num, num_pos;                /* sampler num, int(num * pos_fraction) */
+  int32_t num_pieces;
+  double piece_fractions[8];
+  float piece_thrs[8];
+} sstb200_roi_sample_cfg;
+typedef struct {
+  int32_t smooth_l1;                   /* 0: L1Loss, 1: SmoothL1Loss(beta) */
+  float beta;
+  float loss_weight_cls, loss_weight_bbox;
+  int32_t with_corner_loss;
+  int32_t corner_class;                /* -1: every positive */
+  float corner_loss_weight;
+  float code_weights[7];
+} sstb200_roi_loss_cfg;
+int sstb200_roi_assign_sample(sstb200_ctx* ctx, const sstb200_roi_sample_cfg* cfg, const float* proposals, int prop_width,
+                              const int64_t* prop_labels, const float* keys, const int32_t* prop_offsets, const float* gt_boxes,
+                              int gt_width, const int64_t* gt_labels, const int32_t* gt_offsets, int batch, int64_t* out_inds,
+                              float* out_iou, int64_t* out_gt, int64_t* out_labels, int32_t* counts);
+int sstb200_roi_head_targets(sstb200_ctx* ctx, const float* rois, int roi_width, const float* iou, const int64_t* gt_rows,
+                             const int64_t* labels, int64_t num_rows, const float* gt_boxes, int gt_width, int num_classes,
+                             const double* cls_pos_thr, const double* cls_neg_thr, float* soft_labels, int64_t* reg_mask,
+                             float* bbox_targets, float* pos_gt_bboxes);
+int sstb200_roi_head_loss_forward(sstb200_ctx* ctx, const sstb200_roi_loss_cfg* cfg, const float* cls_score, int64_t cls_stride,
+                                  const float* bbox_pred, int64_t pred_stride, const uint8_t* nonempty, const float* soft_labels,
+                                  const int64_t* reg_mask, const float* bbox_targets, const float* pos_gt_bboxes, const int64_t* labels,
+                                  const float* rois, int roi_width, int64_t num_rows, const float* cls_avg_factor,
+                                  const float* reg_avg_factor, float* losses, float* counts);
+int sstb200_roi_head_loss_backward(sstb200_ctx* ctx, const sstb200_roi_loss_cfg* cfg, const float* cls_score, int64_t cls_stride,
+                                   const float* bbox_pred, int64_t pred_stride, const uint8_t* nonempty, const float* soft_labels,
+                                   const int64_t* reg_mask, const float* bbox_targets, const float* pos_gt_bboxes, const int64_t* labels,
+                                   const float* rois, int roi_width, int64_t num_rows, const float* cls_avg_factor,
+                                   const float* reg_avg_factor, const float* counts, const float* grad_losses, float* grad_cls,
+                                   float* grad_pred);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,7 +6,7 @@ from . import registry
 from .registry import BACKBONES, MIDDLE_ENCODERS, MODELS, ROI_EXTRACTORS, VOXEL_ENCODERS, build_backbone, build_middle_encoder, build_voxel_encoder  # noqa: F401
 from . import norm  # noqa: F401
 from . import ops  # noqa: F401
-from . import sst_modules, voxel_modules, sir_modules, neck_modules, fsdv2_modules, spconv_modules, fsd_modules, roiaware_modules, dcn_modules, centerhead_modules, anchor3d_modules, voteseg_modules, cluster_head_modules, fsdv2_head_modules  # noqa: F401
+from . import sst_modules, voxel_modules, sir_modules, neck_modules, fsdv2_modules, spconv_modules, fsd_modules, roiaware_modules, dcn_modules, centerhead_modules, anchor3d_modules, voteseg_modules, cluster_head_modules, fsdv2_head_modules, roi_head_modules  # noqa: F401
 from .sst_modules import SSTInputLayer, SSTInputLayerV2, SSTv1, SSTv2, SST, PseudoMiddleEncoderForSpconvFSD  # noqa: F401
 from .voxel_modules import DynamicVFE, DynamicScatterVFE  # noqa: F401
 from .sir_modules import SIR, SIRLayer  # noqa: F401
@@ -20,6 +20,7 @@ from .anchor3d_modules import SECONDFPN, Anchor3DHead  # noqa: F401
 from .voteseg_modules import VoteSegHead, VoteSegmentor  # noqa: F401
 from .cluster_head_modules import FSDSeparateHead, SparseClusterHeadV2  # noqa: F401
 from .fsdv2_head_modules import FSDV2Head  # noqa: F401
+from .roi_head_modules import FullySparseBboxHead, GroupCorrectionHead  # noqa: F401
 from .spconv_modules import SimpleSparseUNet, SparseUNet, VirtualVoxelMixer, SparseConvTensor  # noqa: F401
 # `from mmdet3d.ops import SparseBasicBlock, make_sparse_convmodule` (mmdet3d/ops/__init__.py:21-22) resolves on the op namespace too
 ops.SparseBasicBlock, ops.make_sparse_convmodule = spconv_modules.SparseBasicBlock, spconv_modules.make_sparse_convmodule

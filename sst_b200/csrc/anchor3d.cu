@@ -158,8 +158,7 @@ __global__ void __launch_bounds__(A3_THREADS) a3_iou_kernel(const __grid_constan
       const float iou = bev_iou(sg[k], an);
       if (PASS == 0) {
         if (live && iou > best) best = iou, arg = c0 + k - begin;
-        const unsigned m = __reduce_max_sync(0xffffffffu, live ? __float_as_uint(iou) : 0u);
-        if ((threadIdx.x & 31) == 0 && m) atomicMax(smax + k, m);
+        warp_max_iou(smax + k, live ? __float_as_uint(iou) : 0u);
       } else if (live && __float_as_uint(iou) == smax[k]) {
         if (all) lq = c0 + k - begin + 1;
         else atomicMin(a.gt_arg + (size_t)s * a.N + c0 + k, j);

@@ -1,4 +1,4 @@
-// The pieces every detection head's training kernels share (anchor3d.cu, centerpoint.cu, voteseg.cu, cluster_head.cu).  The heads'
+// The pieces every detection head's training kernels share (anchor3d.cu, centerpoint.cu, voteseg.cu, cluster_head.cu, roi_head.cu).  The heads'
 // run-to-run determinism rests on two rules written once here: a loss is summed as per-block partials in double, then one block adds
 // them in a fixed order (thread0_block_sum, sum_partials); and every head forms its sigmoid and softplus from one exp(-|x|) (sig).
 #pragma once
@@ -75,6 +75,14 @@ __device__ __forceinline__ float sigmoid_focal(float x, bool t, float alpha, flo
 __device__ __forceinline__ float sigmoid_focal_grad(float x, bool t, float alpha, float gamma) {
   const Sig g = sig(x);
   return t ? -alpha * powf(g.q, gamma) * (gamma * g.s * g.sp_neg + g.q) : (1.f - alpha) * powf(g.s, gamma) * (gamma * g.q * g.sp_pos + g.s);
+}
+
+// The per-GT maximum IoU of the assigners (anchor3d.cu, roi_head.cu): folds one warp's IoUs into *slot (shared or global) as the
+// integer max of their fp32 bits.  IoU >= 0, so integer order is float order and the result does not depend on the order of the
+// writes.  Every lane of the warp calls it; a lane that does not take part passes 0.
+__device__ __forceinline__ void warp_max_iou(unsigned* slot, unsigned bits) {
+  const unsigned m = __reduce_max_sync(0xffffffffu, bits);
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(slot, m);
 }
 
 // torch.abs' gradient: sign(d), 0 at 0 and at NaN

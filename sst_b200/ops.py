@@ -23,6 +23,8 @@ and error behaviour; no CPU path - CPU tensors raise.
     cluster_head_targets, cluster_head_loss, multiclass_nms_groups
                                       models/dense_heads/sparse_cluster_head_v2.py (SparseClusterHeadV2 training and proposals),
                                       fsd_v2_head.py (FSDV2Head: centroid assignment, velocity)
+    roi_assign_sample, roi_head_targets, roi_head_loss
+                                      models/roi_heads/fsd_roi_head.py, bbox_heads/fsd_bbox_head.py (FSD's second stage)
 """
 import ctypes as C
 import math
@@ -1917,3 +1919,175 @@ def cluster_head_loss(cls_logits, reg_preds, labels, bbox_targets, num_pos, cls_
         raise L.SSTB200Error("cluster_head_loss: one cls_logits, reg_preds, labels and bbox_targets per task")
     return ClusterHeadLossFunction.apply(cfg, list(labels), list(bbox_targets), num_pos, cls_avg_factor, reg_avg_factor, *cls_logits,
                                          *reg_preds)
+
+
+# ----------------------------------------------------------------------------------------------
+# FSD's second stage: GroupCorrectionHead assignment / sampling, FullySparseBboxHead targets and losses
+# (mmdet3d/models/roi_heads/fsd_roi_head.py, bbox_heads/fsd_bbox_head.py, core/bbox/samplers/iou_neg_piecewise_sampler.py)
+# ----------------------------------------------------------------------------------------------
+class _RoiSampleCfg(C.Structure):
+    _fields_ = [("per_class", C.c_int32), ("num_classes", C.c_int32), ("pos_iou_thr", C.c_float * 8), ("neg_iou_thr", C.c_float * 8),
+                ("min_pos_iou", C.c_float * 8), ("num", C.c_int32), ("num_pos", C.c_int32), ("num_pieces", C.c_int32),
+                ("piece_fractions", C.c_double * 8), ("piece_thrs", C.c_float * 8)]
+
+
+class _RoiLossCfg(C.Structure):
+    _fields_ = [("smooth_l1", C.c_int32), ("beta", C.c_float), ("loss_weight_cls", C.c_float), ("loss_weight_bbox", C.c_float),
+                ("with_corner_loss", C.c_int32), ("corner_class", C.c_int32), ("corner_loss_weight", C.c_float),
+                ("code_weights", C.c_float * 7)]
+
+
+L.SIGNATURES["sstb200_roi_assign_sample"] = (C.c_int, [L.vp, C.POINTER(_RoiSampleCfg), L.vp, C.c_int, L.vp, L.vp, L.P_i32, L.vp, C.c_int,
+                                                        L.vp, L.P_i32, C.c_int, L.vp, L.vp, L.vp, L.vp, L.vp])
+L.SIGNATURES["sstb200_roi_head_targets"] = (C.c_int, [L.vp, L.vp, C.c_int, L.vp, L.vp, L.vp, C.c_int64, L.vp, C.c_int, C.c_int,
+                                                       C.POINTER(C.c_double), C.POINTER(C.c_double), L.vp, L.vp, L.vp, L.vp])
+_RL_ARGS = [L.vp, C.POINTER(_RoiLossCfg), L.vp, C.c_int64, L.vp, C.c_int64, L.vp, L.vp, L.vp, L.vp, L.vp, L.vp, L.vp, C.c_int, C.c_int64,
+            L.vp, L.vp]
+L.SIGNATURES["sstb200_roi_head_loss_forward"] = (C.c_int, _RL_ARGS + [L.vp, L.vp])
+L.SIGNATURES["sstb200_roi_head_loss_backward"] = (C.c_int, _RL_ARGS + [L.vp, L.vp, L.vp, L.vp])
+
+
+class RoiSampleConfig:
+    """The assigners (one per class, or one over every GT) and the IoUNegPiecewiseSampler of GroupCorrectionHead's train_cfg, built
+    once per head.  pos / neg / min_pos: one float per assigner."""
+
+    def __init__(self, pos_iou_thr, neg_iou_thr, min_pos_iou, per_class, num, pos_fraction, neg_piece_fractions, neg_iou_piece_thrs):
+        if not (len(pos_iou_thr) == len(neg_iou_thr) == len(min_pos_iou)) or not 1 <= len(pos_iou_thr) <= 8:
+            raise L.SSTB200Error(f"roi_assign_sample: 1 to 8 assigners, got {len(pos_iou_thr)}")
+        if len(neg_piece_fractions) != len(neg_iou_piece_thrs) or not 1 <= len(neg_piece_fractions) <= 8:
+            raise L.SSTB200Error("roi_assign_sample: 1 to 8 IoU pieces, one fraction per threshold")
+        self.per_class, self.num = bool(per_class), int(num)
+        self.num_pos = int(num * pos_fraction)  # IoUNegPiecewiseSampler.sample: int(self.num * self.pos_fraction)
+        s = _RoiSampleCfg()
+        s.per_class, s.num_classes = int(self.per_class), len(pos_iou_thr)
+        for k in range(len(pos_iou_thr)):
+            s.pos_iou_thr[k], s.neg_iou_thr[k], s.min_pos_iou[k] = float(pos_iou_thr[k]), float(neg_iou_thr[k]), float(min_pos_iou[k])
+        s.num, s.num_pos, s.num_pieces = self.num, self.num_pos, len(neg_piece_fractions)
+        for q in range(len(neg_piece_fractions)):
+            s.piece_fractions[q], s.piece_thrs[q] = float(neg_piece_fractions[q]), float(neg_iou_piece_thrs[q])
+        self.struct = s
+
+
+def roi_assign_sample(proposals, prop_labels, prop_sizes, keys, gt_boxes, gt_labels, gt_sizes, cfg):
+    """GroupCorrectionHead._assign_and_sample for every sample in one launch (sstb200_roi_assign_sample).  proposals fp32 [P, 7|9] and
+    prop_labels int64 [P] of the samples one after another (prop_sizes: host counts, each >= 1: the caller puts in the fake box), keys
+    fp32 [P] (one uniform draw per proposal: where the reference calls random_choice(gallery, k), the k members with the smallest keys
+    are kept, ties to the lower index), gt_boxes fp32 [G, 7|9|10] / gt_labels int64 [G] with host gt_sizes; cfg a RoiSampleConfig.
+    Returns (inds, iou, gt_rows, labels, num_pos): the sampled rows of every sample, positives by ascending proposal index then
+    negatives by ascending index, as int64 global proposal rows, fp32 max_overlaps, int64 global GT rows (-1 on negatives), int64 GT
+    labels (-1 on negatives); num_pos / num_rows host lists per sample.  One host sync, for the row counts."""
+    _need_cuda(proposals, prop_labels, keys, gt_boxes, gt_labels)
+    props = _fp32_cuda("proposals", proposals, 2)
+    gt = _fp32_cuda("gt_boxes", gt_boxes, 2)
+    dev = props.device
+    B = len(prop_sizes)
+    P = props.shape[0]
+    if keys.shape != (P,) or prop_labels.shape != (P,) or gt_labels.shape != (gt.shape[0],) or len(gt_sizes) != B:
+        raise L.SSTB200Error("roi_assign_sample: keys / labels do not match the boxes")
+    out_inds = torch.empty((B * cfg.num,), dtype=torch.int64, device=dev)
+    out_iou = torch.empty((B * cfg.num,), dtype=torch.float32, device=dev)
+    out_gt = torch.empty_like(out_inds)
+    out_lab = torch.empty_like(out_inds)
+    counts = torch.empty((B, 2), dtype=torch.int32, device=dev)
+    plab, gl = prop_labels.long().contiguous(), gt_labels.long().contiguous()
+    k = _fp32_cuda("keys", keys, 1)
+    c = L.ctx(dev)
+    L.check(c, L.lib().sstb200_roi_assign_sample(
+        c, C.byref(cfg.struct), props.data_ptr(), props.shape[1], plab.data_ptr(), k.data_ptr(), L.arr(C.c_int32, _offsets(prop_sizes)),
+        L.ptr(gt) if gt.numel() else None, gt.shape[1] if gt.shape[0] else 7, L.ptr(gl) if gl.numel() else None,
+        L.arr(C.c_int32, _offsets(gt_sizes)), B, out_inds.data_ptr(), out_iou.data_ptr(), out_gt.data_ptr(), out_lab.data_ptr(),
+        counts.data_ptr()))
+    cnt = counts.tolist()
+    num_pos, num_rows = [r[0] for r in cnt], [r[1] for r in cnt]
+    sl = [slice(b * cfg.num, b * cfg.num + num_rows[b]) for b in range(B)]
+    cat = lambda t: torch.cat([t[s] for s in sl])  # noqa: E731
+    return cat(out_inds), cat(out_iou), cat(out_gt), cat(out_lab), num_pos, num_rows
+
+
+def roi_head_targets(rois, iou, gt_rows, labels, gt_boxes, cls_pos_thr, cls_neg_thr):
+    """FullySparseBboxHead.get_targets for all R sampled rows in one launch (sstb200_roi_head_targets): rois fp32 [R, 7|9], the rows of
+    roi_assign_sample, gt_boxes fp32 [G, 7|9|10], one cls_pos_thr / cls_neg_thr per class.  Returns (soft labels fp32 [R], reg_mask int64
+    [R], bbox_targets fp32 [R, 7], pos_gt_bboxes fp32 [R, 7]); the last two are 0 on negatives.  No host sync."""
+    _need_cuda(rois, iou, gt_rows, labels, gt_boxes)
+    r = _fp32_cuda("rois", rois, 2)
+    gt = _fp32_cuda("gt_boxes", gt_boxes, 2)
+    R, dev = r.shape[0], r.device
+    soft = torch.empty((R,), dtype=torch.float32, device=dev)
+    reg_mask = torch.empty((R,), dtype=torch.int64, device=dev)
+    bt = torch.empty((R, 7), dtype=torch.float32, device=dev)
+    pg = torch.empty((R, 7), dtype=torch.float32, device=dev)
+    iou, gt_rows, labels = _fp32_cuda("iou", iou, 1), gt_rows.long().contiguous(), labels.long().contiguous()
+    c = L.ctx(dev)
+    L.check(c, L.lib().sstb200_roi_head_targets(
+        c, L.ptr(r) if R else None, r.shape[1], L.ptr(iou) if R else None, L.ptr(gt_rows) if R else None, L.ptr(labels) if R else None, R,
+        L.ptr(gt) if gt.numel() else None, gt.shape[1] if gt.shape[0] else 7, len(cls_pos_thr),
+        L.arr(C.c_double, [float(v) for v in cls_pos_thr]), L.arr(C.c_double, [float(v) for v in cls_neg_thr]), L.ptr(soft) if R else None,
+        L.ptr(reg_mask) if R else None, L.ptr(bt) if R else None, L.ptr(pg) if R else None))
+    return soft, reg_mask, bt, pg
+
+
+class RoiLossConfig:
+    """The constant part of FullySparseBboxHead.loss: loss_cls (sigmoid CrossEntropyLoss) and loss_bbox (L1 / SmoothL1) weights, the
+    corner loss and train_cfg's rcnn_code_weights.  corner_class: the class of corner_loss_only_car, -1 for every positive."""
+
+    def __init__(self, loss_weight_cls=1.0, loss_weight_bbox=1.0, smooth_l1=False, beta=1.0, with_corner_loss=False, corner_class=-1,
+                 corner_loss_weight=1.0, code_weights=None):
+        cw = [1.0] * 7 if code_weights is None else [float(v) for v in code_weights]
+        if len(cw) != 7:
+            raise L.SSTB200Error(f"roi_head_loss: 7 code weights, got {len(cw)}")
+        self.struct = _RoiLossCfg(int(bool(smooth_l1)), float(beta), float(loss_weight_cls), float(loss_weight_bbox),
+                                  int(bool(with_corner_loss)), int(corner_class), float(corner_loss_weight), (C.c_float * 7)(*cw))
+
+
+class RoiHeadLossFunction(Function):
+    """FullySparseBboxHead.loss in one launch sequence (sstb200_roi_head_loss_forward): returns losses fp32 [3] = (loss_rcnn_cls,
+    loss_rcnn_bbox, loss_rcnn_corner) carrying gradients to cls_score [R, 1] and bbox_pred [R, 7].  The backward writes each RoI's own
+    rows with no atomics (bit-identical from run to run).  No host sync."""
+
+    @staticmethod
+    def forward(ctx, cfg, nonempty, soft, reg_mask, bbox_targets, pos_gt, labels, rois, cls_avg, reg_avg, cls_score, bbox_pred):
+        x = _fp32_cuda("cls_score", cls_score, 2)
+        p = _fp32_cuda("bbox_pred", bbox_pred, 2)
+        R = x.shape[0]
+        if R < 1 or x.shape[1] != 1 or p.shape != (R, 7):
+            raise L.SSTB200Error(f"roi_head_loss: cls_score {tuple(x.shape)} and bbox_pred {tuple(p.shape)} must be [R, 1] and [R, 7]")
+        ins = (nonempty.to(torch.uint8).contiguous(), _fp32_cuda("labels", soft, 1), reg_mask.long().contiguous(),
+               _fp32_cuda("bbox_targets", bbox_targets, 2), _fp32_cuda("pos_gt_bboxes", pos_gt, 2), labels.long().contiguous(),
+               _fp32_cuda("rois", rois, 2), _fp32_cuda("cls_avg_factor", cls_avg.reshape(1), 1),
+               _fp32_cuda("reg_avg_factor", reg_avg.reshape(1), 1))
+        for k, t in enumerate(ins):
+            if t.shape[0] != (R if k < 7 else 1) or t.device != x.device:
+                raise L.SSTB200Error(f"roi_head_loss: an input of shape {tuple(t.shape)} on {t.device} does not fit {R} RoIs on {x.device}")
+        if ins[3].shape[1] != 7 or ins[4].shape[1] != 7 or ins[6].shape[1] not in (7, 9):
+            raise L.SSTB200Error("roi_head_loss: bbox_targets and pos_gt_bboxes must be [R, 7], rois [R, 7 | 9]")
+        losses = torch.empty((3,), dtype=torch.float32, device=x.device)
+        counts = torch.empty((2,), dtype=torch.float32, device=x.device)
+        c = L.ctx(x.device)
+        L.check(c, L.lib().sstb200_roi_head_loss_forward(c, C.byref(cfg.struct), x.data_ptr(), x.stride(0), p.data_ptr(), p.stride(0),
+                                                         *[t.data_ptr() for t in ins[:7]], ins[6].shape[1], R, ins[7].data_ptr(),
+                                                         ins[8].data_ptr(), losses.data_ptr(), counts.data_ptr()))
+        ctx.save_for_backward(x, p, counts, *ins)
+        ctx.cfg, ctx.dtypes = cfg, (cls_score.dtype, bbox_pred.dtype)
+        return losses
+
+    @staticmethod
+    def backward(ctx, grad_losses):
+        x, p, counts, *ins = ctx.saved_tensors
+        R = x.shape[0]
+        gx = torch.empty((R, 1), dtype=torch.float32, device=x.device)
+        gp = torch.empty((R, 7), dtype=torch.float32, device=x.device)
+        gl = grad_losses.float().contiguous()
+        c = L.ctx(x.device)
+        L.check(c, L.lib().sstb200_roi_head_loss_backward(c, C.byref(ctx.cfg.struct), x.data_ptr(), x.stride(0), p.data_ptr(), p.stride(0),
+                                                          *[t.data_ptr() for t in ins[:7]], ins[6].shape[1], R, ins[7].data_ptr(),
+                                                          ins[8].data_ptr(), counts.data_ptr(), gl.data_ptr(), gx.data_ptr(), gp.data_ptr()))
+        return (None,) * 10 + (gx.to(ctx.dtypes[0]), gp.to(ctx.dtypes[1]))
+
+
+def roi_head_loss(cls_score, bbox_pred, nonempty, soft_labels, reg_mask, bbox_targets, pos_gt_bboxes, labels, rois, cls_avg_factor,
+                  reg_avg_factor, cfg):
+    """losses fp32 [3] = (loss_rcnn_cls, loss_rcnn_bbox, loss_rcnn_corner) of RoiHeadLossFunction.  nonempty bool [R]; soft_labels,
+    reg_mask, bbox_targets, pos_gt_bboxes from roi_head_targets; labels int64 [R] the rows' GT labels; rois fp32 [R, 7|9] without the
+    batch column; cls_avg_factor / reg_avg_factor fp32 device scalars (see FullySparseBboxHead.loss for how the head forms them)."""
+    return RoiHeadLossFunction.apply(cfg, nonempty, soft_labels, reg_mask, bbox_targets, pos_gt_bboxes, labels, rois, cls_avg_factor,
+                                     reg_avg_factor, cls_score, bbox_pred)
