@@ -959,8 +959,11 @@ int sstb200_cluster_head_loss_backward_ex(sstb200_ctx* ctx, const sstb200_cluste
  *   Outputs: sample b's rows at [b * num, b * num + counts[2 b + 1]), positives (counts[2 b] of them) by ascending proposal index, then
  *   negatives by ascending index: out_inds (global proposal row), out_iou (max_overlaps), out_gt (global GT row, -1 on negatives),
  *   out_labels (the GT's label, -1 on negatives); counts int32 [batch, 2] on the device.  Temporaries from the context arena.
- *   Errors: a NULL pointer, a width other than the above, offsets that do not start at 0 or decrease, a sample without proposals
- *   (SSTB_ERR_ARG); more than 4096 proposals or GTs in a sample, more than 8 assigners or IoU pieces (SSTB_ERR_UNSUPPORTED).
+ *   With at most 3 pieces, fractions >= 0 and the non-last fractions summing to at most 1, a sample never gets more than num rows;
+ *   with 4 or more the reference's carry-over can ask a piece for more than num rows, so they are refused.
+ *   Errors: a NULL pointer, a width other than the above, offsets that do not start at 0 or decrease, a sample without proposals, a
+ *   negative piece fraction or non-last piece fractions summing past 1 (SSTB_ERR_ARG); more than 4096 proposals or GTs in a sample,
+ *   more than 8 assigners, more than 3 IoU pieces (SSTB_ERR_UNSUPPORTED).
  *
  * sstb200_roi_head_targets: FullySparseBboxHead.get_targets for all num_rows sampled rows in one launch.  rois [R, roi_width] the
  *   sampled proposals, iou / gt_rows / labels the rows of sstb200_roi_assign_sample (gt_rows index gt_boxes).  Outputs per row:
@@ -976,7 +979,9 @@ int sstb200_cluster_head_loss_backward_ex(sstb200_ctx* ctx, const sstb200_cluste
  *   - bbox: loss_weight_bbox * sum over positives on non-empty RoIs of L1 / SmoothL1(beta) times code_weights, over reg_avg_factor;
  *   - corner: corner_loss_weight * the mean over those positives (of class corner_class, or all with -1) and their 8 corners of the
  *     Huber (delta 1) distance from the prediction decoded against its RoI to the nearer of the GT's and the heading-flipped GT's.
- *   A term without rows is exactly 0.  counts fp32 [2] = (positives on non-empty RoIs, corner rows), for the backward.  Block partials
+ *   A term without rows is exactly 0.  counts fp32 [2] = (positives on non-empty RoIs, corner rows), for the backward.  Logits: a
+ *   NaN makes cls NaN and its own gradient NaN, no other; +inf gives cls inf (NaN on a soft label of 1, 0 * inf) and gradient
+ *   w (1 - y); -inf gives cls inf (NaN on a soft label of 0) and gradient -w y, w the row's upstream scale.  Block partials
  *   in double summed in a fixed order: deterministic.  Two launches, partials from the context arena.
  * sstb200_roi_head_loss_backward: grad_losses (device [3]) -> grad_cls [R] and grad_pred [R, 7], contiguous, each row writing only its
  *   own entries (no atomics).  One launch.

@@ -27,6 +27,32 @@ def iou3d(gt, props):
     return ov3 / (v(g)[:, None] + v(p)[None] - ov3).clamp(min=1e-8)
 
 
+def iou3d_fp32_axis(gt, props):
+    """The native kernel's fp32 3-D IoU of yaw-0 boxes whose BEV corners and overlap are exact in fp32 (coordinates dyadic with few
+    enough bits): [G, N] float32, bit for bit.  load_box3's x -/+ w / 2, the z range and the volume, then iou3d's overlap height, product,
+    union and quotient, each a correctly rounded fp32 operation in the kernel's order.  With yaw 0 the kernel's clipped polygon is the
+    intersection rectangle and its shoelace sum is exact, so the BEV overlap is the product of the two side overlaps."""
+    g, p = gt.float(), props.float()
+    assert bool((g[:, 6] == 0).all()) and bool((p[:, 6] == 0).all()), "yaw-0 boxes only"
+
+    def lo_hi(b, c, e):
+        h = b[:, e] / 2
+        return b[:, c] - h, b[:, c] + h
+
+    gx0, gx1 = lo_hi(g, 0, 3)
+    gy0, gy1 = lo_hi(g, 1, 4)
+    px0, px1 = lo_hi(p, 0, 3)
+    py0, py1 = lo_hi(p, 1, 4)
+    ox = (torch.min(gx1[:, None], px1[None]) - torch.max(gx0[:, None], px0[None])).clamp(min=0)
+    oy = (torch.min(gy1[:, None], py1[None]) - torch.max(gy0[:, None], py0[None])).clamp(min=0)
+    bev = ox * oy
+    bev = torch.where(((g[:, 3] * g[:, 4]) == 0)[:, None] | ((p[:, 3] * p[:, 4]) == 0)[None], torch.zeros_like(bev), bev)
+    oh = (torch.min((g[:, 2] + g[:, 5])[:, None], (p[:, 2] + p[:, 5])[None]) - torch.max(g[:, 2][:, None], p[:, 2][None])).clamp(min=0)
+    ov = bev * oh
+    v = lambda b: (b[:, 3] * b[:, 4]) * b[:, 5]  # noqa: E731
+    return ov / ((v(g)[:, None] + v(p)[None]) - ov).clamp(min=1e-8)
+
+
 def assign(overlaps, gt_labels, pos, neg, min_pos):
     """assign_wrt_overlaps with match_low_quality and gt_max_assign_all: (gt_inds 1-based / 0 / -1, max_overlaps, labels)"""
     G, N = overlaps.shape
@@ -82,8 +108,10 @@ def sample(gi, mo, keys, num, pos_fraction, fractions, thrs):
     return pos, neg.unique()
 
 
-def assign_and_sample(props, plabels, keys, gt, gl, assigners, per_class, num, pos_fraction, fractions, thrs):
-    """one sample -> (inds, iou, gt_rows (sample-local, -1 on negatives), labels, num_pos); assigners: (pos, neg, min_pos) per class"""
+def assign_and_sample(props, plabels, keys, gt, gl, assigners, per_class, num, pos_fraction, fractions, thrs, iou=iou3d):
+    """one sample -> (inds, iou, gt_rows (sample-local, -1 on negatives), labels, num_pos); assigners: (pos, neg, min_pos) per class.
+    iou(gt, props) -> [G, N] overlaps: the float64 iou3d, or iou3d_fp32_axis (with thresholds rounded to fp32, every compare is then the
+    kernel's fp32 compare)"""
     N = len(props)
     gi = torch.zeros(N, dtype=torch.int64)
     mo = torch.zeros(N, dtype=torch.float64)
@@ -91,11 +119,11 @@ def assign_and_sample(props, plabels, keys, gt, gl, assigners, per_class, num, p
     if per_class:
         for i, (p, n, m) in enumerate(assigners):
             gm, pm = gl == i, plabels == i
-            g_i, mo_i, l_i = assign(iou3d(gt[gm], props[pm]), gl[gm], p, n, m)
+            g_i, mo_i, l_i = assign(iou(gt[gm], props[pm]).double(), gl[gm], p, n, m)
             pad = torch.cat([torch.tensor([-1, 0]), torch.nonzero(gm).view(-1) + 1])
             gi[pm], mo[pm], lab[pm] = pad[g_i + 1], mo_i, l_i
     else:
-        gi, mo, lab = assign(iou3d(gt, props), gl, *assigners[0])
+        gi, mo, lab = assign(iou(gt, props).double(), gl, *assigners[0])
     pos, neg = sample(gi, mo, keys, num, pos_fraction, fractions, thrs)
     inds = torch.cat([pos, neg])
     rows = torch.cat([gi[pos] - 1, torch.full((len(neg),), -1, dtype=torch.int64)])
@@ -153,7 +181,9 @@ def decode(rois, pred):
 def losses(cls_score, bbox_pred, nonempty, soft, reg_mask, bbox_targets_rows, pos_gt_rows, labels_rows, rois, cfg):
     """FullySparseBboxHead.loss in float64 (torch autograd gives the gradient): dict of the three losses.  The *_rows tensors are
     row-aligned with the RoIs.  cfg: w_cls, w_bbox, smooth_l1, beta, code_weights, with_corner, corner_class, w_corner, cls_avg,
-    reg_avg (None: the positive count)"""
+    reg_avg (None: the positive count), exact_flip (the flipped GT's corners as the GT's reflected through its centre, equal to
+    yaw + pi in exact arithmetic and free of sin(pi)'s rounding, so that a corner on the bisector ties exactly; default False, the
+    reference's yaw + pi)"""
     x = cls_score.view(-1)
     y = soft.double()
     w = nonempty.double()
@@ -181,6 +211,8 @@ def losses(cls_score, bbox_pred, nonempty, soft, reg_mask, bbox_targets_rows, po
     gf = g.clone()
     gf[:, 6] += math.pi
     pc, gc, fc = corners(pb), corners(g), corners(gf)
+    if cfg.get('exact_flip'):
+        fc = torch.cat([2 * g[:, None, :2] - gc[..., :2], gc[..., 2:]], -1)
     dist = torch.min(torch.norm(pc - gc, dim=2), torch.norm(pc - fc, dim=2))
     q = dist.clamp(max=1.0)
     out['loss_rcnn_corner'] = cfg['w_corner'] * (0.5 * q ** 2 + (dist - q)).mean()

@@ -11,7 +11,7 @@
 //   write   positives by ascending proposal index, then negatives by ascending index (the reference's two `unique` calls)
 // The IoU is LiDARInstance3DBoxes.overlaps(gt, proposal): bev_overlap (bev_overlap.cuh, the kernel of boxes_overlap_bev) times the
 // overlap of [z, z + h], over max(v_gt + v_proposal - overlap, 1e-8), each step a correctly rounded fp32 operation as in torch.
-// It is recomputed per (proposal, GT) pair in both passes, never stored.
+// It is recomputed per (proposal, GT) pair in both passes, never stored, by one non-inlined function (iou3d_rows).
 //
 // Targets (rs_targets_kernel): one thread per sampled row: the soft label, the canonical transform and the encode in double, rounded once.
 // Losses: forward = block partials in double, one block sums them in a fixed order; backward = one pass, each row writes its own
@@ -24,7 +24,8 @@ namespace {
 
 #define RS_THREADS 512
 #define RS_MAX_CLASSES 8
-#define RS_MAX_PIECES 8
+#define RS_MAX_PIECES 8       // the config struct's capacity
+#define RS_MAX_USED_PIECES 3  // what the sampler accepts: more could write past a sample's rows (see sstb200_roi_assign_sample)
 #define RS_MAX_PROPOSALS 4096  // per sample
 #define RS_MAX_GT 4096         // per sample: the per-GT maxima live in shared memory
 
@@ -53,6 +54,13 @@ __device__ __forceinline__ float iou3d(const Box3& g, const Box3& p) {
   const float ov_h = fmaxf(__fsub_rn(fminf(g.zt, p.zt), fmaxf(g.zb, p.zb)), 0.f);
   const float ov = __fmul_rn(bev_overlap(g.bev, p.bev), ov_h);
   return __fdiv_rn(ov, fmaxf(__fsub_rn(__fadd_rn(g.vol, p.vol), ov), 1e-8f));
+}
+
+// The IoU of GT row g with proposal row p, as one compiled function: the max pass and the low-quality pass both call it, and the
+// low-quality pass compares its result with the per-GT maximum with ==.  Inlined into each pass, bev_overlap's unrounded products could
+// be contracted into FMAs differently in the two copies, and a GT's best proposal would then lose its low-quality match.
+__device__ __noinline__ float iou3d_rows(const float* __restrict__ g, const float* __restrict__ p) {
+  return iou3d(load_box3(g), load_box3(p));
 }
 
 struct RsArgs {
@@ -160,14 +168,13 @@ __global__ void __launch_bounds__(RS_THREADS) rs_assign_sample_kernel(const __gr
     const int i = base + threadIdx.x;
     const bool live = i < p1;
     const int c = live ? assigner_of(a, i) : -1;
-    Box3 p;
-    if (c >= 0) p = load_box3(a.props + (size_t)i * a.pw);
+    const float* p = a.props + (size_t)i * a.pw;
     float best = -1.f;
     int arg = -1;
     for (int g = g0; g < g1; g++) {
       float iou = 0.f;
       if (c >= 0 && sees(a, c, g)) {
-        iou = iou3d(load_box3(a.gt + (size_t)g * a.gw), p);
+        iou = iou3d_rows(a.gt + (size_t)g * a.gw, p);
         if (iou > best) best = iou, arg = g - g0;
       }
       warp_max_iou(gmax + (g - g0), __float_as_uint(iou));
@@ -186,12 +193,12 @@ __global__ void __launch_bounds__(RS_THREADS) rs_assign_sample_kernel(const __gr
     float mo = 0.f;  // no assigner, or no GT for it: negative with max_overlaps 0
     if (c >= 0 && arg >= 0) {
       mo = a.mo[i];
-      const Box3 p = load_box3(a.props + (size_t)i * a.pw);
+      const float* p = a.props + (size_t)i * a.pw;
       int lq = 0;
       for (int g = g0; g < g1; g++) {
         if (!sees(a, c, g)) continue;
         const float m = __uint_as_float(gmax[g - g0]);
-        if (m >= a.min_pos[c] && iou3d(load_box3(a.gt + (size_t)g * a.gw), p) == m) lq = g - g0 + 1;
+        if (m >= a.min_pos[c] && iou3d_rows(a.gt + (size_t)g * a.gw, p) == m) lq = g - g0 + 1;
       }
       gi = -1;
       if (mo >= 0.f && mo < a.neg_thr[c]) gi = 0;
@@ -344,28 +351,36 @@ __device__ __forceinline__ float reg_grad(const LsArgs& a, float d) {
 // get_corner_loss_lidar of one row: the prediction decoded against its RoI (decode, rotate by roi_yaw + pi / 2, shift), its corners
 // against the nearer of the GT's and the heading-flipped GT's, Huber (delta 1), summed over the 8 corners.  With grad != nullptr, also
 // d(sum) / d(bbox_pred row) into grad[7].  rotation_3d_in_axis(axis 2) maps (x, y) to (x cos + y sin, -x sin + y cos).
+// The corner positions are formed with explicitly rounded operations (no FMA contraction), the prediction's and the GT's by the same
+// sequence, so a prediction that decodes to the GT gives every corner distance exactly 0 and a gradient of exactly 0, and a corner on
+// the bisector of a GT corner and its flipped twin ties exactly (the flipped corners are the GT's reflected through its centre).
+__device__ __forceinline__ double rmul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double radd(double a, double b) { return __dadd_rn(a, b); }
+
 __device__ double corner_row_loss(const float* p, const float* roi, const float* gt, double* grad) {
   const double pw = roi[3], pl = roi[4], ph = roi[5], pr = roi[6];
   const double diag = sqrt(pl * pl + pw * pw);
   const double xl = p[0] * diag, yl = p[1] * diag;
   const double w = exp((double)p[3]) * pw, l = exp((double)p[4]) * pl, h = exp((double)p[5]) * ph;
-  const double zc = p[2] * ph + 0.5 * ph - 0.5 * h;
+  const double zc = radd(radd(rmul(p[2], ph), rmul(0.5, ph)), -rmul(0.5, h));
   const double yaw = (double)p[6] + pr;
   double sa, ca, sy, cy, sg, cg;
   sincos(pr + 0.5 * RS_PI, &sa, &ca);
   sincos(yaw, &sy, &cy);
   sincos((double)gt[6], &sg, &cg);
-  const double cx = xl * ca + yl * sa + roi[0], cyy = -xl * sa + yl * ca + roi[1], cz = zc + roi[2];
+  const double cx = radd(radd(rmul(xl, ca), rmul(yl, sa)), roi[0]), cyy = radd(radd(-rmul(xl, sa), rmul(yl, ca)), roi[1]);
+  const double cz = radd(zc, roi[2]);
   double gcx = 0, gcy = 0, gcz = 0, gyaw = 0, gw = 0, gl = 0, gh = 0, loss = 0;
   for (int k = 0; k < 8; k++) {
     // corners_norm[[0, 1, 3, 2, 4, 5, 7, 6]] - (0.5, 0.5, 0)
     const int bits = (k & 4) | ((k & 2) ? ((k & 1) ? 2 : 3) : (k & 1));
     const double ux = ((bits >> 2) & 1) - 0.5, uy = ((bits >> 1) & 1) - 0.5, uz = bits & 1;
     const double ox = ux * w, oy = uy * l, oz = uz * h;
-    const double X = ox * cy + oy * sy + cx, Y = -ox * sy + oy * cy + cyy, Z = oz + cz;
+    const double X = radd(radd(rmul(ox, cy), rmul(oy, sy)), cx), Y = radd(radd(-rmul(ox, sy), rmul(oy, cy)), cyy), Z = radd(oz, cz);
     const double gox = ux * gt[3], goy = uy * gt[4];
-    const double GX = gox * cg + goy * sg + gt[0], GY = -gox * sg + goy * cg + gt[1], GZ = uz * gt[5] + gt[2];
-    const double FX = -gox * cg - goy * sg + gt[0], FY = gox * sg - goy * cg + gt[1];  // yaw + pi
+    const double GA = radd(rmul(gox, cg), rmul(goy, sg)), GB = radd(-rmul(gox, sg), rmul(goy, cg));
+    const double GX = radd(GA, gt[0]), GY = radd(GB, gt[1]), GZ = radd(rmul(uz, gt[5]), gt[2]);
+    const double FX = radd(-GA, gt[0]), FY = radd(-GB, gt[1]);  // yaw + pi
     const double ex = X - GX, ey = Y - GY, ez = Z - GZ, fx = X - FX, fy = Y - FY;
     const double d1 = sqrt(ex * ex + ey * ey + ez * ez), d2 = sqrt(fx * fx + fy * fy + ez * ez);
     const double d = fmin(d1, d2);
@@ -509,8 +524,25 @@ extern "C" int sstb200_roi_assign_sample(sstb200_ctx* c, const sstb200_roi_sampl
   CHECK_ARG(c, proposals && prop_labels && keys && (G == 0 || (gt_boxes && gt_labels)));
   const int K = cfg->per_class ? cfg->num_classes : 1;
   if (K < 1 || K > RS_MAX_CLASSES) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "roi_assign_sample: %d assigners, 1 to %d supported", K, RS_MAX_CLASSES);
-  if (cfg->num_pieces < 1 || cfg->num_pieces > RS_MAX_PIECES)
-    return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "roi_assign_sample: %d IoU pieces, 1 to %d supported", cfg->num_pieces, RS_MAX_PIECES);
+  // Sample b owns rows [b num, (b + 1) num), so the sampler must never pick more than num rows.  The reference's carry-over
+  // (extend += want - n, where want already holds extend) doubles what an empty piece passes on, and with four pieces a non-last
+  // piece can then be asked for more than nexp rows (fractions 0.3 / 0.3 / 0.3 / 0.1 with pieces 0 and 1 empty ask piece 2 for
+  // 0.3 nexp + 0.6 nexp + 0.3 nexp).  With at most three pieces, fractions >= 0 and a non-last sum <= 1 it cannot: piece 0 takes
+  // chosen <= want0 = int(nexp f0); piece 1 asks for want1 = int(nexp f1) + (want0 - chosen) and takes at most that, so after it
+  // chosen <= want0 + int(nexp f1) <= nexp (f0 + f1) <= nexp; the last piece takes at most nexp - chosen.  So rows <= npos_sel + nexp
+  // = num.
+  if (cfg->num_pieces < 1 || cfg->num_pieces > RS_MAX_USED_PIECES)
+    return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "roi_assign_sample: %d IoU pieces, 1 to %d supported", cfg->num_pieces,
+                     RS_MAX_USED_PIECES);
+  double head = 0.0;
+  for (int q = 0; q < cfg->num_pieces; q++) {
+    if (!(cfg->piece_fractions[q] >= 0.0))
+      return sstb_fail(c, SSTB_ERR_ARG, "roi_assign_sample: IoU piece %d has fraction %g, must be >= 0", q, cfg->piece_fractions[q]);
+    if (q < cfg->num_pieces - 1) head += cfg->piece_fractions[q];
+  }
+  if (head > 1.0)
+    return sstb_fail(c, SSTB_ERR_ARG, "roi_assign_sample: the IoU pieces before the last take fractions summing to %g, more than 1",
+                     head);
   CHECK_ARG(c, cfg->num >= 1 && cfg->num_pos >= 0 && cfg->num_pos <= cfg->num);
   RsArgs a;
   a.props = proposals, a.plab = prop_labels, a.keys = keys, a.gt = gt_boxes, a.glab = gt_labels;

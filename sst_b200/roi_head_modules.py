@@ -318,8 +318,13 @@ class GroupCorrectionHead(nn.Module):
         if not s.get('return_iou', False):
             _refuse("the sampler must have return_iou=True (get_targets reads the IoU)", name)
         fr, th = list(s['neg_piece_fractions']), list(s['neg_iou_piece_thrs'])
-        if sum(fr[:-1]) > 1 or any(th[i] < th[i + 1] for i in range(len(th) - 1)):
-            _refuse(f"neg_piece_fractions must sum to at most 1 and neg_iou_piece_thrs descend, got {fr} and {th}", name)
+        # With at most 3 pieces, fractions >= 0 and sum(fr[:-1]) <= 1, the reference's carry-over never asks for more than the
+        # sample's num rows (the proof is at sstb200_roi_assign_sample); with 4 it can, and the native sampler refuses them.
+        if not 1 <= len(fr) <= 3:
+            _refuse(f"1 to 3 IoU pieces are supported, got {len(fr)}", name)
+        if any(f < 0 for f in fr) or sum(fr[:-1]) > 1 or any(th[i] < th[i + 1] for i in range(len(th) - 1)):
+            _refuse(f"neg_piece_fractions must be >= 0 and sum to at most 1 before the last, and neg_iou_piece_thrs descend, got {fr} "
+                    f"and {th}", name)
         if cfg.get('class_wise_cls_weights') is not None or cfg.get('class_wise_box_weights') is not None:
             _refuse("class_wise_cls_weights / class_wise_box_weights are not supported", name)
         return ops.RoiSampleConfig([a['pos_iou_thr'] for a in assigners], [a['neg_iou_thr'] for a in assigners],

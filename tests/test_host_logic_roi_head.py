@@ -51,3 +51,58 @@ def test_fsd_head_builds_with_reference_keys():
 def test_refusals(kw):
     with pytest.raises(ValueError):
         _build(**kw)
+
+
+def _rows(n_neg, num, fractions, thrs, seed, npos=0):
+    """the oracle sampler's row count for one sample: npos positives and n_neg negatives with IoUs drawn over [0, 0.6)"""
+    import torch
+    from oracle import roi_head_oracle as RO
+    g = torch.Generator().manual_seed(seed)
+    gi = torch.cat([torch.ones(npos, dtype=torch.int64), torch.zeros(n_neg, dtype=torch.int64)])
+    mo = torch.cat([torch.full((npos,), 0.9, dtype=torch.float64), torch.rand(n_neg, generator=g, dtype=torch.float64) * 0.6])
+    # quantised IoUs leave some pieces empty, so the carry-over runs
+    mo = torch.where(torch.rand(len(mo), generator=g) < 0.5, (mo * 4).floor() / 4, mo)
+    p, n = RO.sample(gi, mo, torch.rand(len(gi), generator=g), num, 0.5, fractions, thrs)
+    return len(p) + len(n)
+
+
+def test_oracle_sampler_never_exceeds_num_with_three_pieces():
+    """with 1 to 3 pieces, fractions >= 0 and a non-last sum <= 1, the reference's carry-over keeps every sample within num rows (the
+    bound the native sampler's output layout relies on)"""
+    import random
+    rng = random.Random(0)
+    for t in range(300):
+        k = rng.choice([1, 2, 3])
+        head = [rng.random() for _ in range(k - 1)]
+        if sum(head) > 1:
+            head = [h / sum(head) for h in head]
+        fr = head + [rng.random()]
+        thrs = sorted((rng.random() * 0.6 for _ in range(k)), reverse=True)
+        num = rng.choice([1, 7, 64, 100, 256])
+        rows = _rows(rng.choice([0, 5, 150, 600]), num, fr, thrs, t, npos=rng.choice([0, 3, 40]))
+        assert rows <= num, (fr, thrs, num, rows)
+
+
+def test_oracle_sampler_exceeds_num_with_four_pieces():
+    """the example the refusal guards against: pieces 0 and 1 empty, the carry-over doubles and piece 2 is asked for 120 of 100 rows"""
+    import torch
+    from oracle import roi_head_oracle as RO
+    N = 200
+    p, n = RO.sample(torch.zeros(N, dtype=torch.int64), torch.full((N,), 0.25, dtype=torch.float64), torch.rand(N), 100, 0.55,
+                     [0.3, 0.3, 0.3, 0.1], [0.55, 0.45, 0.3, 0.1])
+    assert len(p) + len(n) == 120
+
+
+@pytest.mark.parametrize("fr,th", [
+    ([0.3, 0.3, 0.3, 0.1], [0.55, 0.45, 0.3, 0.1]),     # four pieces
+    ([0.5, -0.1, 0.6], [0.55, 0.3, 0.1]),               # a negative fraction
+    ([0.7, 0.4, 0.1], [0.55, 0.3, 0.1]),                # non-last fractions summing past 1
+])
+def test_refuses_piece_settings_that_could_overflow(fr, th):
+    with pytest.raises(ValueError):
+        _build(sampler=dict(neg_piece_fractions=fr, neg_iou_piece_thrs=th))
+
+
+@pytest.mark.parametrize("fr,th", [([1.0], [0.55]), ([0.8, 0.2], [0.55, 0.1]), ([0.5, 0.5, 0.2], [0.55, 0.3, 0.1])])
+def test_accepts_one_to_three_pieces(fr, th):
+    assert _build(sampler=dict(neg_piece_fractions=fr, neg_iou_piece_thrs=th)).sample_cfg.struct.num_pieces == len(fr)

@@ -144,3 +144,61 @@ def _unshare(x):
     if isinstance(x, (list, tuple)):
         return type(x)(_unshare(v) for v in x)
     return x
+
+
+# settings no config uses but the native sampler accepts, each pinned here so that the GPU edge tests may use the oracle for them:
+# (assigners (pos, neg, min_pos) per class, fractions, thresholds, pos_fraction)
+SETTINGS = {
+    "ignore_band": ([(0.6, 0.3, 0.6), (0.5, 0.2, 0.5), (0.5, 0.25, 0.5)], [0.8, 0.2], [0.55, 0.1], 0.55),
+    "min_pos_below_pos": ([(0.7, 0.7, 0.2), (0.6, 0.6, 0.1), (0.6, 0.4, 0.3)], [0.8, 0.2], [0.55, 0.1], 0.55),
+    "min_pos_zero": ([(0.45, 0.45, 0.0), (0.35, 0.35, 0.0), (0.35, 0.35, 0.0)], [0.8, 0.2], [0.55, 0.1], 0.55),
+    "one_piece": ([(0.45, 0.45, 0.45), (0.35, 0.35, 0.35), (0.35, 0.35, 0.35)], [1.0], [0.55], 0.3),
+    "three_pieces": ([(0.45, 0.45, 0.45), (0.35, 0.35, 0.35), (0.35, 0.35, 0.35)], [0.5, 0.3, 0.2], [0.55, 0.3, 0.05], 0.25),
+    "pos_fraction_0": ([(0.45, 0.45, 0.45), (0.35, 0.35, 0.35), (0.35, 0.35, 0.35)], [0.8, 0.2], [0.55, 0.1], 0.0),
+    "pos_fraction_1": ([(0.45, 0.45, 0.45), (0.35, 0.35, 0.35), (0.35, 0.35, 0.35)], [0.8, 0.2], [0.55, 0.1], 1.0),
+}
+
+
+def _settings_batch(assigners, thrs, per_class, seed, duplicates):
+    """four samples as MG.batch draws them, kept 1e-4 away from every threshold of the setting; with duplicates, GT and proposal rows
+    repeated so that the argmax, the low-quality match and gt_max_assign_all meet exact ties"""
+    t = sorted({v for a in assigners for v in a} | set(thrs))
+    out = []
+    for b, (n, g) in enumerate([(300, 60), (120, 40), (200, 50), (80, 0)]):
+        s = seed * 100 + b
+        while True:
+            p, l, gt, gl = RO.synth_sample(s, n, g)
+            if duplicates and g:
+                gt, gl = torch.cat([gt, gt[:g // 3]]), torch.cat([gl, gl[:g // 3]])
+                p, l = torch.cat([p, p[: n // 4]]), torch.cat([l, l[: n // 4]])
+            if not RO.near_threshold(p, l, gt, gl, [v for v in t if v > 0], per_class=per_class):
+                break
+            s += 1000
+        out.append((p, l, gt, gl))
+    return out
+
+
+@pytest.mark.parametrize("per_class", [True, False])
+@pytest.mark.parametrize("setting", list(SETTINGS) + ["duplicates"])
+def test_assign_and_sample_settings_match_reference(setting, per_class):
+    N = RR.load_roi_head()
+    assigners, fr, th, pf = SETTINGS.get(setting, SETTINGS["min_pos_below_pos"])
+    if not per_class:
+        assigners = assigners[:1]
+    num = 96
+    a = [dict(type='MaxIoUAssigner', iou_calculator=dict(type='BboxOverlaps3D', coordinate='lidar'), pos_iou_thr=p, neg_iou_thr=n,
+              min_pos_iou=m, ignore_iof_thr=-1) for p, n, m in assigners]
+    cfg = dict(MG.train_cfg(per_class=per_class, num=num), assigner=a if per_class else a[0],
+               sampler=dict(type='IoUNegPiecewiseSampler', num=num, pos_fraction=pf, neg_piece_fractions=fr, neg_iou_piece_thrs=th,
+                            neg_pos_ub=-1, add_gt_as_proposals=False, return_iou=True))
+    batch = _settings_batch(assigners, th, per_class, 5 + len(setting), setting == "duplicates")
+    keys = [torch.rand(len(p), generator=torch.Generator().manual_seed(20 + b), dtype=torch.float64) for b, (p, _, _, _) in enumerate(batch)]
+    props = [(N.Boxes(p.double()), torch.rand(len(p)), l) for p, l, _, _ in batch]
+    res = N.assign_and_sample(cfg, props, [N.Boxes(g.double()) for _, _, g, _ in batch], [l for _, _, _, l in batch], keys)
+    for b, ((p, l, g, gl), r) in enumerate(zip(batch, res)):
+        inds, iou, rows, lab, npos = RO.assign_and_sample(p, l, keys[b], g, gl, assigners, per_class, num, pf, fr, th)
+        assert torch.equal(inds, torch.cat([r.pos_inds, r.neg_inds])), b
+        assert npos == len(r.pos_inds) and len(inds) <= num
+        assert torch.equal(rows[:npos], r.pos_assigned_gt_inds)
+        assert torch.equal(lab[:npos], r.pos_gt_labels)
+        assert torch.equal(iou, r.iou)
