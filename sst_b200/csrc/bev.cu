@@ -2,7 +2,9 @@
 // The reference zero-fills one canvas per sample and index_puts the transposed rows; here ONE pass writes every output byte
 // exactly once (HBM-write bound: B*C*ny*nx*4 bytes): a cell -> row map (4 bytes per cell) is filled first, then each block
 // transposes the rows of 128 consecutive x cells, 32 channels at a time, through shared memory so that the canvas is written
-// as 512-byte warp stores (float4 per lane, streaming); all-empty blocks only stream zeros.
+// as 512-byte warp stores (float4 per lane, streaming); all-empty blocks only stream zeros.  The float4 path needs every canvas
+// row to start 16-byte aligned: nx % 4 == 0 and a 16-byte-aligned canvas, which the host checks (a contiguous view of a larger
+// buffer may start at any 4-byte offset); otherwise the same tiles leave through scalar stores.
 #include <stdarg.h>
 #include "common.cuh"
 
@@ -24,7 +26,7 @@ __global__ void bev_map_kernel(const long long* __restrict__ coors, int M, int B
 #define BEV_CC 32    // channels per pass
 #define BEV_PITCH 132  // floats; == 4 (mod 32): 16-byte row reads by 32 lanes are conflict-free
 __global__ void __launch_bounds__(256) bev_fill_kernel(const float* __restrict__ feat, int C, const int32_t* __restrict__ cell_map, int ny,
-                                                       int nx, float* __restrict__ out) {
+                                                       int nx, int vec4, float* __restrict__ out) {
   pdl_wait();
   pdl_launch();
   __shared__ __align__(16) float tile[BEV_CC][BEV_PITCH];  // [channel][cell]
@@ -45,8 +47,7 @@ __global__ void __launch_bounds__(256) bev_fill_kernel(const float* __restrict__
   const int cell = threadIdx.x & (BEV_X - 1), chalf = threadIdx.x >> 7;  // phase A: thread = (cell, half of the channel pass)
   const int myrow = sRow[cell];
   const int x = x0 + lane * 4;
-  const size_t cstride = (size_t)ny * nx;
-  const bool vec = ((nx & 3) == 0) && x + 3 < nx;
+  const bool vec = vec4 && x + 3 < nx;
   for (int c0 = 0; c0 < C; c0 += BEV_CC) {
     if (some) {
       __syncthreads();  // previous pass read out
@@ -73,6 +74,9 @@ __global__ void __launch_bounds__(256) bev_fill_kernel(const float* __restrict__
   }
 }
 
+// float4 rows: every (b, c, y) row of a [B, C, ny, nx] canvas starts 16-byte aligned
+static inline int bev_vec4(const float* canvas, int nx) { return (nx & 3) == 0 && ((uintptr_t)canvas & 15) == 0; }
+
 extern "C" int sstb200_recover_bev(sstb200_ctx* c, const float* voxel_feat, const int64_t* coors, int M, int C, int B, int ny, int nx,
                                    float* canvas) {
   CHECK_ARG(c, c && M >= 0 && C >= 1 && C <= 1024 && B >= 1 && ny >= 1 && nx >= 1 && canvas);
@@ -89,7 +93,7 @@ extern "C" int sstb200_recover_bev(sstb200_ctx* c, const float* voxel_feat, cons
   if (M > 0)
     launch_pdl(bev_map_kernel, dim3((M + 255) / 256), dim3(256), (size_t)0, c->stream, (const long long*)coors, M, B, ny, nx, cell_map, err);
   launch_pdl(bev_fill_kernel, dim3((nx + BEV_X - 1) / BEV_X, ny, B), dim3(256), (size_t)0, c->stream, voxel_feat, C, (const int32_t*)cell_map, ny, nx,
-             canvas);
+             bev_vec4(canvas, nx), canvas);
   LAUNCH_CHECK(c);
   CUDA_TRY(c, cudaMemcpyAsync(c->pinned_i32, err, 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
@@ -102,7 +106,7 @@ extern "C" int sstb200_recover_bev(sstb200_ctx* c, const float* voxel_feat, cons
 // 512-byte warp loads, transposes them through shared memory and stores each voxel's channels as one contiguous run of its row.
 // Blocks without a voxel read nothing, so the traffic is the occupied (b, y, 128-x) segments plus the M x C rows.
 __global__ void __launch_bounds__(256) bev_gather_kernel(const float* __restrict__ grad, int C, const int32_t* __restrict__ cell_map, int ny,
-                                                         int nx, float* __restrict__ grad_feat) {
+                                                         int nx, int vec4, float* __restrict__ grad_feat) {
   pdl_wait();
   pdl_launch();
   __shared__ __align__(16) float tile[BEV_CC][BEV_PITCH];  // [channel][cell]
@@ -124,7 +128,7 @@ __global__ void __launch_bounds__(256) bev_gather_kernel(const float* __restrict
   const int myrow = sRow[cell];
   const int x = x0 + lane * 4;
   const size_t cstride = (size_t)ny * nx;
-  const bool vec = ((nx & 3) == 0) && x + 3 < nx;
+  const bool vec = vec4 && x + 3 < nx;
   for (int c0 = 0; c0 < C; c0 += BEV_CC) {
     __syncthreads();  // previous pass read out
     for (int c = warp; c < BEV_CC; c += 8) {
@@ -190,7 +194,7 @@ extern "C" int sstb200_recover_bev_backward(sstb200_ctx* c, const float* grad_ca
   CUDA_TRY(c, cudaMemsetAsync(cell_map, 0xFF, cells * 4, c->stream));
   launch_pdl(bev_map_kernel, dim3((M + 255) / 256), dim3(256), (size_t)0, c->stream, (const long long*)coors, M, B, ny, nx, cell_map, err);
   launch_pdl(bev_gather_kernel, dim3((nx + BEV_X - 1) / BEV_X, ny, B), dim3(256), (size_t)0, c->stream, grad_canvas, C, (const int32_t*)cell_map,
-             ny, nx, grad_feat);
+             ny, nx, bev_vec4(grad_canvas, nx), grad_feat);
   launch_pdl(bev_dup_kernel, dim3((unsigned)(((size_t)M * 32 + 255) / 256)), dim3(256), (size_t)0, c->stream, (const long long*)coors, M, C, B,
              ny, nx, (const int32_t*)cell_map, grad_feat);
   LAUNCH_CHECK(c);

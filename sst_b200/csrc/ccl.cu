@@ -7,19 +7,26 @@
 // union-find whose roots are always the SMALLEST index of their tree (hook the larger root under the smaller with atomicMin), and the
 // labels are the rank of (batch, root) - exactly scipy's numbering (components numbered by their first node, samples in order).
 // Adjacency is evaluated with the reference's fp32 arithmetic: sqrt(dx*dx + dy*dy) < dist, round-to-nearest at every step.
+//
+// The cell is dist * 1.01, and the binning must keep any two centres whose fp32 distance is below dist at most one cell apart.
+// An fp32 distance below dist bounds the exact one by dist (1 + 2^-22), so the exact coordinate difference is under 0.991 cells
+// and the binning may err by at most the remaining 0.009 cell.  In fp32, (v - x0) * inv_cell errs by about 2^-23 of the cell
+// index, which exceeds that slack once an axis has more than ~2.5e5 cells (dist 6e-4 over 160 m puts two centres 5.95e-4 apart
+// in cells 257258 and 257260).  So the binning runs in double: floor(((double)v - x0) / cell) with x0 and cell held in double
+// errs by ~2^-52 of the cell index, under 1e-9 cell at the 1e6 cells per axis the call accepts.
 #include <stdarg.h>
 #include "index.cuh"
 
 namespace {
 
 struct CclGrid {
-  float x0, y0, inv_cell;
+  double x0, y0, cell;
   int nx, ny, B;
 };
 
-__device__ __forceinline__ int ccl_cell(float v, float v0, float inv_cell, int n) {
-  const float f = floorf((v - v0) * inv_cell);
-  return f < 0.f ? 0 : (f >= (float)n ? n - 1 : (int)f);   // also sends NaN to cell 0
+__device__ __forceinline__ int ccl_cell(float v, double v0, double cell, int n) {
+  const double f = floor(((double)v - v0) / cell);
+  return !(f >= 0.0) ? 0 : (f >= (double)n ? n - 1 : (int)f);   // also sends NaN to cell 0, +-inf to the border cells
 }
 
 __global__ void ccl_rows_kernel(const float* __restrict__ centers, int stride, const int32_t* __restrict__ batch_idx, int n, CclGrid g,
@@ -29,8 +36,8 @@ __global__ void ccl_rows_kernel(const float* __restrict__ centers, int stride, c
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   rows[3 * i + 0] = batch_idx ? batch_idx[i] : 0;
-  rows[3 * i + 1] = ccl_cell(centers[(size_t)i * stride + 0], g.x0, g.inv_cell, g.nx);
-  rows[3 * i + 2] = ccl_cell(centers[(size_t)i * stride + 1], g.y0, g.inv_cell, g.ny);
+  rows[3 * i + 1] = ccl_cell(centers[(size_t)i * stride + 0], g.x0, g.cell, g.nx);
+  rows[3 * i + 2] = ccl_cell(centers[(size_t)i * stride + 1], g.y0, g.cell, g.ny);
   parent[i] = i;
 }
 
@@ -122,11 +129,12 @@ extern "C" int sstb200_connected_components(sstb200_ctx* c, const float* centers
   }
   CHECK_ARG(c, centers && labels && xy_max[0] >= xy_min[0] && xy_max[1] >= xy_min[1]);
   CclGrid g;
-  const float cell = dist * 1.01f;   // > dist by far more than the fp32 rounding of the binning: neighbours are at most one cell apart
+  const double cell = (double)dist * 1.01;   // > dist by far more than the rounding of the fp64 binning (see the top of the file)
   g.x0 = xy_min[0];
   g.y0 = xy_min[1];
-  g.inv_cell = 1.0f / cell;
-  const double ex = ((double)xy_max[0] - xy_min[0]) / cell, ey = ((double)xy_max[1] - xy_min[1]) / cell;
+  g.cell = cell;
+  // the kernel's own expression at xy_max: an in-range centre never bins past cell n - 1
+  const double ex = ((double)xy_max[0] - g.x0) / cell, ey = ((double)xy_max[1] - g.y0) / cell;
   if (ex > 1e6 || ey > 1e6) return sstb_fail(c, SSTB_ERR_UNSUPPORTED, "connected_components: xy range / dist too large (%g x %g cells)", ex, ey);
   g.nx = (int)ex + 1;
   g.ny = (int)ey + 1;

@@ -33,7 +33,14 @@ def connected_components(points, batch_idx, dist, batch_size=None, xy_bounds=Non
     if batch_size is None:
         batch_size = 1 if bi is None else int(bi.max().item()) + 1
     if xy_bounds is None:
-        lo, hi = pts[:, :2].amin(0).tolist(), pts[:, :2].amax(0).tolist()
+        # the grid spans the finite coordinates only: a NaN or infinite centre connects to nothing (every distance test fails), so it
+        # is a singleton in whichever border cell it lands; an axis with no finite coordinate takes any bounds
+        xy = pts[:, :2]
+        fin = torch.isfinite(xy)
+        lo = torch.where(fin, xy, float("inf")).amin(0)
+        hi = torch.where(fin, xy, float("-inf")).amax(0)
+        none = ~fin.any(0)
+        lo, hi = torch.stack([lo.masked_fill(none, 0.0), hi.masked_fill(none, 0.0)]).tolist()
     else:
         lo, hi = xy_bounds
     num_dev = torch.empty((1,), dtype=torch.int32, device=pts.device)
