@@ -559,7 +559,8 @@ int sstb200_nms_bev(sstb200_ctx* ctx, const float* boxes, int num, const int32_t
  * sstb200_points_in_boxes: pts [batch, num_pts, 3], boxes [batch, num_boxes, 7] (sample b's points against sample b's boxes).
  * mode SSTB200_PIB_FIRST (points_in_boxes_gpu): out int32 [batch, num_pts] = the LOWEST box index containing the point, else -1.
  * mode SSTB200_PIB_ALL (points_in_boxes_batch): out int32 [batch, num_pts, num_boxes] = 1 inside, else 0.
- * Every entry is written (no fill needed); zero-size boxes contain nothing.  No atomics, no sync.  Errors: negative sizes or an unknown
+ * Every entry is written (no fill needed); zero-size boxes contain nothing.  out needs only int32 alignment (ALL mode aligns its 16-byte
+ * stores to the address).  No atomics, no sync.  Errors: negative sizes or an unknown
  * mode (SSTB_ERR_ARG); more than 786432 boxes per sample in ALL mode (SSTB_ERR_UNSUPPORTED). */
 #define SSTB200_PIB_FIRST 0
 #define SSTB200_PIB_ALL 1

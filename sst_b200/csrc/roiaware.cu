@@ -95,10 +95,12 @@ __global__ void __launch_bounds__(PIB_THREADS) pib_all_kernel(const float* __res
     }
   }
   __syncthreads();
-  // the tile's output is the contiguous range [base, base + rows * T): scalar head up to 16-byte alignment, int4 body, scalar tail
+  // the tile's output is the contiguous range [base, base + rows * T): scalar head up to 16-byte alignment, int4 body, scalar tail.
+  // The head comes from the address, not from base: the caller's `out` need only be 4-byte aligned, and an `out` 4, 8 or 12 bytes past
+  // a 16-byte boundary would otherwise put every int4 store off its alignment.
   const size_t base = ((size_t)b * M + row0) * (size_t)T;
   const long long E = (long long)rows * T;
-  const long long head = min((long long)((4 - (base & 3)) & 3), E);
+  const long long head = min((long long)((4 - ((reinterpret_cast<uintptr_t>(out + base) >> 2) & 3)) & 3), E);
   auto bit = [&](int r, int col) -> int { return (int)((bits[r * W + (col >> 5)] >> (col & 31)) & 1u); };
   for (long long e = threadIdx.x; e < head; e += blockDim.x) out[base + e] = bit((int)(e / T), (int)(e % T));
   const long long nvec = (E - head) >> 2;
